@@ -347,8 +347,10 @@ class SphkOps:
         total, it = 3.4e38, 0        # correctDivergenceError :331-363
         while (it < 1 or total > self.div_thr * n * rho0) and it < self.max_iter:
             self._run(self.dfsph_div_correct, "vel")
-            self._run(self.dfsph_div_error, "scalar", self.kappa)
             it += 1
+            if it == self.max_iter:  # the loop ends whatever the error is, and nothing reads it again: dead sweep
+                break
+            self._run(self.dfsph_div_error, "scalar", self.kappa)
             if self.div_thr >= 0:    # negative threshold: the test cannot depend on the sum (Q11) -> no host sync
                 total = self.reduce_sum(self.reduce_abs_sum(self.owned(self.error)))
         self.it_div = it

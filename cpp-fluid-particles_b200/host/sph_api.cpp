@@ -239,10 +239,14 @@ int DFSPHSolver::correctDivergenceError(float rho0, float dt, float errorThresho
     while ((iter < 1 || totalError > errorThreshold * thresholdCount * rho0) && iter < maxIter_) {
         check(sphk_dfsph_div_correct(ctx, &current_.abi, bufferFloat.addr()), "sphk_dfsph_div_correct");
         produced(1, current_.abi.fluid.vel, 3);
+        ++iter;
+        // After the last permitted iteration the loop ends whatever the error is, and nothing reads this error, stiffness or
+        // record scalar again: the density solve forms its own before it reads them.  The reference's final error sweep
+        // (DFSPHSolver.cu:354) is dead work -- one of the 20 list sweeps of a fixed 4+4 step.
+        if (iter == maxIter_) break;
         check(sphk_dfsph_div_error(ctx, &current_.abi, alpha.addr(), error.addr(), bufferFloat.addr(), dt, rho0),
               "sphk_dfsph_div_error");
         produced(2, bufferFloat.addr(), 1);
-        ++iter;
         if (errorThreshold >= 0.0f) totalError = reduceError(num);
     }
     return iter;
