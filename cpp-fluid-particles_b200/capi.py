@@ -24,7 +24,7 @@ SPHK_FUNCTIONS = [
     "sphk_pressure_force", "sphk_advect", "sphk_dfsph_density_alpha", "sphk_dfsph_div_error", "sphk_dfsph_div_correct",
     "sphk_dfsph_den_error", "sphk_dfsph_den_correct", "sphk_reduce_abs_sum", "sphk_copy", "sphk_pbd_density_lambda",
     "sphk_pbd_delta_pos_apply", "sphk_pbd_velocity_from_positions", "sphk_pbd_xsph", "sphk_get_permutation",
-    "sphk_list_stats", "sphk_get_skin_displacement", "sphk_set_active_range", "sphk_push_range", "sphk_build_neighbor_list", "sphk_get_neighbor_list", "sphk_fused_density_color_grad",
+    "sphk_list_stats", "sphk_get_skin_displacement", "sphk_set_active_range", "sphk_push_range", "sphk_build_neighbor_list", "sphk_get_neighbor_list", "sphk_get_tile_lists", "sphk_fused_density_color_grad",
     "sphk_fused_dfsph_density_alpha_color_grad", "sphk_fused_dfsph_density_alpha_div_error", "sphk_fused_pbd_xsph_color_grad", "sphk_scene_fluid_block", "sphk_scene_boundary_count", "sphk_scene_boundary_shell", "sphk_loop_begin", "sphk_loop_next", "sphk_loop_end", "sphk_loop_iterations", "sphk_fused_viscosity_surface", "sphk_export_dots", "sphk_particles_advect", "sphk_add_launches",
     "sphk_mg_unique_id", "sphk_mg_init", "sphk_mg_destroy", "sphk_mg_ipc_handle", "sphk_mg_ipc_connect", "sphk_mg_set_transport",
     "sphk_mg_exchange_ints", "sphk_mg_exchange_ints_async", "sphk_mg_plane_ranges", "sphk_mg_halo_device", "sphk_mg_check_async", "sphk_set_active_range_device", "sphk_mg_allreduce_sum", "sphk_mg_exchange_slices", "sphk_mg_halo", "sphk_mg_check", "sphk_mg_stats",
@@ -37,6 +37,9 @@ SPH_APP_FUNCTIONS = [
 ]
 
 OPT_NEIGHBOR_LIST, OPT_LIST_CAPACITY, OPT_LIST_SKIN, OPT_SIMPLE_LIST_BUILD, OPT_TILE, OPT_STAGED_LIST_BUILD, OPT_PATCH = 1, 2, 5, 6, 9, 10, 11
+# tile-list geometry of csrc/sphk_internal.cuh (SPHK_BLOCK, SPHK_TILE_WINS, SPHK_TILE_CAP): sphk_get_tile_lists copies
+# TILE_WINDOWS windows per tile of TILE_PARTICLES particles; a tile whose windows exceed TILE_CAP records walks the cells
+TILE_PARTICLES, TILE_WINDOWS, TILE_CAP = 128, 18, 1535
 
 
 class SphkGrid(C.Structure):

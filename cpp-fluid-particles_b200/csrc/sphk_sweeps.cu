@@ -22,6 +22,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <type_traits>
 #include "sphk_internal.cuh"
 
 // =================================================================================================
@@ -134,9 +135,10 @@ struct OpDensityAlpha {
         a.gs += mg;
         a.lam += isB ? 0.0f : dot3(mg, mg);         // boundary excluded from the second term, :218
     }
+    __device__ static float alpha_of(const Acc& a) { return -1.0f / fmaxf(SPHK_EPS, dot3(a.gs, a.gs) + a.lam); }
     __device__ void end(Acc& a, int i, float4, float4, const DevScene&) const {
         density[i] = a.den;
-        alpha[i] = -1.0f / fmaxf(SPHK_EPS, dot3(a.gs, a.gs) + a.lam);
+        alpha[i] = alpha_of(a);
     }
 };
 
@@ -152,15 +154,17 @@ template <bool kDensity> struct OpDfsphError {
     __device__ void pair(Acc& a, int, int, bool, float3 d, float r2, float mj, float4 lo, float4 hi, const DevScene& s) const {
         a.e += mj * dot3(a.vi - xyz(hi), d * grad_w_factor(sqrtf(r2), s.k));
     }
-    __device__ void end(Acc& a, int i, float4, float4, const DevScene&) const {
+    __device__ void end(Acc& a, int i, float4, float4, const DevScene&) const { finish(a, i, density[i], alpha[i]); }
+    // the epilogue with the particle's density and alpha given (the fused sweep passes the values it has just formed)
+    __device__ void finish(Acc& a, int i, float rho_i, float alpha_i) const {
         float e;
-        if (kDensity) e = fmaxf(0.0f, dt * a.e + density[i] - rho0);
+        if (kDensity) e = fmaxf(0.0f, dt * a.e + rho_i - rho0);
         else {
             e = fmaxf(0.0f, a.e);
-            if (density[i] + dt * e < rho0 && density[i] <= rho0) e = 0.0f;     // :302-303
+            if (rho_i + dt * e < rho0 && rho_i <= rho0) e = 0.0f;     // :302-303
         }
         error[i] = e;
-        const float k = e * alpha[i];
+        const float k = e * alpha_i;
         stiff[i] = k;
         rec_set_s(rec + i, k);
         if (kDensity && warm) warm[i] += k;
@@ -262,6 +266,28 @@ template <class A, class B> struct OpPair {
         if (!(B::kFluidOnly && isB)) b.pair(c.b, i, j, isB, d, r2, mj, lo, hi, s);
     }
     __device__ void end(Acc& c, int i, float4 lo, float4 hi, const DevScene& s) const { a.end(c.a, i, lo, hi, s); b.end(c.b, i, lo, hi, s); }
+};
+
+// density / alpha (+ colour gradient when kColorGrad) and the divergence error in one sweep.  The error's epilogue takes the
+// particle's density and alpha from the registers they were formed in.  Reading them back from the arrays the same sweep
+// has just written is not safe: nvcc compiled those reads of the cell-walk instantiation as read-only loads issued before
+// the stores (LDG.E.CONSTANT), so the stiffness was formed with the alpha of the previous call.
+template <bool kColorGrad> struct OpDensityAlphaDivError {
+    using DA = typename std::conditional<kColorGrad, OpPair<OpDensityAlpha, OpColorGrad>, OpDensityAlpha>::type;
+    using P = OpPair<DA, OpDfsphError<false>>;
+    P p;
+    static constexpr bool kFluidOnly = P::kFluidOnly, kHi = P::kHi;
+    using Acc = typename P::Acc;
+    __device__ void begin(Acc& c, int i, float4 lo, float4 hi, const DevScene& s) const { p.begin(c, i, lo, hi, s); }
+    __device__ void pair(Acc& c, int i, int j, bool isB, float3 d, float r2, float mj, float4 lo, float4 hi, const DevScene& s) const {
+        p.pair(c, i, j, isB, d, r2, mj, lo, hi, s);
+    }
+    __device__ void end(Acc& c, int i, float4 lo, float4 hi, const DevScene& s) const {
+        p.a.end(c.a, i, lo, hi, s);
+        const OpDensityAlpha::Acc* da;
+        if constexpr (kColorGrad) da = &c.a.a; else da = &c.a;
+        p.b.finish(c.b, i, da->den, OpDensityAlpha::alpha_of(*da));
+    }
 };
 
 // viscosity + surface tension / air pressure in one sweep (BasicSPHSolver.cu:183-225 then :332-381): the
@@ -604,7 +630,10 @@ k_build_tile(const DevScene s, unsigned short* __restrict__ nbr16, int* __restri
         }
     }
     cnt[i] = n;
-    for (int m = n; (m & 7) && m < s.kmax; ++m) { *wp = static_cast<unsigned short>(T); ++wp; }   // pad the open batch with the dummy slot
+    // pad the open batch to its end with the dummy slot: the sweep reads whole batches of 8, also when kmax = 4 (mod 8).
+    // The buffer holds kmax/4 planes of 16 bytes per particle (the int32 lists' layout), at least the ceil(kmax/8) needed here.
+    if (n <= s.kmax)
+        for (int m = n; m & 7; ++m) { *wp = static_cast<unsigned short>(T); ++wp; }
 }
 
 // The default list builder: the tile's candidate windows are staged in shared memory exactly as above (cp.async.bulk +
@@ -1368,11 +1397,11 @@ extern "C" int sphk_fused_dfsph_density_alpha_div_error(sphk_ctx* c, const sphk_
     const OpDfsphError<false> err{c->rec, s->fluid.density, alpha, error, stiff, nullptr, dt, rho0};
     int rc;
     if (color_grad_or_null) {
-        OpPair<OpPair<OpDensityAlpha, OpColorGrad>, OpDfsphError<false>> op{
-            OpPair<OpDensityAlpha, OpColorGrad>{OpDensityAlpha{s->fluid.density, alpha}, OpColorGrad{color_grad_or_null, rho0, rhoB}}, err};
+        OpDensityAlphaDivError<true> op{{OpPair<OpDensityAlpha, OpColorGrad>{OpDensityAlpha{s->fluid.density, alpha},
+                                                                             OpColorGrad{color_grad_or_null, rho0, rhoB}}, err}};
         rc = run_sweep(c, s, op);
     } else {
-        OpPair<OpDensityAlpha, OpDfsphError<false>> op{OpDensityAlpha{s->fluid.density, alpha}, err};
+        OpDensityAlphaDivError<false> op{{OpDensityAlpha{s->fluid.density, alpha}, err}};
         rc = run_sweep(c, s, op);
     }
     c->sTag = stiff;
@@ -1413,13 +1442,26 @@ extern "C" int sphk_build_neighbor_list(sphk_ctx* c, const sphk_scene* s) {
 
 extern "C" int sphk_get_neighbor_list(sphk_ctx* c, const sphk_scene* s, int* counts_out, int* entries_out) {
     SPHK_CHECK_SCENE(c, s);
-    if (c->tile) return SPHK_ERR_STATE;     // tile lists hold 16-bit window slots: use sphk_get_tile_lists
+    if (c->tile) return SPHK_ERR_STATE;     // tile lists hold 16-bit window slots: sphk_get_tile_lists reads them
     const DevScene d = dev_scene(c, s);
     const int rc = ensure_list(c, d);
     if (rc != SPHK_OK) return rc;
     if (counts_out) SPHK_CUDA_TRY(cudaMemcpyAsync(counts_out, c->cnt, sizeof(int) * static_cast<size_t>(c->nF), cudaMemcpyDeviceToDevice, c->stream));
     if (entries_out) SPHK_CUDA_TRY(cudaMemcpyAsync(entries_out, c->nbr, sizeof(int) * static_cast<size_t>(c->kmax) * c->capF,
                                                    cudaMemcpyDeviceToDevice, c->stream));
+    return SPHK_OK;
+}
+
+extern "C" int sphk_get_tile_lists(sphk_ctx* c, const sphk_scene* s, int* counts_out, unsigned short* slots_out, int* windows_out) {
+    SPHK_CHECK_SCENE(c, s);
+    if (!c->tile) return SPHK_ERR_STATE;    // int32 lists: sphk_get_neighbor_list
+    const DevScene d = dev_scene(c, s);
+    const int rc = ensure_list(c, d);
+    if (rc != SPHK_OK) return rc;
+    const size_t planes = static_cast<size_t>(c->kmax + 7) / 8, tiles = (static_cast<size_t>(c->nF) + SPHK_BLOCK - 1) / SPHK_BLOCK;
+    if (counts_out) SPHK_CUDA_TRY(cudaMemcpyAsync(counts_out, c->cnt, sizeof(int) * static_cast<size_t>(c->nF), cudaMemcpyDeviceToDevice, c->stream));
+    if (slots_out) SPHK_CUDA_TRY(cudaMemcpyAsync(slots_out, c->nbr, 16 * planes * c->capF, cudaMemcpyDeviceToDevice, c->stream));
+    if (windows_out) SPHK_CUDA_TRY(cudaMemcpyAsync(windows_out, c->tileWin, sizeof(int2) * tiles * SPHK_TILE_WINS, cudaMemcpyDeviceToDevice, c->stream));
     return SPHK_OK;
 }
 

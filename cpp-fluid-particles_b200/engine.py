@@ -77,6 +77,8 @@ class SphkOps:
     (fluid, boundary, cs_fluid, cs_boundary, solver buffers), ctx and params.  The sync_* hooks are no-ops on
     one GPU; the slab driver overrides them with halo exchanges."""
 
+    list_capacity = 96               # SPHK_OPT_LIST_CAPACITY of ctx (set_option keeps it current)
+
     # ---- multi-GPU hooks ---------------------------------------------------------------------------------
     def sync_vel(self):
         pass
@@ -166,16 +168,29 @@ class SphkOps:
         check(self.L.sphk_list_stats(self.ctx, self._s(), out))
         return {"max": int(out[0]), "overflow": int(out[1]), "total": int(out[2])}
 
-    def neighbor_list(self, capacity: int = 96):
-        """(counts[n], entries[capacity/4, cap, 4]) of the current list, as torch tensors."""
-        n, cap = self.fluid.n, self.fluid.pos.shape[0]
+    def neighbor_list(self):
+        """(counts[n], entries[capacity/4, cap, 4]) of the current int32 list, as torch tensors."""
+        n, cap, kmax = self.fluid.n, self.fluid.pos.shape[0], self.list_capacity
         cnt = torch.zeros(n, dtype=torch.int32, device=self.device)
-        ent = torch.zeros(capacity * cap, dtype=torch.int32, device=self.device)
-        check(self.L.sphk_get_neighbor_list(self.ctx, self._s(), _ptr(cnt), _ptr(ent)))
-        return cnt, ent.view(capacity // 4, cap, 4)
+        ent = torch.zeros(kmax * cap, dtype=torch.int32, device=self.device)
+        check(self.L.sphk_get_neighbor_list(self.ctx, self._s(), _ptr(cnt), _ptr(ent)), "sphk_get_neighbor_list")
+        return cnt, ent.view(kmax // 4, cap, 4)
+
+    def tile_lists(self):
+        """(counts[n], slots[ceil(capacity/8), cap, 8], windows[tiles, 18, 2]) of the current tile lists (SPHK_OPT_TILE = 1),
+        as torch tensors; the slots are raw 16-bit values in an int16 tensor (read them as uint16)."""
+        n, cap, kmax = self.fluid.n, self.fluid.pos.shape[0], self.list_capacity
+        planes, tiles, wins = (kmax + 7) // 8, (n + capi.TILE_PARTICLES - 1) // capi.TILE_PARTICLES, capi.TILE_WINDOWS
+        cnt = torch.zeros(n, dtype=torch.int32, device=self.device)
+        slots = torch.zeros(planes * cap * 8, dtype=torch.int16, device=self.device)
+        win = torch.zeros(tiles * wins * 2, dtype=torch.int32, device=self.device)
+        check(self.L.sphk_get_tile_lists(self.ctx, self._s(), _ptr(cnt), _ptr(slots), _ptr(win)), "sphk_get_tile_lists")
+        return cnt, slots.view(planes, cap, 8), win.view(tiles, wins, 2)
 
     def set_option(self, opt: int, value: int):
         check(self.L.sphk_set_option(self.ctx, int(opt), int(value)))
+        if int(opt) == capi.OPT_LIST_CAPACITY:
+            self.list_capacity = int(value)
 
     def export_dots(self):
         """generate_dots (vbo.cu:26-51): (dot, colour) device tensors for the fluid set."""
@@ -461,7 +476,7 @@ class SphkSystem(SphkOps):
         check(self.L.sphk_create(C.byref(self.ctx), C.c_int(self.fluid.n), C.c_int(self.boundary.n), C.byref(g),
                                  C.c_void_p(self.stream.cuda_stream)), "sphk_create")
         if list_capacity is not None:
-            check(self.L.sphk_set_option(self.ctx, capi.OPT_LIST_CAPACITY, int(list_capacity)))
+            self.set_option(capi.OPT_LIST_CAPACITY, list_capacity)
         self.solver = self.p.solver
         self.use_list = True if use_list is None else bool(use_list)
         n = self.fluid.n

@@ -79,7 +79,8 @@ enum {
                                     unchanged since the search (WCSPH, DFSPH); 0: always walk the
                                     27 cells.  default 1 */
     SPHK_OPT_LIST_CAPACITY = 2,  /* max neighbours kept per particle; particles with more fall back
-                                    to the cell walk individually.  default 96 */
+                                    to the cell walk individually.  A multiple of 4 in [8, 1024], for the int32 lists and
+                                    the tile lists alike (a tile list is padded to whole 8-slot batches).  default 96 */
     SPHK_OPT_STAGED_LIST_BUILD = 10, /* 1 (default): the list builder stages each tile's 9 + 9 candidate windows in shared memory
                                     (cp.async.bulk + mbarrier) and tests candidates from there; 0: candidates read from global memory */
     SPHK_OPT_PATCH = 11,         /* experiment (default 0 = off): S > 0 makes the 4 warps of a list-sweep block take their
@@ -347,6 +348,16 @@ int sphk_get_permutation(sphk_ctx* ctx, int* perm_out, int n);
 /* raw copy of the current neighbour list (device to device): counts int[n]; entries int[capacity*max_fluid] in
  * the int4-packed layout nbr4[(k/4)*max_fluid + i].{x,y,z,w}.  Either pointer may be NULL. */
 int sphk_get_neighbor_list(sphk_ctx* ctx, const sphk_scene* s, int* counts_out, int* entries_out);
+/* raw copy of the current tile lists (SPHK_OPT_TILE = 1; device to device), building them first if needed:
+ *   counts_out  int[n]: neighbour count, or capacity + 1 for a particle that walks the cells (its tile's windows exceed
+ *               the staging capacity, or it lies outside the grid)
+ *   slots_out   uint16[8 * ceil(capacity/8) * max_fluid]: batch b of particle i is the 8 slots at (b*max_fluid + i)*8.  A slot
+ *               indexes the tile's staged windows (window w holds slots [pre_w, pre_w + count_w), pre_w = sum of the
+ *               counts of the windows before it); the dummy slot T = sum of all 18 counts pads the last batch to 8
+ *   windows_out int[2 * 18 * ceil(n/128)]: {first record, count} of the 9 fluid then 9 boundary windows of every tile of
+ *               128 particles (record index of boundary particle b = max_fluid + b)
+ * Any pointer may be NULL. */
+int sphk_get_tile_lists(sphk_ctx* ctx, const sphk_scene* s, int* counts_out, unsigned short* slots_out, int* windows_out);
 /* largest displacement of any particle since the skin list was built (PBD; synchronises) */
 int sphk_get_skin_displacement(sphk_ctx* ctx, float* host_out);
 /* neighbour-list statistics of the last build: host ints {max_count, overflow_particles, total} */

@@ -153,3 +153,11 @@ def test_class_api_conformance_compiles_against_both_header_sets():
     bad = open(src).read().replace("float (SPHSystem::*)()", "double (SPHSystem::*)()")
     r = subprocess.run(ours[:-1] + ["-x", "c++", "-"], input=bad, capture_output=True, text=True, timeout=300)
     assert r.returncode != 0 and "float step()" in r.stderr
+
+
+def test_tile_geometry_matches_the_library():
+    """capi's tile-list constants size the buffers sphk_get_tile_lists copies into: they must be the C definitions."""
+    from cpp_fluid_particles_b200 import capi
+    txt = open(os.path.join(ROOT, "cpp-fluid-particles_b200", "csrc", "sphk_internal.cuh")).read()
+    defs = {k: int(v) for k, v in re.findall(r"#define (SPHK_BLOCK|SPHK_TILE_WINS|SPHK_TILE_CAP)\s+(\d+)", txt)}
+    assert defs == {"SPHK_BLOCK": capi.TILE_PARTICLES, "SPHK_TILE_WINS": capi.TILE_WINDOWS, "SPHK_TILE_CAP": capi.TILE_CAP}

@@ -117,6 +117,81 @@ def test_oracle_pinned_to_reference_cuda_golden(pkg, O, solver):
     s.close()
 
 
+def oracle_per_element_ratios(O, A, p, rng):
+    """Every oracle sweep operator on A against the float64 reference (tests/ref64.py), per element.  Returns the
+    largest |x - ref| / mag of each output."""
+    import ref64
+    P = ref64.Pairs(A)
+    n = A.n
+    F = np.float32
+    vel = (0.5 * np.sin(7.0 * A.posF) + 0.05 * rng.standard_normal((n, 3))).astype(F)
+    out = {}
+
+    def dv(x, base):
+        return np.asarray(x, np.float64) - np.asarray(base, np.float64), ref64.f32_spacing(x)
+
+    dens = O.density(A)
+    out["density"] = ref64.ratio(dens, ref64.density(P))
+    dhi = (dens * F(1.3)).astype(F)
+    pres = O.pressure(dhi, p.rho0, p.stiff)
+    x, fl = dv(O.pressure_force(A, dhi, pres, vel, p.dt), vel)
+    out["pressure force"] = ref64.ratio(x, ref64.pressure_force_dv(P, dhi, pres, p.dt), fl)
+    out["viscosity"] = ref64.ratio(O.viscosity(A, vel, p.rho0, p.visc, p.dt), ref64.viscosity_dv(P, vel, p.rho0, p.visc, p.dt))
+    cg = O.color_grad(A, p.rho0, p.rho_boundary)
+    out["colour gradient"] = ref64.ratio(cg, ref64.color_grad(P, p.rho0, p.rho_boundary))
+    x, fl = dv(O.surface(A, cg, np.zeros_like(vel), p.dt, p.rho0, p.surface_tension, p.air_pressure), 0.0)
+    out["surface"] = ref64.ratio(x, ref64.surface_dv(P, cg, p.rho0, p.surface_tension, p.air_pressure, p.dt), fl)
+    d, a = O.dfsph_density_alpha(A)
+    rd, ra = ref64.dfsph_density_alpha(P)
+    out["dfsph density"], out["alpha"] = ref64.ratio(d, rd), ref64.ratio(a, ra)
+    e, k = O.dfsph_error(A, vel, d, a, p.dt, p.rho0, "div")
+    re_, rk = ref64.dfsph_div_error(P, vel, d, a, p.dt, p.rho0, tau=ref64.TAU)
+    out["divergence error"], out["divergence stiffness"] = ref64.ratio(e, re_), ref64.ratio(k, rk)
+    x, fl = dv(O.dfsph_correct(A, k, vel, 0.0), vel)
+    out["divergence correct"] = ref64.ratio(x, ref64.dfsph_correct_dv(P, k), fl)
+    dhi = (d * F(1.28)).astype(F)
+    e, k = O.dfsph_error(A, vel, dhi, a, p.dt, p.rho0, "den")
+    re_, rk = ref64.dfsph_den_error(P, vel, dhi, a, p.dt, p.rho0)
+    out["density error"], out["density stiffness"] = ref64.ratio(e, re_), ref64.ratio(k, rk)
+    x, fl = dv(O.dfsph_correct(A, k, vel, p.dt), vel)
+    out["density correct"] = ref64.ratio(x, ref64.dfsph_correct_dv(P, k, p.dt), fl)
+    rho0 = float(np.median(d))         # (PBD: about half the particles above rest density, lambda != 0)
+    d, lam = O.pbd_density_lambda(A, rho0, 0.75)
+    rd, rl = ref64.pbd_density_lambda(P, rho0, 0.75)
+    assert (lam != 0).sum() > n // 4
+    out["pbd density"], out["lambda"] = ref64.ratio(d, rd), ref64.ratio(lam, rl)
+    out["delta pos"] = ref64.ratio(O.pbd_delta_pos(A, lam, rho0), ref64.pbd_delta_pos(P, lam, rho0))
+    x, fl = dv(O.pbd_xsph(A, vel, 0.05, rho0), vel)
+    out["xsph"] = ref64.ratio(x, ref64.pbd_xsph_dv(P, vel, 0.05, rho0), fl)
+    return out
+
+
+@pytest.mark.parametrize("masses", ["uniform", "nonuniform"])
+@pytest.mark.parametrize("name,jitter", [("mini", 0.004), ("config0", 0.002), ("walls", None)])
+def test_oracle_per_element_vs_float64(pkg, O, name, jitter, masses):
+    """Every oracle operator against the float64 reference per element (not scale-relative): a wrong term on a
+    low-magnitude (surface, boundary-adjacent) particle cannot hide under the bulk's scale.  Jittered scenes (the
+    lattice puts pairs exactly at the surface-tension kernel's jump 2r = R); non-uniform masses m0 * U(0.5, 2); "walls":
+    a block against all six walls (boundary terms) with particles outside the grid (tests/sweep_driver.py)."""
+    from sweep_driver import walls_scene
+    sc = walls_scene(pkg) if name == "walls" else pkg.scene.make_scene(name, jitter=jitter)
+    p = sc.params
+    g = O.grid(p.cell_size, p.cell_length)
+    ps, _, _, cs, _ = O.neighbor_search(sc.fluid, np.zeros_like(sc.fluid), g)
+    pb, _, _, csb, _ = O.neighbor_search(sc.boundary, None, g)
+    mb = O.boundary_mass(pb, csb, g, p.rho_boundary, p.radius)
+    rng = np.random.default_rng(5)
+    m = np.full(ps.shape[0], p.m0, np.float32)
+    if masses == "nonuniform":
+        m = (m * rng.uniform(0.5, 2.0, m.shape)).astype(np.float32)
+    A = O.SceneArrays(ps, m, cs, pb, mb, csb, g, p.radius)
+    ratios = oracle_per_element_ratios(O, A, p, rng)
+    print({k: f"{v:.2e}" for k, v in ratios.items()})
+    import ref64
+    bad = {k: v for k, v in ratios.items() if not v <= ref64.TAU}
+    assert not bad, f"outside |x - ref| <= {ref64.TAU:.0e} * mag: {bad}"
+
+
 def test_oracle_dfsph_iteration_control(pkg, O):
     """Q11: negative thresholds force exactly maxIter iterations; default thresholds stop early or at 20."""
     sc = pkg.scene.benchmark_scene("mini", "dfsph")

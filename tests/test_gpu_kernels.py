@@ -86,102 +86,11 @@ def _scene_arrays(O, s, p, rcp):
 @pytest.mark.parametrize("use_list", [True, False])
 @pytest.mark.parametrize("name,jitter", [("mini", 0.004), ("config0", 0.002)])
 def test_sweeps_vs_oracle(pkg, built, O, name, jitter, use_list):
-    """Each sweep kernel on identical inputs: jittered dam-break block + a smooth random velocity field."""
-    torch = _torch()
-    sc, s = _system(pkg, name, solver="dfsph", jitter=jitter, max_iter=4, den_thr=-1.0, div_thr=-1.0, use_list=use_list)
-    p = sc.params
-    s.set_use_list(use_list)
-    rcp = s.device_rcp(p.cell_length)
-    st, A = _scene_arrays(O, s, p, rcp)
-    n = A.n
-    rng = np.random.default_rng(7)
-    vel = (0.5 * np.sin(7.0 * st["pos"]) + 0.05 * rng.standard_normal((n, 3))).astype(np.float32)
-    dev = s.device
-
-    def set_vel(v):
-        s.fluid.vel.copy_(torch.from_numpy(np.ascontiguousarray(v)))
-        s.refresh()
-        if use_list:       # refresh marks positions dirty; a new search re-validates the list on identical order
-            s.search_fluid()
-
-    # density + EOS
-    s.density(); s.pressure()
-    dens = O.density(A)
-    pres = O.pressure(dens, p.rho0, 30.0)
-    s2 = s.state()
-    assert_close(s2["density"], dens, what="density")
-    # (stiff raised so that the lattice, rho<rho0, still yields non-zero pressures for the force test)
-    s.fluid.density.copy_(torch.from_numpy(dens * np.float32(1.3)))
-    s.pressure()
-    pres = O.pressure(dens * np.float32(1.3), p.rho0, p.stiff)
-    assert_close(s.state()["pressure"], pres, what="pressure (Tait EOS)")
-    assert pres.max() > 0
-    # pressure force
-    set_vel(vel)
-    s.pressure_force()
-    v_ref = O.pressure_force(A, dens * np.float32(1.3), pres, vel, p.dt)
-    assert_close(s.state()["vel"] - vel, v_ref - vel, tol=2e-5, what="pressure force dv")
-    assert_close(s.state()["vel"], v_ref, what="pressure force vel")
-    # gravity + viscosity
-    set_vel(vel)
-    s.viscosity()
-    dv_ref = O.viscosity(A, vel, p.rho0, p.visc, p.dt)
-    assert_close(s.buffer3.cpu().numpy(), dv_ref, what="viscosity deltaV")
-    assert_close(s.state()["vel"], vel + dv_ref, what="viscosity vel")
-    # colour gradient + surface tension / air pressure
-    s.color_grad()
-    cg_ref = O.color_grad(A, p.rho0, p.rho_boundary)
-    assert_close(s.buffer3.cpu().numpy(), cg_ref, what="colour gradient")
-    set_vel(vel)
-    s.buffer3.copy_(torch.from_numpy(cg_ref))
-    s.surface()
-    v_ref = O.surface(A, cg_ref, vel, p.dt, p.rho0, p.surface_tension, p.air_pressure)
-    assert_close(s.state()["vel"] - vel, v_ref - vel, tol=2e-5, what="surface dv")
-    # DFSPH
-    s.dfsph_density_alpha()
-    d_ref, a_ref = O.dfsph_density_alpha(A)
-    assert_close(s.state()["density"], d_ref, what="dfsph density")
-    assert_close(s.alpha.cpu().numpy(), a_ref, what="dfsph alpha")
-    set_vel(vel)
-    s.alpha.copy_(torch.from_numpy(a_ref)); s.fluid.density.copy_(torch.from_numpy(d_ref))
-    s.dfsph_div_error()
-    e_ref, k_ref = O.dfsph_error(A, vel, d_ref, a_ref, p.dt, p.rho0, "div")
-    # the divergence sum cancels strongly; compare on the scale of its terms (sum_j m_j |v_ij . gradW_ij|)
-    assert_close(s.error.cpu().numpy(), e_ref, tol=5e-5, what="divergence error")
-    assert_close(s.kappa.cpu().numpy(), k_ref, tol=5e-5, what="divergence stiffness")
-    s.kappa.copy_(torch.from_numpy(k_ref))
-    s.dfsph_div_correct()
-    v_ref = O.dfsph_correct(A, k_ref, vel, 0.0)
-    assert_close(s.state()["vel"], v_ref, what="divergence correct")
-    set_vel(vel)
-    dens_hi = (d_ref * np.float32(1.28)).astype(np.float32)
-    s.fluid.density.copy_(torch.from_numpy(dens_hi))
-    s.warm.zero_()
-    s.dfsph_den_error(True)
-    e_ref, k_ref = O.dfsph_error(A, vel, dens_hi, a_ref, p.dt, p.rho0, "den")
-    assert e_ref.max() > 0
-    assert_close(s.error.cpu().numpy(), e_ref, what="density error")
-    assert_close(s.kappa.cpu().numpy(), k_ref, what="density stiffness")
-    assert_close(s.warm.cpu().numpy(), k_ref, what="warm stiffness accumulate")
-    s.kappa.copy_(torch.from_numpy(k_ref))
-    s.dfsph_den_correct()
-    v_ref = O.dfsph_correct(A, k_ref, vel, p.dt)
-    assert_close(s.state()["vel"], v_ref, what="density correct")
-    # abs-sum reduction (order unspecified in the reference: tolerance, not bit-exact)
-    tot = s.reduce_abs_sum(s.error)
-    assert abs(tot - float(np.abs(e_ref.astype(np.float64)).sum())) <= 1e-5 * max(1.0, float(np.abs(e_ref).sum()))
-    # advect + clamp: push some particles through the walls
-    big = vel.copy(); big[::5] *= 400.0
-    set_vel(big)
-    pos0 = s.state()["pos"]
-    s.advect()
-    p_ref, v_ref = O.advect(pos0, big, p.dt, p.space)
-    st3 = s.state()
-    assert_close(st3["pos"], p_ref, tol=1e-6, what="advect pos")
-    assert np.array_equal(st3["vel"] == 0, v_ref == 0)
-    assert_close(st3["vel"], v_ref, tol=1e-6, what="advect vel (clamped)")
-    assert st3["pos"].min() >= 0.0 and st3["pos"].max() <= 0.99 * p.space[0] + 1e-7
-    s.close()
+    """Each sweep kernel on identical inputs: jittered dam-break block + a smooth random velocity field (the shared driver
+    of tests/sweep_driver.py; the full path matrix is tests/test_gpu_paths.py)."""
+    from sweep_driver import PATHS, Case, run_sweeps
+    sc = pkg.scene.make_scene(name, solver="dfsph", jitter=jitter, max_iter=4, den_thr=-1.0, div_thr=-1.0)
+    run_sweeps(pkg, O, Case(name, sc, lattice_like=False), PATHS["list" if use_list else "cells"])
 
 
 @pytest.mark.parametrize("name,jitter", [("mini", 0.004), ("config0", 0.002)])
