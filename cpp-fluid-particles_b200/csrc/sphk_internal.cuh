@@ -79,7 +79,6 @@ struct sphk_ctx {
     const int* rangeDev = nullptr;   // non-null: the active range {begin, count} lives in DEVICE memory (slab ranks: computed from
                                      // the cell ranges by sphk_mg_plane_ranges, never read by the host); kernels are launched over
                                      // all nF particles and the ones outside the range return
-    const int* listRangeDev = nullptr;
     int kmax = 96;
     bool useList = true;
     int patch = 0;                   // SPHK_OPT_PATCH (experiment): list sweeps map a block onto a y x z patch of cells

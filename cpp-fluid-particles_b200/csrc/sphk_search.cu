@@ -213,9 +213,15 @@ extern "C" int sphk_create(sphk_ctx** out, int max_fluid, int max_boundary, cons
     }
     if (e == cudaSuccess) e = cudaMallocHost(reinterpret_cast<void**>(&c->pinned), 64);
     if (e == cudaSuccess) {
+        // sized for the widest key any grid can need (32 bits), not only for this grid's: the scratch grows with the number
+        // of 8-bit passes, and sphk_set_grid may re-target the context at a grid with more cells without re-allocating
         c->cubTempBytes = 0;
-        e = cub::DeviceRadixSort::SortPairs(nullptr, c->cubTempBytes, c->keys, c->keysSorted, c->idx, c->idxSorted,
-                                            static_cast<int>(cap), 0, c->endBit, c->stream);
+        for (int bits : {c->endBit, 32}) {
+            size_t bytes = 0;
+            if (e == cudaSuccess) e = cub::DeviceRadixSort::SortPairs(nullptr, bytes, c->keys, c->keysSorted, c->idx, c->idxSorted,
+                                                                      static_cast<int>(cap), 0, bits, c->stream);
+            if (bytes > c->cubTempBytes) c->cubTempBytes = bytes;
+        }
         if (e == cudaSuccess) e = cudaMalloc(&c->cubTemp, c->cubTempBytes ? c->cubTempBytes : 1);
     }
     if (e != cudaSuccess) { sphk_destroy(c); cudaGetLastError(); return e == cudaErrorMemoryAllocation ? SPHK_ERR_ALLOC : static_cast<int>(e); }

@@ -1035,15 +1035,18 @@ SkinTrack sphk_skin_track(const sphk_ctx* c, float radius, bool on) {
 }
 
 static int ensure_list(sphk_ctx* c, const DevScene& d) {
-    // lists are built for the particles the sweeps will compute (the active range: ghosts of a slab rank need none)
-    if (c->listEpoch == c->searchEpoch && d.iBegin >= c->listBegin && d.iEnd <= c->listEnd && c->listRangeDev == c->rangeDev) return SPHK_OK;
+    // lists are built for the particles the sweeps will compute (the active range: ghosts of a slab rank need none).  A
+    // device-resident range is not known to the host, and its contents may change between sweeps: the lists are then built for
+    // all nF particles (d.iBegin = 0, d.iEnd = nF), so any range the device later holds finds its lists.
+    if (c->listEpoch == c->searchEpoch && d.iBegin >= c->listBegin && d.iEnd <= c->listEnd) return SPHK_OK;
     if (!c->nbr) {
         const size_t bytes = sizeof(int) * static_cast<size_t>(c->kmax) * (static_cast<size_t>(c->capF) + 2);
         if (cudaMalloc(reinterpret_cast<void**>(&c->nbr), bytes) != cudaSuccess) { cudaGetLastError(); return SPHK_ERR_ALLOC; }
     }
     DevScene b = d;
     b.nbr = c->nbr;
-    c->listBegin = d.iBegin; c->listEnd = d.iEnd; c->listRangeDev = c->rangeDev;
+    b.rangeDev = nullptr;
+    c->listBegin = d.iBegin; c->listEnd = d.iEnd;
     c->listHasSkin = c->skin > 0.f;
     if (c->listHasSkin) {
         const float rs = d.k.R * (1.0f + c->skin);

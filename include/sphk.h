@@ -107,7 +107,8 @@ int  sphk_create(sphk_ctx** ctx, int max_fluid, int max_boundary, const sphk_gri
 void sphk_destroy(sphk_ctx* ctx);
 int  sphk_set_option(sphk_ctx* ctx, int option, int value);
 /* re-target the context at another (sub-)grid with the same cell length (a slab rank whose cuts moved): both particle
- * sets must be searched again before the next sweep; capacities and buffers are kept */
+ * sets must be searched again before the next sweep; capacities and buffers are kept (the sort scratch is sized at creation
+ * for any grid) */
 int  sphk_set_grid(sphk_ctx* ctx, const sphk_grid* grid);
 int  sphk_synchronize(sphk_ctx* ctx);
 const char* sphk_error_string(int code);
@@ -257,7 +258,8 @@ int sphk_export_dots(sphk_ctx* ctx, const sphk_particles* p, float* dot_xyz, flo
  * arrays (contiguous slices) and are mirrored into the packed records. */
 /* restrict every subsequent sweep to particles [begin, begin+count) of the fluid set (count<0: all) */
 int sphk_set_active_range(sphk_ctx* ctx, int begin, int count);
-/* the same with {begin, count} in DEVICE memory, read by the kernels themselves (NULL: back to the host-side range) */
+/* the same with {begin, count} in DEVICE memory, read by the kernels themselves (NULL: back to the host-side range).  The
+ * contents may change between sweeps (the neighbour lists are then built for all particles of the set) */
 int sphk_set_active_range_device(sphk_ctx* ctx, const int* device_begin_count);
 /* copy API data of particles [begin, begin+count) into the packed records: what is a bit mask -- 1: vel
  * (scene->fluid.vel), 2: neighbour scalar from `array` (float[n]), 4: pos (scene->fluid.pos; PBD ghosts moved by
