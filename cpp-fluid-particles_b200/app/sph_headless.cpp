@@ -8,7 +8,10 @@
 // (positions, densities and the generate_dots colours of vbo.cu:26-51) for offline viewing.
 //
 //   sph_headless [--solver sph|dfsph|pbd] [--frames N] [--box L | --box LX LY LZ] [--block NX NY NZ] [--origin X Y Z]
-//                [--dt DT] [--iters K] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] [--ranks N [--rank R --rendezvous DIR]] [--bullets K]
+//                [--dt DT] [--iters K] [--vorticity EPS] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] [--ranks N [--rank R --rendezvous DIR]]
+//                [--bullets K]
+// --vorticity EPS turns on vorticity confinement of strength EPS (BasicSPHSolver::setVorticityConfinement) after the
+// constructor's step 0, for every solver and with --ranks.
 // --emit-scene writes the generated scene (PREFIX.fluid.f32, PREFIX.boundary.f32) and exits: needs no GPU, lets a
 // test compare this generator with the python one the benchmarks use.
 // --ranks N runs the same scene on N GPUs through SlabSPHSystem (host/sph_slab.hpp: the class API sharded by x-slabs):
@@ -53,6 +56,7 @@ struct Options {
     int iters = 0;                            // > 0: fixed iteration count (DFSPH thresholds -1, Q11)
     std::string dump, emitScene;
     bool quiet = false;
+    float vorticity = 0.0f;                   // --vorticity EPS: vorticity confinement from frame 1 on (0: off)
     int bullets = 0;                          // test aid: this many top-layer particles start at ~3 cell planes per step
     int ranks = 1, rank = -1;                 // --ranks N: SlabSPHSystem on N GPUs; --rank R: this process is rank R
     std::string rendezvous;
@@ -70,6 +74,7 @@ bool parse(int argc, char** argv, Options& o) {
         else if (a == "--emit-scene" && need(i, 1)) o.emitScene = argv[++i];
         else if (a == "--quiet") o.quiet = true;
         else if (a == "--bullets" && need(i, 1)) o.bullets = std::atoi(argv[++i]);
+        else if (a == "--vorticity" && need(i, 1)) o.vorticity = static_cast<float>(std::atof(argv[++i]));
         else if (a == "--ranks" && need(i, 1)) o.ranks = std::atoi(argv[++i]);
         else if (a == "--rank" && need(i, 1)) o.rank = std::atoi(argv[++i]);
         else if (a == "--rendezvous" && need(i, 1)) o.rendezvous = argv[++i];
@@ -89,7 +94,7 @@ bool parse(int argc, char** argv, Options& o) {
         }
     }
     if (o.ranks < 1 || o.rank >= o.ranks || (o.rank >= 0 && o.ranks > 1 && o.rendezvous.empty())) return false;
-    return o.frames >= 0 && o.block[0] > 0 && o.block[1] > 0 && o.block[2] > 0 &&
+    return o.frames >= 0 && o.vorticity >= 0.0f && o.block[0] > 0 && o.block[1] > 0 && o.block[2] > 0 &&
            (o.solver == "sph" || o.solver == "wcsph" || o.solver == "dfsph" || o.solver == "pbd");
 }
 
@@ -175,7 +180,7 @@ int main(int argc, char** argv) {
     Options o;
     if (!parse(argc, argv, o)) {
         std::fprintf(stderr, "usage: sph_headless [--solver sph|dfsph|pbd] [--frames N] [--box L | LX LY LZ] [--block NX NY NZ] "
-                             "[--origin X Y Z] [--dt DT] [--iters K] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] "
+                             "[--origin X Y Z] [--dt DT] [--iters K] [--vorticity EPS] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] "
                              "[--ranks N [--rank R --rendezvous DIR]]\n");
         return 2;
     }
@@ -260,6 +265,7 @@ int main(int argc, char** argv) {
         pSolver = o.iters > 0 ? std::make_shared<DFSPHSolver>(nFluid, -1.0f, -1.0f, o.iters) : std::make_shared<DFSPHSolver>(nFluid);
     else
         pSolver = std::make_shared<BasicSPHSolver>(nFluid);
+    BasicSPHSolver* basicSolver = dynamic_cast<BasicSPHSolver*>(pSolver.get());   // (the systems take pSolver over)
     std::shared_ptr<SPHSystem> pSystem;
     std::shared_ptr<SlabSPHSystem> pSlab;
     if (slab) {
@@ -278,6 +284,8 @@ int main(int argc, char** argv) {
         std::fprintf(stderr, "sph_headless: %s\n", cudaGetErrorString(cudaGetLastError()));
         return 4;
     }
+
+    if (o.vorticity > 0.0f) basicSolver->setVorticityConfinement(o.vorticity);
 
     if (o.bullets > 0) {
         const int hit = slab ? shoot(o, sphSpacing, dt, pSlab->getFluids(), static_cast<size_t>(pSlab->ownedBegin()), static_cast<size_t>(pSlab->size()))

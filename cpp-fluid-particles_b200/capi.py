@@ -25,7 +25,8 @@ SPHK_FUNCTIONS = [
     "sphk_dfsph_den_error", "sphk_dfsph_den_correct", "sphk_reduce_abs_sum", "sphk_copy", "sphk_pbd_density_lambda",
     "sphk_pbd_delta_pos_apply", "sphk_pbd_velocity_from_positions", "sphk_pbd_xsph", "sphk_get_permutation",
     "sphk_list_stats", "sphk_get_skin_displacement", "sphk_set_active_range", "sphk_push_range", "sphk_build_neighbor_list", "sphk_get_neighbor_list", "sphk_get_tile_lists", "sphk_fused_density_color_grad",
-    "sphk_fused_dfsph_density_alpha_color_grad", "sphk_fused_dfsph_density_alpha_div_error", "sphk_fused_pbd_xsph_color_grad", "sphk_scene_fluid_block", "sphk_scene_boundary_count", "sphk_scene_boundary_shell", "sphk_loop_begin", "sphk_loop_next", "sphk_loop_end", "sphk_loop_iterations", "sphk_fused_viscosity_surface", "sphk_export_dots", "sphk_particles_advect", "sphk_add_launches",
+    "sphk_fused_dfsph_density_alpha_color_grad", "sphk_fused_dfsph_density_alpha_div_error", "sphk_fused_pbd_xsph_color_grad", "sphk_scene_fluid_block", "sphk_scene_boundary_count", "sphk_scene_boundary_shell", "sphk_loop_begin", "sphk_loop_next", "sphk_loop_end", "sphk_loop_iterations", "sphk_fused_viscosity_surface", "sphk_vorticity", "sphk_vorticity_confinement",
+    "sphk_fused_viscosity_surface_vorticity", "sphk_fused_pbd_xsph_vorticity", "sphk_export_dots", "sphk_particles_advect", "sphk_add_launches",
     "sphk_mg_unique_id", "sphk_mg_init", "sphk_mg_destroy", "sphk_mg_ipc_handle", "sphk_mg_ipc_connect", "sphk_mg_set_transport",
     "sphk_mg_exchange_ints", "sphk_mg_exchange_ints_async", "sphk_mg_plane_ranges", "sphk_mg_halo_device", "sphk_mg_check_async", "sphk_set_active_range_device", "sphk_mg_allreduce_sum", "sphk_mg_exchange_slices", "sphk_mg_halo", "sphk_mg_check", "sphk_mg_stats",
     "sphk_strays_block_floats", "sphk_strays_collect", "sphk_strays_append", "sphk_mg_strays_route", "sphk_strays_counts",
@@ -33,7 +34,7 @@ SPHK_FUNCTIONS = [
 SPH_APP_FUNCTIONS = [
     "sph_app_create", "sph_app_destroy", "sph_app_step", "sph_app_fluid_size", "sph_app_boundary_size",
     "sph_app_download_fluid", "sph_app_download_boundary", "sph_app_upload_fluid", "sph_app_engine",
-    "sph_app_submit", "sph_app_wait", "sph_app_dfsph_iterations", "sph_app_set_option",
+    "sph_app_submit", "sph_app_wait", "sph_app_dfsph_iterations", "sph_app_set_option", "sph_app_set_vorticity",
 ]
 
 OPT_NEIGHBOR_LIST, OPT_LIST_CAPACITY, OPT_LIST_SKIN, OPT_SIMPLE_LIST_BUILD, OPT_TILE, OPT_STAGED_LIST_BUILD, OPT_PATCH = 1, 2, 5, 6, 9, 10, 11
@@ -206,6 +207,11 @@ class SphApp:
         """1: device-side loop tests (adaptive DFSPH), 2: fused sweeps, 3: step graph."""
         if self.L.sph_app_set_option(self.h, C.c_int(option), C.c_int(value)):
             raise RuntimeError("sph_app_set_option failed")
+
+    def set_vorticity(self, eps: float):
+        """Vorticity confinement of strength eps in every following step (0: off).  Not on the reference engine."""
+        if self.L.sph_app_set_vorticity(self.h, C.c_float(eps)):
+            raise RuntimeError("sph_app_set_vorticity failed (reference engine, or eps < 0)")
 
     def close(self):
         if getattr(self, "h", None):

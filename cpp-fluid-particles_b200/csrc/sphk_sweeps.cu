@@ -322,6 +322,56 @@ struct OpViscositySurface {
     }
 };
 
+// ---- vorticity confinement (no reference counterpart; Macklin & Mueller 2013, section 5) ----------------------------------
+__device__ __forceinline__ float3 cross3(float3 a, float3 b) {
+    return f3(a.y * b.z - a.z * b.y, a.z * b.x - a.x * b.z, a.x * b.y - a.y * b.x);
+}
+
+// omega_i = sum_j V_j (v_i - v_j) x gradW_ij, V_j = m_j / rho0, fluid neighbours only (a boundary has no velocity field to
+// curl).  Rigid rotation v = W x x gives +2 W in the bulk.  |omega_i| goes to omegaNorm only, never to rec.s: a fused sweep
+// gathers the neighbours' rec.s = |c|^2 while this runs.  r^2, r and the arithmetic after the kernel gradient are written with
+// rounded intrinsics: nvcc contracts a * b - c * d into an FMA either way round depending on the kernel it is inlined into,
+// and the fused sweeps must form omega bit for bit as this sweep does.
+struct OpVorticity {
+    float* omega; float* omegaNorm; float invRho0;
+    static constexpr bool kFluidOnly = true, kHi = true;
+    struct Acc { float3 w; float3 vi; template <class F> __device__ void sums(F f) { f(w.x); f(w.y); f(w.z); } };
+    __device__ void begin(Acc& a, int, float4, float4 hi, const DevScene&) const { a.w = f3(0, 0, 0); a.vi = xyz(hi); }
+    __device__ void pair(Acc& a, int, int, bool, float3 d, float, float mj, float4, float4 hi, const DevScene& s) const {
+        // (r^2 formed here: the drivers' dot product is contracted differently in different instantiations)
+        const float r2 = __fmaf_rn(d.z, d.z, __fmaf_rn(d.y, d.y, __fmul_rn(d.x, d.x)));
+        const float gw = grad_w_factor(__fsqrt_rn(r2), s.k);
+        const float3 g = f3(__fmul_rn(d.x, gw), __fmul_rn(d.y, gw), __fmul_rn(d.z, gw));
+        const float3 u = f3(__fsub_rn(a.vi.x, hi.x), __fsub_rn(a.vi.y, hi.y), __fsub_rn(a.vi.z, hi.z));
+        const float V = __fmul_rn(mj, invRho0);
+        a.w.x = __fmaf_rn(V, __fsub_rn(__fmul_rn(u.y, g.z), __fmul_rn(u.z, g.y)), a.w.x);
+        a.w.y = __fmaf_rn(V, __fsub_rn(__fmul_rn(u.z, g.x), __fmul_rn(u.x, g.z)), a.w.y);
+        a.w.z = __fmaf_rn(V, __fsub_rn(__fmul_rn(u.x, g.y), __fmul_rn(u.y, g.x)), a.w.z);
+    }
+    __device__ void end(Acc& a, int i, float4, float4, const DevScene&) const {
+        store3(omega, i, a.w);
+        omegaNorm[i] = __fsqrt_rn(__fmaf_rn(a.w.z, a.w.z, __fmaf_rn(a.w.y, a.w.y, __fmul_rn(a.w.x, a.w.x))));
+    }
+};
+
+// eta_i = sum_j V_j (|omega_j| - |omega_i|) gradW_ij (difference form: a uniform |omega| gives exactly 0), N = eta / max(|eta|,
+// eps), v_i += dt eps (N x omega_i).  rec.s = |omega| (mirrored by the entry).  Reads no neighbour velocity: in place.
+struct OpVorticityConfinement {
+    Rec rec; float* vel; const float* omega; float invRho0, dtEps;
+    static constexpr bool kFluidOnly = true, kHi = false;
+    struct Acc { float3 eta; float wi; template <class F> __device__ void sums(F f) { f(eta.x); f(eta.y); f(eta.z); } };
+    __device__ void begin(Acc& a, int, float4 lo, float4, const DevScene&) const { a.eta = f3(0, 0, 0); a.wi = lo.w; }
+    __device__ void pair(Acc& a, int, int, bool, float3 d, float r2, float mj, float4 lo, float4, const DevScene& s) const {
+        a.eta += (mj * invRho0 * (lo.w - a.wi)) * (d * grad_w_factor(sqrtf(r2), s.k));
+    }
+    __device__ void end(Acc& a, int i, float4, float4 hi, const DevScene&) const {
+        const float3 n = a.eta / fmaxf(sqrtf(dot3(a.eta, a.eta)), SPHK_EPS);
+        const float3 dv = dtEps * cross3(n, load3(omega, i));
+        const float3 v = f3(hi.x + dv.x, hi.y + dv.y, hi.z + dv.z);
+        rec_set_vel(rec + i, v); store3(vel, i, v);
+    }
+};
+
 // =================================================================================================
 // Sweep drivers
 // =================================================================================================
@@ -1429,6 +1479,83 @@ extern "C" int sphk_fused_viscosity_surface(sphk_ctx* c, const sphk_scene* s, fl
     if (rc != SPHK_OK) return rc;
     const int b = (c->actCount < 0 || c->rangeDev) ? 0 : c->actBegin, e = (c->actCount < 0 || c->rangeDev) ? c->nF : c->actBegin + c->actCount;
     if (e > b) k_commit_vel<<<sphk_blocks(e - b), SPHK_BLOCK, 0, c->stream>>>(tmp, c->rec, nullptr, b, e, c->rangeDev);
+    c->launches++;
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+// ---- vorticity confinement (no reference counterpart) ---------------------------------------------------------------------
+// The entries that form omega never write |omega| into rec.s (the fused viscosity + surface sweep gathers rec.s = |c|^2);
+// they leave omega_norm, which sphk_vorticity_confinement mirrors into the records before it gathers it.
+static int check_vorticity(const float* omega, const float* omega_norm, float rho0) {
+    if (!omega || !omega_norm || omega == omega_norm || !(rho0 > 0.f)) return SPHK_ERR_INVALID;
+    return SPHK_OK;
+}
+
+extern "C" int sphk_vorticity(sphk_ctx* c, const sphk_scene* s, float* omega, float* omega_norm, float rho0) {
+    SPHK_CHECK_SCENE(c, s);
+    if (check_vorticity(omega, omega_norm, rho0) != SPHK_OK) return SPHK_ERR_INVALID;
+    if (c->sTag == omega_norm) c->sTag = nullptr;
+    OpVorticity op{omega, omega_norm, 1.0f / rho0};
+    return run_sweep(c, s, op);
+}
+
+extern "C" int sphk_vorticity_confinement(sphk_ctx* c, const sphk_scene* s, const float* omega, const float* omega_norm, float eps,
+                                          float dt, float rho0) {
+    SPHK_CHECK_SCENE(c, s);
+    if (check_vorticity(omega, omega_norm, rho0) != SPHK_OK || !(eps >= 0.f) || !(dt == dt)) return SPHK_ERR_INVALID;
+    ensure_scalar(c, omega_norm);
+    OpVorticityConfinement op{c->rec, s->fluid.vel, omega, 1.0f / rho0, dt * eps};
+    return run_sweep(c, s, op);
+}
+
+// viscosity + surface tension / air pressure + vorticity in one sweep: omega is formed from the velocities the viscosity
+// term reads (the records before the commit of the new velocities)
+extern "C" int sphk_fused_viscosity_surface_vorticity(sphk_ctx* c, const sphk_scene* s, float* delta_v, const float* color_grad,
+                                                      float rho0, float visc, float dt, float kappa, float airP, float* omega,
+                                                      float* omega_norm) {
+    SPHK_CHECK_SCENE(c, s);
+    if (!delta_v || !color_grad || delta_v == color_grad) return SPHK_ERR_INVALID;
+    if (check_vorticity(omega, omega_norm, rho0) != SPHK_OK) return SPHK_ERR_INVALID;
+    if (c->sTag == omega_norm) c->sTag = nullptr;
+    const void* tag = reinterpret_cast<const void*>(reinterpret_cast<uintptr_t>(color_grad) | 1u);
+    if (c->sTag != tag) {
+        k_s_cg2<<<sphk_blocks(c->nF), SPHK_BLOCK, 0, c->stream>>>(color_grad, c->rec, c->nF);
+        c->launches++;
+        c->sTag = tag;
+    }
+    float4* tmp = c->snapB;
+    OpPair<OpViscositySurface, OpVorticity> op{OpViscositySurface{tmp, s->fluid.vel, delta_v, rho0, visc, dt, kappa, airP},
+                                               OpVorticity{omega, omega_norm, 1.0f / rho0}};
+    const int rc = run_sweep(c, s, op);
+    if (rc != SPHK_OK) return rc;
+    const int b = (c->actCount < 0 || c->rangeDev) ? 0 : c->actBegin, e = (c->actCount < 0 || c->rangeDev) ? c->nF : c->actBegin + c->actCount;
+    if (e > b) k_commit_vel<<<sphk_blocks(e - b), SPHK_BLOCK, 0, c->stream>>>(tmp, c->rec, nullptr, b, e, c->rangeDev);
+    c->launches++;
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+// XSPH (+ colour gradient when color_grad_or_null != NULL) + vorticity in one sweep: omega is formed from the velocities XSPH
+// reads
+extern "C" int sphk_fused_pbd_xsph_vorticity(sphk_ctx* c, const sphk_scene* s, float xc, float rho0, float* color_grad_or_null,
+                                             float rhoB, float* omega, float* omega_norm) {
+    SPHK_CHECK_SCENE(c, s);
+    if (check_vorticity(omega, omega_norm, rho0) != SPHK_OK) return SPHK_ERR_INVALID;
+    if (c->sTag == omega_norm) c->sTag = nullptr;
+    float4* tmp = c->snapB;
+    const OpVorticity vort{omega, omega_norm, 1.0f / rho0};
+    int rc;
+    if (color_grad_or_null) {
+        OpPair<OpPair<OpXsph, OpColorGrad>, OpVorticity> op{{OpXsph{tmp, xc, rho0}, OpColorGrad{color_grad_or_null, rho0, rhoB}}, vort};
+        rc = run_sweep(c, s, op);
+    } else {
+        OpPair<OpXsph, OpVorticity> op{OpXsph{tmp, xc, rho0}, vort};
+        rc = run_sweep(c, s, op);
+    }
+    if (rc != SPHK_OK) return rc;
+    const int b = (c->actCount < 0 || c->rangeDev) ? 0 : c->actBegin, e = (c->actCount < 0 || c->rangeDev) ? c->nF : c->actBegin + c->actCount;
+    if (e > b) k_commit_vel<<<sphk_blocks(e - b), SPHK_BLOCK, 0, c->stream>>>(tmp, c->rec, s->fluid.vel, b, e, c->rangeDev);
     c->launches++;
     SPHK_CUDA_TRY(cudaGetLastError());
     return SPHK_OK;

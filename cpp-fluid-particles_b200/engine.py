@@ -78,6 +78,7 @@ class SphkOps:
     one GPU; the slab driver overrides them with halo exchanges."""
 
     list_capacity = 96               # SPHK_OPT_LIST_CAPACITY of ctx (set_option keeps it current)
+    vorticity_eps = 0.0              # vorticity confinement strength (BasicSPHSolver::setVorticityConfinement); 0: off
 
     # ---- multi-GPU hooks ---------------------------------------------------------------------------------
     def sync_vel(self):
@@ -251,6 +252,33 @@ class SphkOps:
                                                   C.c_float(self.p.surface_tension), C.c_float(self.p.air_pressure)),
               "sphk_fused_viscosity_surface")
 
+    # ---- vorticity confinement (no reference counterpart) ----------------------------------------------------------------
+    def _vort_buffers(self):
+        if getattr(self, "omega", None) is None:   # allocated on first use, like the class layer's
+            n = self.buffer3.shape[0]
+            self.omega = torch.zeros((n, 3), dtype=torch.float32, device=self.device)
+            self.omega_norm = torch.zeros(n, dtype=torch.float32, device=self.device)
+        return _ptr(self.omega), _ptr(self.omega_norm)
+
+    def vorticity(self):
+        check(self.L.sphk_vorticity(self.ctx, self._s(), *self._vort_buffers(), C.c_float(self.p.rho0)), "sphk_vorticity")
+
+    def vorticity_confinement(self, eps=None):
+        check(self.L.sphk_vorticity_confinement(self.ctx, self._s(), *self._vort_buffers(),
+                                                C.c_float(self.vorticity_eps if eps is None else eps), C.c_float(self.p.dt),
+                                                C.c_float(self.p.rho0)), "sphk_vorticity_confinement")
+
+    def fused_viscosity_surface_vorticity(self):
+        check(self.L.sphk_fused_viscosity_surface_vorticity(self.ctx, self._s(), _ptr(self.buffer3), _ptr(self.color_grad_buf),
+                                                            C.c_float(self.p.rho0), C.c_float(self.p.visc), C.c_float(self.p.dt),
+                                                            C.c_float(self.p.surface_tension), C.c_float(self.p.air_pressure),
+                                                            *self._vort_buffers()), "sphk_fused_viscosity_surface_vorticity")
+
+    def fused_pbd_xsph_vorticity(self, with_color_grad: bool):
+        check(self.L.sphk_fused_pbd_xsph_vorticity(self.ctx, self._s(), C.c_float(self.xsph_c), C.c_float(self.p.rho0),
+                                                   _ptr(self.buffer3) if with_color_grad else None, C.c_float(self.p.rho_boundary),
+                                                   *self._vort_buffers()), "sphk_fused_pbd_xsph_vorticity")
+
     def pressure(self):
         check(self.L.sphk_pressure(self.ctx, self._s(), C.c_float(self.p.rho0), C.c_float(self.p.stiff)), "sphk_pressure")
 
@@ -334,14 +362,27 @@ class SphkOps:
     def step_wcsph(self):            # BasicSPHSolver.cu:237-260
         self.set_use_list(self.use_list)
         self.gravity()
+        vort = self.vorticity_eps > 0
+        if vort:
+            self._vort_buffers()
         if self.fused and self._surface_enabled():
             self._run(lambda: self.fused_density_color_grad(False), "array", self.color_grad_buf)
-            self._run(self.fused_viscosity_surface, "vel", split=False)
+            if vort:                 # + omega from the velocities the viscosity term reads
+                self._run(self.fused_viscosity_surface_vorticity, "vel", split=False)
+                self.sync_scalar(self.omega_norm)
+            else:
+                self._run(self.fused_viscosity_surface, "vel", split=False)
+            if vort:
+                self._run(self.vorticity_confinement, "vel")
         else:
+            if vort:
+                self._run(self.vorticity, "scalar", self.omega_norm)
             self._run(self.viscosity, "vel", split=False)
             if self._surface_enabled():  # handleSurface, :262-275
                 self._run(self.color_grad, "array", self.buffer3)
                 self._run(self.surface, "vel")
+            if vort:
+                self._run(self.vorticity_confinement, "vel")
             self.density()
         self.pressure()
         self.sync_array(self.fluid.density); self.sync_array(self.fluid.pressure)
@@ -370,13 +411,23 @@ class SphkOps:
                 total = self.reduce_sum(self.reduce_abs_sum(self.owned(self.error)))
         self.it_div = it
         self.gravity()
-        if fused:
+        vort = self.vorticity_eps > 0
+        if vort:
+            self._vort_buffers()
+        if fused and vort:           # + omega from the velocities the viscosity term reads
+            self._run(self.fused_viscosity_surface_vorticity, "vel", split=False)
+            self.sync_scalar(self.omega_norm)
+        elif fused:
             self._run(self.fused_viscosity_surface, "vel", split=False)
         else:
+            if vort:
+                self._run(self.vorticity, "scalar", self.omega_norm)
             self._run(self.viscosity, "vel", split=False)
             if self._surface_enabled():
                 self._run(self.color_grad, "array", self.buffer3)
                 self._run(self.surface, "vel")
+        if vort:                     # after surface, before the density solve
+            self._run(self.vorticity_confinement, "vel")
         total, it = 3.4e38, 0        # project :160-210
         self.permute(self.warm, 1)
         self._run(lambda: self.dfsph_den_correct(self.warm), "vel")
@@ -402,15 +453,29 @@ class SphkOps:
             self._run(self.pbd_density_lambda, "scalar", self.lam)
             self.pbd_delta_pos_apply(); self.sync_positions()
         self.pbd_velocity_from_positions()
-        if self.fused and self._surface_enabled():   # XSPH + colour gradient in one sweep, then the surface sweep
+        vort = self.vorticity_eps > 0
+        if vort:
+            self._vort_buffers()
+        if self.fused and vort:      # XSPH (+ colour gradient) + omega from the velocities XSPH reads
+            surf = self._surface_enabled()
+            self._run(lambda: self.fused_pbd_xsph_vorticity(surf), "vel", split=False)
+            self.sync_scalar(self.omega_norm)
+            if surf:
+                self.sync_array(self.buffer3)
+                self._run(self.surface, "vel")
+        elif self.fused and self._surface_enabled():   # XSPH + colour gradient in one sweep, then the surface sweep
             self._run(self.fused_pbd_xsph_color_grad, "vel", split=False)
             self.sync_array(self.buffer3)
             self._run(self.surface, "vel")
         else:
+            if vort:
+                self._run(self.vorticity, "scalar", self.omega_norm)
             self._run(self.pbd_xsph, "vel", split=False)
             if self._surface_enabled():
                 self._run(self.color_grad, "array", self.buffer3)
                 self._run(self.surface, "vel")
+        if vort:                     # after XSPH and surface, before gravity
+            self._run(self.vorticity_confinement, "vel")
         self.gravity()
         self.copy(self.pos_last, self.fluid.pos)
         self.advect()

@@ -260,6 +260,18 @@ extern "C" int sph_app_set_option(sph_app* app, int option, int value) {
 #endif
 }
 
+extern "C" int sph_app_set_vorticity(sph_app* app, float eps) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)eps;
+    return 1;
+#else
+    auto* b = dynamic_cast<BasicSPHSolver*>(app->solver);
+    if (!b || !(eps >= 0.0f)) return 1;
+    b->setVorticityConfinement(eps);
+    return 0;
+#endif
+}
+
 extern "C" const char* sph_app_engine(void) {
 #ifdef SPH_APP_REFERENCE_ENGINE
     return "reference-cuda";

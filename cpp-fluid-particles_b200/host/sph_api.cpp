@@ -90,15 +90,18 @@ void BasicSPHSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shar
         if (surface) produced(0, colorGradBuffer(), 3);
         diffuseAndSurface(rho0, rhoB, visc, dt, surfaceTensionIntensity, airPressure, surface, true);
         producedVel(fluids);
+        if (vorticityOn()) confine(fluids, rho0, dt);
         check(sphk_pressure(current_.ctx, &current_.abi, rho0, stiff), "sphk_pressure");
         produced(0, fluids->getDensityPtr(), 1); produced(0, fluids->getPressurePtr(), 1);
         check(sphk_pressure_force(current_.ctx, &current_.abi, dt), "sphk_pressure_force");
     } else {
+        if (vorticityOn()) vorticity(rho0);
         diffuse(fluids, cellStartFluid, cellSize, cellLength, rho0, radius, visc, dt);
         producedVel(fluids);
         if (surface)
             handleSurface(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, rhoB, cellSize, cellLength, radius,
                           dt, surfaceTensionIntensity, airPressure);
+        if (vorticityOn()) confine(fluids, rho0, dt);
         project(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, stiff, cellSize, cellLength, radius, dt);
     }
     advect(fluids, dt, spaceSize);
@@ -121,12 +124,46 @@ void BasicSPHSolver::diffuseAndSurface(float rho0, float rhoB, float visc, float
     float* dv = reinterpret_cast<float*>(bufferFloat3.addr());
     float* cg = reinterpret_cast<float*>(bufferColorGrad.addr());
     if (!surface) {
+        if (vorticityOn()) vorticity(rho0);
         check(sphk_viscosity(current_.ctx, &current_.abi, dv, rho0, visc, dt), "sphk_viscosity");
         return;
     }
     if (!colorGradReady) check(sphk_color_grad(current_.ctx, &current_.abi, cg, rho0, rhoB), "sphk_color_grad");
+    if (vorticityOn()) {
+        // omega from the velocities the viscosity term reads, in the same sweep
+        check(sphk_fused_viscosity_surface_vorticity(current_.ctx, &current_.abi, dv, cg, rho0, visc, dt, surfaceTensionIntensity,
+                                                     airPressure, omegaBuffer(), omegaNormBuffer()),
+              "sphk_fused_viscosity_surface_vorticity");
+        produced(2, omegaNormBuffer(), 1);
+        return;
+    }
     check(sphk_fused_viscosity_surface(current_.ctx, &current_.abi, dv, cg, rho0, visc, dt, surfaceTensionIntensity, airPressure),
           "sphk_fused_viscosity_surface");
+}
+
+// addition (no reference counterpart): vorticity confinement, sphk.h
+void BasicSPHSolver::setVorticityConfinement(float eps) {
+    if (!(eps >= 0.0f)) {
+        printf("setVorticityConfinement: eps must be >= 0 (got %g); the setting is kept at %g\n", eps, vortEps_);
+        return;
+    }
+    if (eps > 0.0f && !omega_) {
+        omega_ = std::make_unique<DArray<float3>>(num_);
+        omegaNorm_ = std::make_unique<DArray<float>>(num_);
+    }
+    if (eps != vortEps_) ++configEpoch_;
+    vortEps_ = eps;
+}
+
+void BasicSPHSolver::vorticity(float rho0) {
+    check(sphk_vorticity(current_.ctx, &current_.abi, omegaBuffer(), omegaNormBuffer(), rho0), "sphk_vorticity");
+    produced(2, omegaNormBuffer(), 1);
+}
+
+void BasicSPHSolver::confine(const std::shared_ptr<SPHParticles>& fluids, float rho0, float dt) {
+    check(sphk_vorticity_confinement(current_.ctx, &current_.abi, omegaBuffer(), omegaNormBuffer(), vortEps_, dt, rho0),
+          "sphk_vorticity_confinement");
+    producedVel(fluids);
 }
 
 // :227-235
@@ -200,12 +237,14 @@ void DFSPHSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shared_
         diffuseAndSurface(rho0, rhoB, visc, dt, surfaceTensionIntensity, airPressure, surface, true);
         producedVel(fluids);
     } else {
+        if (vorticityOn()) vorticity(rho0);
         BasicSPHSolver::diffuse(fluids, cellStartFluid, cellSize, cellLength, rho0, radius, visc, dt);
         producedVel(fluids);
         if (surface)
             handleSurface(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, rhoB, cellSize, cellLength, radius,
                           dt, surfaceTensionIntensity, airPressure);
     }
+    if (vorticityOn()) confine(fluids, rho0, dt);      // after surface, before the density solve
     itDen_ = project(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, cellSize, cellLength, radius, dt,
                      densityErrorThreshold, maxIter);
     advect(fluids, dt, spaceSize);
@@ -337,7 +376,18 @@ void PBDSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shared_pt
     check(sphk_pbd_velocity_from_positions(current_.ctx, &current_.abi, reinterpret_cast<float*>(fluidPosLast.addr()), dt),
           "sphk_pbd_velocity_from_positions");
     const bool surface = surfaceTensionIntensity > EPSILON || airPressure > EPSILON;
-    if (fusedSweeps_ && surface) {
+    if (fusedSweeps_ && vorticityOn()) {
+        // XSPH (+ colour gradient) + vorticity in one sweep, omega from the velocities XSPH reads
+        float* cg = surface ? colorGradBuffer() : nullptr;
+        check(sphk_fused_pbd_xsph_vorticity(current_.ctx, &current_.abi, xSPH_c, rho0, cg, rhoB, omegaBuffer(), omegaNormBuffer()),
+              "sphk_fused_pbd_xsph_vorticity");
+        producedVel(fluids); produced(2, omegaNormBuffer(), 1);
+        if (surface) {
+            produced(0, cg, 3);
+            check(sphk_surface(current_.ctx, &current_.abi, cg, dt, rho0, surfaceTensionIntensity, airPressure), "sphk_surface");
+            producedVel(fluids);
+        }
+    } else if (fusedSweeps_ && surface) {
         // XSPH + colour gradient in one sweep (positions are final after the projection), then the surface sweep
         float* cg = colorGradBuffer();
         check(sphk_fused_pbd_xsph_color_grad(current_.ctx, &current_.abi, xSPH_c, rho0, cg, rhoB), "sphk_fused_pbd_xsph_color_grad");
@@ -345,12 +395,14 @@ void PBDSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shared_pt
         check(sphk_surface(current_.ctx, &current_.abi, cg, dt, rho0, surfaceTensionIntensity, airPressure), "sphk_surface");
         producedVel(fluids);
     } else {
+        if (vorticityOn()) vorticity(rho0);
         diffuse(fluids, cellStartFluid, cellSize, cellLength, rho0, radius, xSPH_c);
         producedVel(fluids);
         if (surface)
             handleSurface(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, rhoB, cellSize, cellLength, radius,
                           dt, surfaceTensionIntensity, airPressure);
     }
+    if (vorticityOn()) confine(fluids, rho0, dt);      // after XSPH and surface, before gravity
     force(fluids, dt, G);
     predict(fluids, dt, spaceSize);
 }

@@ -169,9 +169,14 @@ protected:
 // ---- BasicSPHSolver.h:20-51 (WCSPH; also the base of DFSPH and PBD) ----------------------------
 class BasicSPHSolver : public BaseSolver {
 public:
-    explicit BasicSPHSolver(int num) : bufferFloat3(num), bufferColorGrad(num) {}
+    explicit BasicSPHSolver(int num) : bufferFloat3(num), bufferColorGrad(num), num_(num) {}
     // addition: false = one kernel per reference launch site (the per-op C-ABI path); true (default) = fused sweeps
     void setFusedSweeps(bool on) { if (on != fusedSweeps_) ++configEpoch_; fusedSweeps_ = on; }
+    // addition: vorticity confinement (sphk_vorticity_confinement) with strength eps in every step; 0 (default) = off, the
+    // reference's step.  Negative or NaN eps is refused (printed, setting kept).  The two buffers it needs are allocated on
+    // the first enable.
+    void setVorticityConfinement(float eps);
+    float vorticityConfinement() const { return vortEps_; }
     // addition: true when step() enqueues the same kernel sequence every call and never synchronises the host.
     // Only the three shipped solver types can say so: a user-derived solver (the reference API allows subclassing
     // BasicSPHSolver) has per-step host logic of its own, so it is never captured into a step graph.
@@ -228,9 +233,20 @@ protected:
     bool beginStep(std::shared_ptr<SPHParticles>& fluids, const std::shared_ptr<SPHParticles>& boundaries,
                    const DArray<int>& cellStartFluid, const DArray<int>& cellStartBoundary, float radius,
                    bool neighborList, int listSkinPermille);
+    // vorticity confinement: on when vortEps_ > 0.  vorticity() forms omega (call it before the viscosity / XSPH sweep reads
+    // the velocities), confine() applies it (after the surface sweep)
+    bool vorticityOn() const { return vortEps_ > 0.0f; }
+    float* omegaBuffer() const { return reinterpret_cast<float*>(omega_->addr()); }
+    float* omegaNormBuffer() const { return omegaNorm_->addr(); }
+    void vorticity(float rho0);
+    void confine(const std::shared_ptr<SPHParticles>& fluids, float rho0, float dt);
 private:
     DArray<float3> bufferFloat3;   // viscosity deltaV, then colour gradient (BasicSPHSolver.h:43)
     DArray<float3> bufferColorGrad;   // addition: the fused viscosity+surface sweep needs both at once
+    const int num_;
+    float vortEps_ = 0.0f;
+    std::unique_ptr<DArray<float3>> omega_;      // vorticity omega
+    std::unique_ptr<DArray<float>> omegaNorm_;   // |omega|, the neighbour scalar of the confinement sweep
 };
 
 // ---- DFSPHSolver.h:20-64 ----------------------------------------------------------------------

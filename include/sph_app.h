@@ -71,6 +71,9 @@ int   sph_app_wait(sph_app* app);
  * reference's host loop with one error sum read back per iteration), 2 = fused sweeps (default on), 3 = step graph. */
 int   sph_app_dfsph_iterations(sph_app* app, int* divergence_iters, int* density_iters);
 int   sph_app_set_option(sph_app* app, int option, int value);
+/* Vorticity confinement of strength eps >= 0 in every following step (BasicSPHSolver::setVorticityConfinement; 0 = off,
+ * the default).  No reference counterpart: returns 1 on the reference build, and for eps < 0 or NaN. */
+int   sph_app_set_vorticity(sph_app* app, float eps);
 /* Name of the engine underneath: "reference-cuda" or "b200-native". */
 const char* sph_app_engine(void);
 

@@ -233,6 +233,31 @@ int sphk_pbd_xsph(sphk_ctx* ctx, const sphk_scene* s, float c, float rho0);
  * masses only, which PBD does not change after its projection) */
 int sphk_fused_pbd_xsph_color_grad(sphk_ctx* ctx, const sphk_scene* s, float c, float rho0, float* color_grad, float rho_boundary);
 
+/* ---- vorticity confinement (no reference counterpart: Macklin & Mueller 2013, section 5; DESIGN.md section 2.2) ----------
+ * Puts back the rotation the discretisation and the viscosity (XSPH, artificial viscosity) smear out.  Fluid neighbours
+ * only, V_j = m_j / rho0, gradW_ij the kernel gradient at x_i - x_j:
+ *   omega_i = sum_j V_j (v_i - v_j) x gradW_ij                  (rigid rotation v = W x x: +2 W in the bulk)
+ *   eta_i   = sum_j V_j (|omega_j| - |omega_i|) gradW_ij,  N_i = eta_i / max(|eta_i|, eps)
+ *   v_i    += dt * eps_conf * (N_i x omega_i)
+ * The class layer forms omega from the velocities its viscosity / XSPH sweep reads and confines right after the surface
+ * sweep (BasicSPHSolver::setVorticityConfinement).  All entries return SPHK_ERR_INVALID for NULL or aliased buffers,
+ * rho0 <= 0, and (confinement) eps_conf < 0 or NaN. */
+/* omega (float3[n]) and omega_norm = |omega| (float[n]).  No reference counterpart. */
+int sphk_vorticity(sphk_ctx* ctx, const sphk_scene* s, float* omega, float* omega_norm, float rho0);
+/* vel += dt * eps * (N x omega) for fluid particles; API array and records.  omega_norm is mirrored into the records
+ * (the neighbour scalar) first.  No reference counterpart. */
+int sphk_vorticity_confinement(sphk_ctx* ctx, const sphk_scene* s, const float* omega, const float* omega_norm, float eps,
+                               float dt, float rho0);
+/* sphk_fused_viscosity_surface + sphk_vorticity in one sweep; omega is formed from the velocities before the viscosity
+ * update, exactly as sphk_vorticity called before sphk_fused_viscosity_surface forms it.  No reference counterpart. */
+int sphk_fused_viscosity_surface_vorticity(sphk_ctx* ctx, const sphk_scene* s, float* delta_v, const float* color_grad,
+                                           float rho0, float visc, float dt, float surface_tension, float air_pressure,
+                                           float* omega, float* omega_norm);
+/* sphk_pbd_xsph (+ the colour gradient of sphk_fused_pbd_xsph_color_grad when color_grad_or_null != NULL) + sphk_vorticity
+ * in one sweep, omega from the velocities before XSPH.  No reference counterpart. */
+int sphk_fused_pbd_xsph_vorticity(sphk_ctx* ctx, const sphk_scene* s, float c, float rho0, float* color_grad_or_null,
+                                  float rho_boundary, float* omega, float* omega_norm);
+
 /* Builds the per-step neighbour list now (sweeps otherwise build it lazily on first use). */
 int sphk_build_neighbor_list(sphk_ctx* ctx, const sphk_scene* s);
 

@@ -1,6 +1,6 @@
 """Multi-rank parity check of the slab driver against a single-GPU run (rank 0 compares and prints a JSON
 verdict).  Launch:  python -m torch.distributed.run --nproc-per-node N --master-addr 127.0.0.1 tools/slab_check.py
-[--backend nccl|gloo] [--scene slabtest] [--solver dfsph] [--steps 3] [--same-gpu]
+[--backend nccl|gloo] [--scene slabtest] [--solver dfsph] [--steps 3] [--same-gpu] [--vorticity EPS]
 --same-gpu puts every rank on cuda:0 (gloo, host-staged halo): lets a 1-GPU box exercise the N>1 path."""
 import argparse, json, os, sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
@@ -24,6 +24,7 @@ ap.add_argument("--skew", type=int, default=0, help="start with the interior cut
 ap.add_argument("--device-scene", action="store_true", help="ranks generate their columns / the boundary shell on the device (no host arrays)")
 ap.add_argument("--bullets", type=int, default=0, help="this many top-layer particles start with a velocity that carries them across "
                 "several cell planes per step (what a violent impact does): exercises the stray routing")
+ap.add_argument("--vorticity", type=float, default=0.0, help="vorticity confinement strength from step 1 on (0: off)")
 a = ap.parse_args()
 rank, world = int(os.environ["RANK"]), int(os.environ["WORLD_SIZE"])
 local = 0 if a.same_gpu else int(os.environ.get("LOCAL_RANK", rank))
@@ -40,6 +41,7 @@ if a.rebalance >= 0:
     os.environ["SPHK_SLAB_REBALANCE"] = str(a.rebalance)
 s = slabs.SlabSystem(sc_ranks, rank, world, torch.device("cuda", local), cut_skew=a.skew)
 cuts0 = list(s.cuts)
+s.vorticity_eps = a.vorticity
 
 
 def shoot(pos, vel):
@@ -83,6 +85,7 @@ s._refresh_ranges()
 dist.all_gather_object(counts, (s.n_gl, s.n_own, s.n_gr, s.cuts))
 if rank == 0:
     ref = engine.SphkSystem(sc, device=torch.device("cuda", local))
+    ref.vorticity_eps = a.vorticity
     if a.bullets:
         assert shoot(ref.fluid.pos[:ref.fluid.n], ref.fluid.vel[:ref.fluid.n]) == a.bullets
     out = {"strays_routed": strays, "world": world, "scene": a.scene, "solver": a.solver, "counts": counts, "steps": [], "cuts_initial": cuts0, "cuts_final": list(s.cuts),
