@@ -9,15 +9,21 @@
 //
 //   sph_headless [--solver sph|dfsph|pbd] [--frames N] [--box L | --box LX LY LZ] [--block NX NY NZ] [--origin X Y Z]
 //                [--dt DT] [--iters K] [--vorticity EPS] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] [--ranks N [--rank R --rendezvous DIR]]
-//                [--bullets K]
+//                [--bullets K] [--stir OMEGA]
 // --vorticity EPS turns on vorticity confinement of strength EPS (BasicSPHSolver::setVorticityConfinement) after the
 // constructor's step 0, for every solver and with --ranks.
-// --emit-scene writes the generated scene (PREFIX.fluid.f32, PREFIX.boundary.f32) and exits: needs no GPU, lets a
-// test compare this generator with the python one the benchmarks use.
+// --stir OMEGA adds one kinematic body (SPHSystem's constructor with a KinematicBody): a flat vertical paddle through the
+// centre of the fluid block, rotating about y at OMEGA rad/s.  It is two layers of the boundary lattice's spacing thick
+// (normal along z), 60 % of the block's x extent wide and as tall as the block; fluid lattice points within one spacing of
+// it are dropped.  Single GPU only.
+// --emit-scene writes the generated scene (PREFIX.fluid.f32, PREFIX.boundary.f32; with --stir also PREFIX.body.f32, the
+// paddle's points in body coordinates, and PREFIX.body_state.f32 = pose {c, q = (x, y, z, w)} + motion {V, Omega}) and
+// exits: needs no GPU, lets a test compare this generator with the python one the benchmarks use, or rebuild the scene.
 // --ranks N runs the same scene on N GPUs through SlabSPHSystem (host/sph_slab.hpp: the class API sharded by x-slabs):
 // without --rank the process forks one child per GPU (rank r on device r) and a fresh rendezvous directory; with
 // --rank R --rendezvous DIR it IS rank R (an external launcher's job).  Every rank dumps the particles it owns
 // (PREFIX.rank<R>.*) and prints its own summary line.
+#include <algorithm>
 #include <cmath>
 #include <cstdio>
 #include <cstdlib>
@@ -57,6 +63,8 @@ struct Options {
     std::string dump, emitScene;
     bool quiet = false;
     float vorticity = 0.0f;                   // --vorticity EPS: vorticity confinement from frame 1 on (0: off)
+    bool stir = false;                        // --stir OMEGA: a paddle rotating about y at OMEGA rad/s
+    float stirOmega = 0.0f;
     int bullets = 0;                          // test aid: this many top-layer particles start at ~3 cell planes per step
     int ranks = 1, rank = -1;                 // --ranks N: SlabSPHSystem on N GPUs; --rank R: this process is rank R
     std::string rendezvous;
@@ -75,6 +83,7 @@ bool parse(int argc, char** argv, Options& o) {
         else if (a == "--quiet") o.quiet = true;
         else if (a == "--bullets" && need(i, 1)) o.bullets = std::atoi(argv[++i]);
         else if (a == "--vorticity" && need(i, 1)) o.vorticity = static_cast<float>(std::atof(argv[++i]));
+        else if (a == "--stir" && need(i, 1)) { o.stir = true; o.stirOmega = static_cast<float>(std::atof(argv[++i])); }
         else if (a == "--ranks" && need(i, 1)) o.ranks = std::atoi(argv[++i]);
         else if (a == "--rank" && need(i, 1)) o.rank = std::atoi(argv[++i]);
         else if (a == "--rendezvous" && need(i, 1)) o.rendezvous = argv[++i];
@@ -94,6 +103,10 @@ bool parse(int argc, char** argv, Options& o) {
         }
     }
     if (o.ranks < 1 || o.rank >= o.ranks || (o.rank >= 0 && o.ranks > 1 && o.rendezvous.empty())) return false;
+    if (o.stir && (o.ranks > 1 || !std::isfinite(o.stirOmega))) {
+        std::fprintf(stderr, "sph_headless: --stir runs on one GPU only (kinematic bodies are not supported with --ranks)\n");
+        return false;
+    }
     return o.frames >= 0 && o.vorticity >= 0.0f && o.block[0] > 0 && o.block[1] > 0 && o.block[2] > 0 &&
            (o.solver == "sph" || o.solver == "wcsph" || o.solver == "dfsph" || o.solver == "pbd");
 }
@@ -126,6 +139,40 @@ std::vector<float3> boundary_shell(const int3 cells, const float3 space) {
     for (int j = 0; j < c.y - 2; ++j)
         for (int k = 0; k < c.z - 2; ++k) { put(0, j + 1, k + 1); put(c.x - 1, j + 1, k + 1); }
     return p;
+}
+
+// --stir: the paddle (body coordinates, centred on the block's centre) and the fluid block without the lattice points
+// within one boundary spacing of it
+sphb200::KinematicBody paddle(const Options& o, float spacing, float boundarySpacing) {
+    sphb200::KinematicBody b;
+    const float sb = boundarySpacing;
+    const float ex = spacing * (o.block[0] - 1), ey = spacing * (o.block[1] - 1);
+    const int nw = std::max(2, static_cast<int>(0.6f * ex / sb) + 1), nh = std::max(2, static_cast<int>(ey / sb) + 1);
+    for (int j = 0; j < nh; ++j)
+        for (int i = 0; i < nw; ++i)
+            for (int k = 0; k < 2; ++k)
+                b.points.push_back(make_float3((i - 0.5f * (nw - 1)) * sb, (j - 0.5f * (nh - 1)) * sb, (k - 0.5f) * sb));
+    b.position = make_float3(o.origin[0] + 0.5f * ex, o.origin[1] + 0.5f * ey, o.origin[2] + 0.5f * spacing * (o.block[2] - 1));
+    b.orientation = make_float4(0.0f, 0.0f, 0.0f, 1.0f);
+    b.linearVelocity = make_float3(0.0f, 0.0f, 0.0f);
+    b.angularVelocity = make_float3(0.0f, o.stirOmega, 0.0f);
+    return b;
+}
+
+std::vector<float3> clear_of(const std::vector<float3>& fluid, const sphb200::KinematicBody& b, float sb) {
+    float3 lo = b.points[0], hi = b.points[0];
+    for (const float3& r : b.points) {
+        lo = make_float3(std::min(lo.x, r.x), std::min(lo.y, r.y), std::min(lo.z, r.z));
+        hi = make_float3(std::max(hi.x, r.x), std::max(hi.y, r.y), std::max(hi.z, r.z));
+    }
+    std::vector<float3> out;
+    for (const float3& p : fluid) {
+        const float dx = p.x - b.position.x, dy = p.y - b.position.y, dz = p.z - b.position.z;   // identity orientation at t = 0
+        const float ox = std::max({lo.x - dx, dx - hi.x, 0.0f}), oy = std::max({lo.y - dy, dy - hi.y, 0.0f}),
+                    oz = std::max({lo.z - dz, dz - hi.z, 0.0f});
+        if (ox * ox + oy * oy + oz * oz >= sb * sb) out.push_back(p);
+    }
+    return out;
 }
 
 std::vector<float> flat(const std::vector<float3>& p) {
@@ -180,7 +227,7 @@ int main(int argc, char** argv) {
     Options o;
     if (!parse(argc, argv, o)) {
         std::fprintf(stderr, "usage: sph_headless [--solver sph|dfsph|pbd] [--frames N] [--box L | LX LY LZ] [--block NX NY NZ] "
-                             "[--origin X Y Z] [--dt DT] [--iters K] [--vorticity EPS] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] "
+                             "[--origin X Y Z] [--dt DT] [--iters K] [--vorticity EPS] [--stir OMEGA] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] "
                              "[--ranks N [--rank R --rendezvous DIR]]\n");
         return 2;
     }
@@ -189,11 +236,28 @@ int main(int argc, char** argv) {
     const float sphSpacing = 0.02f;
     const float sphSmoothingRadius = 2.0f * sphSpacing;
     const float sphCellLength = 1.01f * sphSmoothingRadius;
+    const int3 cellSize = make_int3(static_cast<int>(std::ceil(spaceSize.x / sphCellLength)), static_cast<int>(std::ceil(spaceSize.y / sphCellLength)),
+                                    static_cast<int>(std::ceil(spaceSize.z / sphCellLength)));
+    // the boundary shell's lattice spacing along x (boundary_shell: 0.99 * space / (2 * cells - 1))
+    const float boundarySpacing = 0.99f * spaceSize.x / float(2 * cellSize.x - 1);
+    std::vector<sphb200::KinematicBody> bodies;
+    std::vector<float3> fluidPoints = fluid_block(o, sphSpacing);
+    if (o.stir) {
+        bodies.push_back(paddle(o, sphSpacing, boundarySpacing));
+        fluidPoints = clear_of(fluidPoints, bodies[0], boundarySpacing);
+    }
     if (!o.emitScene.empty()) {
-        const int3 cells = make_int3(static_cast<int>(std::ceil(spaceSize.x / sphCellLength)), static_cast<int>(std::ceil(spaceSize.y / sphCellLength)),
-                                     static_cast<int>(std::ceil(spaceSize.z / sphCellLength)));
-        const bool ok = write_floats(o.emitScene + ".fluid.f32", flat(fluid_block(o, sphSpacing))) &&
-                        write_floats(o.emitScene + ".boundary.f32", flat(boundary_shell(cells, spaceSize)));
+        const int3 cells = cellSize;
+        bool ok = write_floats(o.emitScene + ".fluid.f32", flat(fluidPoints)) &&
+                  write_floats(o.emitScene + ".boundary.f32", flat(boundary_shell(cells, spaceSize)));
+        if (ok && o.stir) {
+            const auto& b = bodies[0];
+            ok = write_floats(o.emitScene + ".body.f32", flat(b.points)) &&
+                 write_floats(o.emitScene + ".body_state.f32",
+                              {b.position.x, b.position.y, b.position.z, b.orientation.x, b.orientation.y, b.orientation.z, b.orientation.w,
+                               b.linearVelocity.x, b.linearVelocity.y, b.linearVelocity.z, b.angularVelocity.x, b.angularVelocity.y,
+                               b.angularVelocity.z});
+        }
         std::printf("{\"cells\": [%d, %d, %d]}\n", cells.x, cells.y, cells.z);
         return ok ? 0 : 5;
     }
@@ -251,11 +315,9 @@ int main(int argc, char** argv) {
     const float sphVisc = 5e-4f;
     const float sphSurfaceTensionIntensity = 0.0001f;
     const float sphAirPressure = 0.0001f;
-    const int3 cellSize = make_int3(static_cast<int>(std::ceil(spaceSize.x / sphCellLength)), static_cast<int>(std::ceil(spaceSize.y / sphCellLength)),
-                                    static_cast<int>(std::ceil(spaceSize.z / sphCellLength)));
 
     // ---- the reference's call sites: particles (main.cpp:86,117), solver (:119-130), system (:131-134) ----
-    auto fluidParticles = std::make_shared<SPHParticles>(fluid_block(o, sphSpacing));
+    auto fluidParticles = std::make_shared<SPHParticles>(fluidPoints);
     auto boundaryParticles = std::make_shared<SPHParticles>(boundary_shell(cellSize, spaceSize));
     const int nFluid = static_cast<int>(fluidParticles->size()), nBoundary = static_cast<int>(boundaryParticles->size());
     std::shared_ptr<BaseSolver> pSolver;
@@ -275,6 +337,10 @@ int main(int argc, char** argv) {
                                                 dt, sphM0, sphRho0, sphRhoBoundary, sphStiff, sphVisc, sphSurfaceTensionIntensity,
                                                 sphAirPressure, sphG, cellSize, boot);
         if (!pSlab->ok()) { std::fprintf(stderr, "sph_headless: rank %d: SlabSPHSystem did not come up\n", o.rank); return 4; }
+    } else if (o.stir) {
+        pSystem = std::make_shared<SPHSystem>(fluidParticles, boundaryParticles, pSolver, spaceSize, sphCellLength, sphSmoothingRadius,
+                                              dt, sphM0, sphRho0, sphRhoBoundary, sphStiff, sphVisc, sphSurfaceTensionIntensity,
+                                              sphAirPressure, sphG, cellSize, bodies);
     } else {
         pSystem = std::make_shared<SPHSystem>(fluidParticles, boundaryParticles, pSolver, spaceSize, sphCellLength, sphSmoothingRadius,
                                               dt, sphM0, sphRho0, sphRhoBoundary, sphStiff, sphVisc, sphSurfaceTensionIntensity,

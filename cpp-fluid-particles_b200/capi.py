@@ -30,11 +30,13 @@ SPHK_FUNCTIONS = [
     "sphk_mg_unique_id", "sphk_mg_init", "sphk_mg_destroy", "sphk_mg_ipc_handle", "sphk_mg_ipc_connect", "sphk_mg_set_transport",
     "sphk_mg_exchange_ints", "sphk_mg_exchange_ints_async", "sphk_mg_plane_ranges", "sphk_mg_halo_device", "sphk_mg_check_async", "sphk_set_active_range_device", "sphk_mg_allreduce_sum", "sphk_mg_exchange_slices", "sphk_mg_halo", "sphk_mg_check", "sphk_mg_stats",
     "sphk_strays_block_floats", "sphk_strays_collect", "sphk_strays_append", "sphk_mg_strays_route", "sphk_strays_counts",
+    "sphk_bodies_init", "sphk_bodies_set_motion", "sphk_bodies_step", "sphk_bodies_get_pose", "sphk_bodies_get_local",
 ]
 SPH_APP_FUNCTIONS = [
     "sph_app_create", "sph_app_destroy", "sph_app_step", "sph_app_fluid_size", "sph_app_boundary_size",
     "sph_app_download_fluid", "sph_app_download_boundary", "sph_app_upload_fluid", "sph_app_engine",
     "sph_app_submit", "sph_app_wait", "sph_app_dfsph_iterations", "sph_app_set_option", "sph_app_set_vorticity",
+    "sph_app_create_with_bodies", "sph_app_set_body_motion", "sph_app_body_pose", "sph_app_step_graph_active",
 ]
 
 OPT_NEIGHBOR_LIST, OPT_LIST_CAPACITY, OPT_LIST_SKIN, OPT_SIMPLE_LIST_BUILD, OPT_TILE, OPT_STAGED_LIST_BUILD, OPT_PATCH = 1, 2, 5, 6, 9, 10, 11
@@ -100,6 +102,7 @@ def app_lib(path: str = LIBHOST):
             sphk()
         L = _load(path)
         L.sph_app_create.restype = C.c_void_p
+        L.sph_app_create_with_bodies.restype = C.c_void_p
         L.sph_app_step.restype = C.c_float
         L.sph_app_engine.restype = C.c_char_p
         L.sph_app_destroy.restype = None
@@ -133,15 +136,29 @@ class SphApp:
     `lib_path` selects the engine underneath: this repo's libsphhost.so (default) or the reference's own
     CUDA build oracle/_ref/libsphref.so -- the facade source is the same file for both."""
 
-    def __init__(self, scene, lib_path: str = LIBHOST):
+    def __init__(self, scene, lib_path: str = LIBHOST, bodies=None):
+        """bodies: kinematic rigid bodies in engine.SphkSystem's format (sph_app_create_with_bodies); their particles follow
+        the static boundary set, so nB counts them."""
         self.L = app_lib(lib_path)
         self.scene = scene
         fl = np.ascontiguousarray(scene.fluid, np.float32)
         bd = np.ascontiguousarray(scene.boundary, np.float32)
         self.nF, self.nB = fl.shape[0], bd.shape[0]
         prm = app_params(scene.params)
-        self.h = self.L.sph_app_create(fl.ctypes.data_as(C.c_void_p), C.c_int(self.nF), bd.ctypes.data_as(C.c_void_p),
-                                       C.c_int(self.nB), C.byref(prm))
+        if bodies is not None:       # (an empty list: the bodies constructor without bodies)
+            pts = [np.asarray(b["points"], np.float32).reshape(-1, 3) for b in bodies]
+            xyz = np.ascontiguousarray(np.concatenate(pts, 0) if pts else np.zeros((0, 3), np.float32))
+            begin = np.ascontiguousarray(np.concatenate([[0], np.cumsum([len(q) for q in pts])]).astype(np.int32))
+            pose = np.ascontiguousarray([[*b["position"], *b["orientation"]] for b in bodies], np.float32).reshape(-1, 7)
+            motion = np.ascontiguousarray([[*b["linear_velocity"], *b["angular_velocity"]] for b in bodies], np.float32).reshape(-1, 6)
+            self.nB += xyz.shape[0]
+            self.h = self.L.sph_app_create_with_bodies(fl.ctypes.data_as(C.c_void_p), C.c_int(self.nF), bd.ctypes.data_as(C.c_void_p),
+                                                       C.c_int(bd.shape[0]), C.c_int(len(bodies)), begin.ctypes.data_as(C.c_void_p),
+                                                       xyz.ctypes.data_as(C.c_void_p), pose.ctypes.data_as(C.c_void_p),
+                                                       motion.ctypes.data_as(C.c_void_p), C.byref(prm))
+        else:
+            self.h = self.L.sph_app_create(fl.ctypes.data_as(C.c_void_p), C.c_int(self.nF), bd.ctypes.data_as(C.c_void_p),
+                                           C.c_int(self.nB), C.byref(prm))
         if not self.h:
             raise RuntimeError("sph_app_create failed (no CUDA device? there is no CPU fallback)")
         self.h = C.c_void_p(self.h)
@@ -212,6 +229,24 @@ class SphApp:
         """Vorticity confinement of strength eps in every following step (0: off).  Not on the reference engine."""
         if self.L.sph_app_set_vorticity(self.h, C.c_float(eps)):
             raise RuntimeError("sph_app_set_vorticity failed (reference engine, or eps < 0)")
+
+    def set_body_motion(self, body: int, linear_velocity, angular_velocity):
+        """New motion of one kinematic body from the next step on.  Not on the reference engine."""
+        v = np.ascontiguousarray(linear_velocity, np.float32)
+        w = np.ascontiguousarray(angular_velocity, np.float32)
+        if self.L.sph_app_set_body_motion(self.h, C.c_int(body), v.ctypes.data_as(C.c_void_p), w.ctypes.data_as(C.c_void_p)):
+            raise RuntimeError("sph_app_set_body_motion failed (reference engine, bad index or non-finite motion)")
+
+    def step_graph_active(self) -> bool:
+        """True when the next step replays a captured step graph (this repository's engine only)."""
+        return int(self.L.sph_app_step_graph_active(self.h)) == 1
+
+    def body_pose(self, body: int) -> np.ndarray:
+        """{cx, cy, cz, qx, qy, qz, qw} of one kinematic body."""
+        out = np.zeros(7, np.float32)
+        if self.L.sph_app_body_pose(self.h, C.c_int(body), out.ctypes.data_as(C.c_void_p)):
+            raise RuntimeError("sph_app_body_pose failed (reference engine or bad index)")
+        return out
 
     def close(self):
         if getattr(self, "h", None):

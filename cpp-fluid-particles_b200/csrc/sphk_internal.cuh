@@ -10,6 +10,7 @@
 #define SPHK_BLOCK 128
 #define SPHK_TILE_CAP 1535                      // records of a tile's staged neighbour windows (+1 dummy slot = 24 KiB per half)
 #define SPHK_TILE_WINS 18                       // 9 (dx,dy) rows of the fluid set + 9 of the boundary set
+#define SPHK_MAX_BODIES 64                      // kinematic bodies per context (sphk_bodies_init)
 
 // Packed particle records, two 16-byte halves in two arrays (unified index: fluid j < capF, boundary capF + b,
 // one far-away zero-mass dummy at capF + capB used as list padding):
@@ -50,6 +51,21 @@ struct LoopState {
     float total;       // last error sum (FLT_MAX before the first reduction)
     int pad;
 };
+
+// Kinematic rigid bodies (sphk_bodies_*, sphk_search.cu): boundary slots [nStatic, nB) of the PRE-search order belong
+// to bodies.  local[] runs parallel to the boundary API arrays (it is permuted with them by every boundary search):
+// {r_k (body coordinates), group} with group 0 = the static set, b + 1 = body b.
+struct BodyState {
+    int nBodies = 0, nStatic = 0, n = 0;   // n: size of the boundary set (static + bodies)
+    float* pose = nullptr;           // device [7 * nBodies]: c.xyz, q.xyzw
+    float* motion = nullptr;         // device [6 * nBodies]: V.xyz, Omega.xyz (world frame)
+    float4* local = nullptr;         // device [capB]
+    float4* snapLocal = nullptr;     // device [capB]: pre-sort snapshot of local (the gather permutes out of place)
+    float* snapMass = nullptr;       // device [capB]: pre-sort snapshot of the boundary mass
+    float* stage = nullptr;          // pinned [6 * SPHK_MAX_BODIES]: staging of sphk_bodies_set_motion
+    cudaEvent_t staged = nullptr;    // the copy out of `stage` has been done
+};
+__device__ __forceinline__ float body_group(float4 local) { return local.w; }
 
 struct sphk_ctx {
     cudaStream_t stream = nullptr;
@@ -101,6 +117,7 @@ struct sphk_ctx {
     bool fluidSearched = false, boundarySearched = false, permValid = false;
     const int* lastCsB = nullptr;
     long long launches = 0;
+    BodyState* bodies = nullptr;     // non-null after sphk_bodies_init
 };
 
 struct DevScene {

@@ -15,9 +15,16 @@
 // HBM-bound; algorithmic bytes per particle are listed in DESIGN.md.
 #include <cub/device/device_radix_sort.cuh>
 #include <cstdio>
+#include <cmath>
 #include <cstdlib>
+#include <cstring>
 #include <new>
+#include <vector>
 #include "sphk_internal.cuh"
+
+// kinematic bodies (end of this file)
+static void sphk_bodies_release(BodyState* b);
+static int sphk_bodies_search(sphk_ctx* c, const sphk_particles* p, int* cell_start);
 
 // ------------------------------------------------------------------------------------------------
 __global__ void __launch_bounds__(SPHK_BLOCK)
@@ -94,14 +101,15 @@ k_permute(const int* __restrict__ idxSorted, const float* __restrict__ src, floa
 
 __global__ void __launch_bounds__(SPHK_BLOCK)
 k_repack(const float* __restrict__ pos, const float* __restrict__ vel, const float* __restrict__ mass,
-         int n, Rec rec, int isFluid, unsigned int* __restrict__ massRange) {
+         int n, Rec rec, int isFluid, unsigned int* __restrict__ massRange, const float4* __restrict__ bodyLocal) {
     const int i = blockIdx.x * SPHK_BLOCK + threadIdx.x;
     float m = 0.f;
     if (i < n) {
         const float3 p = load3(pos, i);
         m = mass[i];
         float4 v = make_float4(0.f, 0.f, 0.f, m);
-        if (vel) { const float3 w = load3(vel, i); v = make_float4(w.x, w.y, w.z, m); }
+        // boundary records with bodies: body particles keep their velocity, the static set keeps zero
+        if (vel && (!bodyLocal || body_group(bodyLocal[i]) != 0.f)) { const float3 w = load3(vel, i); v = make_float4(w.x, w.y, w.z, m); }
         rec_store(rec + i, make_float4(p.x, p.y, p.z, isFluid ? 0.f : m), v);
     }
     if (massRange) {
@@ -235,6 +243,7 @@ extern "C" void sphk_destroy(sphk_ctx* c) {
     cudaFree(c->snapA); cudaFree(c->snapB); cudaFree(c->rec.a); cudaFree(c->rec.b); cudaFree(c->massRange); cudaFree(c->dispMax); cudaFree(c->cellFlag);
     cudaFree(c->tmpF); cudaFree(c->partial); cudaFree(c->loops); cudaFree(c->cnt); cudaFree(c->nbr); cudaFree(c->cubTemp); cudaFree(c->tileWin);
     if (c->pinned) cudaFreeHost(c->pinned);
+    sphk_bodies_release(c->bodies);
     delete c;
 }
 
@@ -327,6 +336,7 @@ extern "C" int sphk_neighbor_search(sphk_ctx* c, int which, const sphk_particles
     if (fluid && !p->vel) return SPHK_ERR_INVALID;
     const int n = p->n;
     if (n > (fluid ? c->capF : c->capB)) return SPHK_ERR_CAPACITY;
+    if (!fluid && c->bodies) return sphk_bodies_search(c, p, cell_start);   // carries mass and body frame along
     const int off = fluid ? 0 : c->capF;
     cudaStream_t st = c->stream;
     k_hash_snapshot<<<sphk_blocks(n), SPHK_BLOCK, 0, st>>>(p->pos, p->vel, n, c->cellLength, c->cs, c->org, p->particle2cell,
@@ -362,14 +372,15 @@ extern "C" int sphk_refresh(sphk_ctx* c, const sphk_scene* s) {
     if (!c->fluidSearched || s->fluid.n != c->nF) return SPHK_ERR_STATE;
     k_init_mass_range<<<1, 1, 0, c->stream>>>(reinterpret_cast<unsigned int*>(c->massRange));
     k_repack<<<sphk_blocks(c->nF), SPHK_BLOCK, 0, c->stream>>>(s->fluid.pos, s->fluid.vel, s->fluid.mass, c->nF, c->rec, 1,
-                                                              reinterpret_cast<unsigned int*>(c->massRange));
+                                                              reinterpret_cast<unsigned int*>(c->massRange), nullptr);
     c->launches++;
     c->posDirty = true;
     c->advected = true;
     c->sTag = nullptr;
     if (c->boundarySearched && s->boundary.pos && s->boundary.n == c->nB) {
-        k_repack<<<sphk_blocks(c->nB), SPHK_BLOCK, 0, c->stream>>>(s->boundary.pos, nullptr, s->boundary.mass, c->nB,
-                                                                  c->rec + c->capF, 0, nullptr);
+        const float4* local = c->bodies ? c->bodies->local : nullptr;
+        k_repack<<<sphk_blocks(c->nB), SPHK_BLOCK, 0, c->stream>>>(s->boundary.pos, local ? s->boundary.vel : nullptr,
+                                                                  s->boundary.mass, c->nB, c->rec + c->capF, 0, nullptr, local);
         c->launches++;
     }
     SPHK_CUDA_TRY(cudaGetLastError());
@@ -615,5 +626,212 @@ extern "C" int sphk_get_permutation(sphk_ctx* c, int* perm_out, int n) {
     if (!c || !perm_out) return SPHK_ERR_INVALID;
     if (!c->permValid || n != c->nF) return SPHK_ERR_STATE;
     SPHK_CUDA_TRY(cudaMemcpyAsync(perm_out, c->idxSorted, sizeof(int) * static_cast<size_t>(n), cudaMemcpyDeviceToDevice, c->stream));
+    return SPHK_OK;
+}
+
+// ---- kinematic rigid bodies (no reference counterpart; DESIGN.md section 2.3) ------------------------------------------
+// A body is a rigid set of boundary particles given in body coordinates r_k, with pose {c, q} and motion {V, Omega} (world
+// frame) in device memory.  Per step (sphk_bodies_step, before the fluid search):
+//   c <- c + dt V;  q <- normalize(dq (x) q), dq = (sin(|Omega| dt / 2) Omega / |Omega|, cos(|Omega| dt / 2))
+//   x_k = c + R(q) r_k,  v_k = V + Omega x (x_k - c)
+// then the boundary set is searched again.  Every boundary search of a context with bodies carries the mass and the
+// {r_k, group} of each particle with it (the reference leaves boundary masses in place, Q2: they are computed once, after
+// the one search) and keeps the body velocities in the records; the static set keeps v = 0.
+
+// One thread per body.  The update is evaluated in double from the float pose and rounded once: with -use_fast_math the
+// float sin / cos would be the approximate intrinsics.
+__global__ void k_bodies_pose(float* __restrict__ pose, const float* __restrict__ motion, int nBodies, float dt) {
+    const int b = blockIdx.x * blockDim.x + threadIdx.x;
+    if (b >= nBodies) return;
+    float* P = pose + 7 * b;
+    const float* M = motion + 6 * b;
+    for (int a = 0; a < 3; ++a) P[a] = __fadd_rn(P[a], __fmul_rn(dt, M[a]));
+    const double wx = M[3], wy = M[4], wz = M[5];
+    const double w = sqrt(wx * wx + wy * wy + wz * wz);
+    if (w == 0.0) return;                                   // dq = identity: q stays bit for bit
+    const double h = 0.5 * w * static_cast<double>(dt), s = sin(h) / w;
+    const double dx = s * wx, dy = s * wy, dz = s * wz, dw = cos(h);
+    const double qx = P[3], qy = P[4], qz = P[5], qw = P[6];
+    // Hamilton product dq (x) q: (dw qv + qw dv + dv x qv, dw qw - dv . qv)
+    double rx = dw * qx + qw * dx + (dy * qz - dz * qy);
+    double ry = dw * qy + qw * dy + (dz * qx - dx * qz);
+    double rz = dw * qz + qw * dz + (dx * qy - dy * qx);
+    double rw = dw * qw - (dx * qx + dy * qy + dz * qz);
+    const double inv = 1.0 / sqrt(rx * rx + ry * ry + rz * rz + rw * rw);
+    P[3] = static_cast<float>(rx * inv); P[4] = static_cast<float>(ry * inv);
+    P[5] = static_cast<float>(rz * inv); P[6] = static_cast<float>(rw * inv);
+}
+
+// Places the body particles at their pose (pos and vel of the boundary API arrays; static particles are left alone) and
+// snapshots mass and {r_k, group} for the gather, which permutes them out of place.
+__global__ void __launch_bounds__(SPHK_BLOCK)
+k_bodies_place(const float4* __restrict__ local, const float* __restrict__ pose, const float* __restrict__ motion,
+               const float* __restrict__ mass, int n, float* __restrict__ pos, float* __restrict__ vel,
+               float4* __restrict__ snapLocal, float* __restrict__ snapMass) {
+    const int i = blockIdx.x * SPHK_BLOCK + threadIdx.x;
+    if (i >= n) return;
+    const float4 l = local[i];
+    snapLocal[i] = l;
+    snapMass[i] = mass[i];
+    const int g = static_cast<int>(body_group(l));
+    if (g == 0) return;
+    const float* P = pose + 7 * (g - 1);
+    const float* M = motion + 6 * (g - 1);
+    const float3 c = f3(P[0], P[1], P[2]), qv = f3(P[3], P[4], P[5]), r = xyz(l);
+    const float qw = P[6];
+    // R(q) r = r + qw t + qv x t, t = 2 qv x r (exactly r for the identity)
+    const float3 t = f3(2.f * (qv.y * r.z - qv.z * r.y), 2.f * (qv.z * r.x - qv.x * r.z), 2.f * (qv.x * r.y - qv.y * r.x));
+    const float3 rr = f3(r.x + qw * t.x + (qv.y * t.z - qv.z * t.y), r.y + qw * t.y + (qv.z * t.x - qv.x * t.z),
+                         r.z + qw * t.z + (qv.x * t.y - qv.y * t.x));
+    const float3 x = c + rr;
+    const float3 d = x - c, W = f3(M[3], M[4], M[5]);
+    const float3 v = f3(M[0] + (W.y * d.z - W.z * d.y), M[1] + (W.z * d.x - W.x * d.z), M[2] + (W.x * d.y - W.y * d.x));
+    store3(pos, i, x);
+    store3(vel, i, v);
+}
+
+// The boundary gather of a context with bodies: sorted pos / vel, mass and {r_k, group} permuted along, records with the
+// body velocities (static records: v = 0)
+__global__ void __launch_bounds__(SPHK_BLOCK)
+k_bodies_gather(const int* __restrict__ idxSorted, const float4* __restrict__ snapPos, const float4* __restrict__ snapVel,
+                const float* __restrict__ snapMass, const float4* __restrict__ snapLocal, int n, float* __restrict__ pos,
+                float* __restrict__ vel, float* __restrict__ mass, float4* __restrict__ local, Rec rec) {
+    const int s = blockIdx.x * SPHK_BLOCK + threadIdx.x;
+    if (s >= n) return;
+    const int src = idxSorted[s];
+    float4 p = snapPos[src], v = snapVel[src];
+    const float4 l = snapLocal[src];
+    const float m = snapMass[src];
+    store3(pos, s, xyz(p));
+    store3(vel, s, xyz(v));
+    mass[s] = m;
+    local[s] = l;
+    if (body_group(l) == 0.f) v = make_float4(0.f, 0.f, 0.f, 0.f);
+    v.w = m;
+    p.w = m;
+    rec_store(rec + s, p, v);
+}
+
+static void sphk_bodies_release(BodyState* b) {
+    if (!b) return;
+    cudaFree(b->pose); cudaFree(b->motion); cudaFree(b->local); cudaFree(b->snapLocal); cudaFree(b->snapMass);
+    if (b->stage) cudaFreeHost(b->stage);
+    if (b->staged) cudaEventDestroy(b->staged);
+    delete b;
+}
+
+static int sphk_bodies_search(sphk_ctx* c, const sphk_particles* p, int* cell_start) {
+    BodyState* B = c->bodies;
+    const int n = p->n;
+    if (!p->vel || n != B->n) return SPHK_ERR_INVALID;      // the set declared by sphk_bodies_init
+    cudaStream_t st = c->stream;
+    k_bodies_place<<<sphk_blocks(n), SPHK_BLOCK, 0, st>>>(B->local, B->pose, B->motion, p->mass, n, p->pos, p->vel,
+                                                         B->snapLocal, B->snapMass);
+    k_hash_snapshot<<<sphk_blocks(n), SPHK_BLOCK, 0, st>>>(p->pos, p->vel, n, c->cellLength, c->cs, c->org, p->particle2cell,
+                                                          c->keys, c->idx, c->snapA, c->snapB);
+    size_t tb = c->cubTempBytes;
+    SPHK_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->cubTemp, tb, c->keys, c->keysSorted, c->idx, c->idxSorted, n, 0,
+                                                  c->endBit, st));
+    k_bodies_gather<<<sphk_blocks(n), SPHK_BLOCK, 0, st>>>(c->idxSorted, c->snapA, c->snapB, B->snapMass, B->snapLocal, n,
+                                                          p->pos, p->vel, p->mass, B->local, c->rec + c->capF);
+    k_cell_start<<<sphk_blocks(c->ncells + 1), SPHK_BLOCK, 0, st>>>(c->keysSorted, n, c->ncells, cell_start);
+    c->launches += 4 + 4;
+    c->nB = n; c->boundarySearched = true; c->listEpoch = ~0ull; c->permValid = false;
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+static bool all_finite(const float* x, int n) {
+    for (int i = 0; i < n; ++i)
+        if (!(x[i] - x[i] == 0.f)) return false;
+    return true;
+}
+
+extern "C" int sphk_bodies_init(sphk_ctx* c, const sphk_particles* boundary, int n_static, int n_bodies, const int* body_begin,
+                                const float* local_xyz, const float* pose, const float* motion) {
+    if (!c || !boundary || !boundary->pos || !boundary->vel || !boundary->mass || !body_begin || !local_xyz || !pose || !motion)
+        return SPHK_ERR_INVALID;
+    const int n = boundary->n;
+    if (n_bodies < 1 || n_bodies > SPHK_MAX_BODIES || n_static < 0 || n > c->capB || body_begin[0] != n_static ||
+        body_begin[n_bodies] != n)
+        return SPHK_ERR_INVALID;
+    for (int b = 0; b < n_bodies; ++b)
+        if (body_begin[b + 1] < body_begin[b]) return SPHK_ERR_INVALID;
+    if (!all_finite(pose, 7 * n_bodies) || !all_finite(motion, 6 * n_bodies) || !all_finite(local_xyz, 3 * (n - n_static)))
+        return SPHK_ERR_INVALID;
+    if (c->bodies || c->boundarySearched) return SPHK_ERR_STATE;   // bodies are declared before the first boundary search
+    std::vector<float4> local(static_cast<size_t>(n), make_float4(0.f, 0.f, 0.f, 0.f));
+    for (int b = 0; b < n_bodies; ++b)
+        for (int k = body_begin[b]; k < body_begin[b + 1]; ++k) {
+            const float* r = local_xyz + 3 * static_cast<size_t>(k - n_static);
+            local[k] = make_float4(r[0], r[1], r[2], static_cast<float>(b + 1));
+        }
+    std::vector<float> q(pose, pose + 7 * n_bodies);
+    for (int b = 0; b < n_bodies; ++b) {                     // unit quaternions (a zero one is refused)
+        float* Q = q.data() + 7 * b + 3;
+        const double l = std::sqrt(double(Q[0]) * Q[0] + double(Q[1]) * Q[1] + double(Q[2]) * Q[2] + double(Q[3]) * Q[3]);
+        if (!(l > 0.0)) return SPHK_ERR_INVALID;
+        if (l != 1.0)
+            for (int a = 0; a < 4; ++a) Q[a] = static_cast<float>(Q[a] / l);
+    }
+    BodyState* B = new (std::nothrow) BodyState;
+    if (!B) return SPHK_ERR_ALLOC;
+    B->nBodies = n_bodies; B->nStatic = n_static; B->n = n;
+    const size_t cap = static_cast<size_t>(c->capB);
+    cudaError_t e = dalloc(&B->pose, 7 * static_cast<size_t>(n_bodies));
+    if (e == cudaSuccess) e = dalloc(&B->motion, 6 * static_cast<size_t>(n_bodies));
+    if (e == cudaSuccess) e = dalloc(&B->local, cap);
+    if (e == cudaSuccess) e = dalloc(&B->snapLocal, cap);
+    if (e == cudaSuccess) e = dalloc(&B->snapMass, cap);
+    if (e == cudaSuccess) e = cudaMallocHost(reinterpret_cast<void**>(&B->stage), sizeof(float) * 6 * SPHK_MAX_BODIES);
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&B->staged, cudaEventDisableTiming);
+    if (e == cudaSuccess) e = cudaMemcpy(B->pose, q.data(), sizeof(float) * q.size(), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(B->motion, motion, sizeof(float) * 6 * n_bodies, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(B->local, local.data(), sizeof(float4) * local.size(), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaEventRecord(B->staged, c->stream);
+    if (e != cudaSuccess) { sphk_bodies_release(B); cudaGetLastError(); return e == cudaErrorMemoryAllocation ? SPHK_ERR_ALLOC : static_cast<int>(e); }
+    c->bodies = B;
+    return SPHK_OK;
+}
+
+extern "C" int sphk_bodies_set_motion(sphk_ctx* c, const float* motion_host) {
+    if (!c || !motion_host) return SPHK_ERR_INVALID;
+    if (!c->bodies) return SPHK_ERR_STATE;
+    BodyState* B = c->bodies;
+    if (!all_finite(motion_host, 6 * B->nBodies)) return SPHK_ERR_INVALID;
+    // the staging buffer is reused: wait until the copy of the previous change has left it (a no-op once the stream got there)
+    SPHK_CUDA_TRY(cudaEventSynchronize(B->staged));
+    std::memcpy(B->stage, motion_host, sizeof(float) * 6 * B->nBodies);
+    SPHK_CUDA_TRY(cudaMemcpyAsync(B->motion, B->stage, sizeof(float) * 6 * B->nBodies, cudaMemcpyHostToDevice, c->stream));
+    SPHK_CUDA_TRY(cudaEventRecord(B->staged, c->stream));
+    return SPHK_OK;
+}
+
+extern "C" int sphk_bodies_step(sphk_ctx* c, const sphk_particles* boundary, int* cell_start_boundary, float dt) {
+    if (!c || !boundary || !cell_start_boundary || !boundary->pos || !boundary->vel || !boundary->mass || !boundary->particle2cell)
+        return SPHK_ERR_INVALID;
+    if (!(dt > 0.f) || !all_finite(&dt, 1)) return SPHK_ERR_INVALID;
+    if (!c->bodies || !c->boundarySearched) return SPHK_ERR_STATE;
+    if (boundary->n != c->nB) return SPHK_ERR_STATE;
+    const BodyState* B = c->bodies;
+    k_bodies_pose<<<1, SPHK_MAX_BODIES, 0, c->stream>>>(B->pose, B->motion, B->nBodies, dt);
+    c->launches++;
+    return sphk_bodies_search(c, boundary, cell_start_boundary);
+}
+
+extern "C" int sphk_bodies_get_pose(sphk_ctx* c, float* pose_host) {
+    if (!c || !pose_host) return SPHK_ERR_INVALID;
+    if (!c->bodies) return SPHK_ERR_STATE;
+    SPHK_CUDA_TRY(cudaMemcpyAsync(pose_host, c->bodies->pose, sizeof(float) * 7 * c->bodies->nBodies, cudaMemcpyDeviceToHost,
+                                  c->stream));
+    SPHK_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    return SPHK_OK;
+}
+
+extern "C" int sphk_bodies_get_local(sphk_ctx* c, float* local_out) {
+    if (!c || !local_out) return SPHK_ERR_INVALID;
+    if (!c->bodies || !c->boundarySearched) return SPHK_ERR_STATE;
+    SPHK_CUDA_TRY(cudaMemcpyAsync(local_out, c->bodies->local, sizeof(float4) * static_cast<size_t>(c->nB), cudaMemcpyDeviceToDevice,
+                                  c->stream));
     return SPHK_OK;
 }

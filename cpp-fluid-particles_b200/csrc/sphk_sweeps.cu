@@ -909,10 +909,12 @@ k_build_list(const DevScene s, int* __restrict__ nbr, int* __restrict__ cnt, flo
 // computeBoundaryMass_CUDA, SPHSystem.cu:79-105: boundary particles against the boundary set only
 __global__ void __launch_bounds__(SPHK_BLOCK)
 k_boundary_mass(Rec recB, float* __restrict__ mass, int n, const int* __restrict__ csB, int3 cs, int3 org,
-                float cellLength, float rhoB, KConst k) {
+                float cellLength, float rhoB, KConst k, const float4* __restrict__ bodyLocal) {
     const int i = blockIdx.x * SPHK_BLOCK + threadIdx.x;
     if (i >= n) return;
     const float4 pi = rec_lo(recB + i);
+    // with kinematic bodies the sum runs over the particle's own group (the static set, or its body): per-group Akinci
+    const float gi = bodyLocal ? body_group(bodyLocal[i]) : 0.f;
     const int cx = cell_coord(pi.x, cellLength) - org.x, cy = cell_coord(pi.y, cellLength) - org.y,
               cz = cell_coord(pi.z, cellLength) - org.z;
     float sum = 0.f;
@@ -921,6 +923,7 @@ k_boundary_mass(Rec recB, float* __restrict__ mass, int n, const int* __restrict
         if (c == cs.x * cs.y * cs.z) continue;
         const int end = csB[c + 1];
         for (int j = csB[c]; j < end; ++j) {
+            if (bodyLocal && body_group(bodyLocal[j]) != gi) continue;
             const float3 d = xyz(pi) - xyz(rec_lo(recB + j));
             sum += w_cubic(sqrtf(dot3(d, d)), k);
         }
@@ -1177,7 +1180,7 @@ extern "C" int sphk_boundary_mass(sphk_ctx* c, const sphk_particles* b, const in
     if (!c->boundarySearched || b->n != c->nB) return SPHK_ERR_STATE;
     const Rec recB = c->rec + c->capF;
     k_boundary_mass<<<sphk_blocks(c->nB), SPHK_BLOCK, 0, c->stream>>>(recB, b->mass, c->nB, csB, c->cs, c->org, c->cellLength, rhoB,
-                                                                     kernel_constants(R));
+                                                                     kernel_constants(R), c->bodies ? c->bodies->local : nullptr);
     k_set_mass<<<sphk_blocks(c->nB), SPHK_BLOCK, 0, c->stream>>>(recB, b->mass, c->nB);
     c->launches += 2;
     c->listEpoch = ~0ull;

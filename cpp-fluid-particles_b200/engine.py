@@ -145,6 +145,31 @@ class SphkOps:
         p = self.boundary.abi()
         check(self.L.sphk_neighbor_search(self.ctx, 1, C.byref(p), _ptr(self.cs_boundary)), "sphk_neighbor_search(b)")
 
+    # ---- kinematic bodies (DESIGN.md section 2.3) -------------------------------------------------------------------------
+    n_bodies = 0
+
+    def bodies_step(self):
+        p = self.boundary.abi()
+        check(self.L.sphk_bodies_step(self.ctx, C.byref(p), _ptr(self.cs_boundary), C.c_float(self.p.dt)), "sphk_bodies_step")
+
+    def set_body_motion(self, body: int, linear_velocity, angular_velocity):
+        """New motion of one body from the next step on (an asynchronous copy, like SPHSystem::setBodyMotion)."""
+        self.body_motion[body] = [*linear_velocity, *angular_velocity]
+        m = np.ascontiguousarray(self.body_motion, np.float32)
+        check(self.L.sphk_bodies_set_motion(self.ctx, m.ctypes.data_as(C.POINTER(C.c_float))), "sphk_bodies_set_motion")
+
+    def body_pose(self) -> np.ndarray:
+        """(n_bodies, 7) poses {c, q = (x, y, z, w)}; synchronises."""
+        out = np.zeros((self.n_bodies, 7), np.float32)
+        check(self.L.sphk_bodies_get_pose(self.ctx, out.ctypes.data_as(C.POINTER(C.c_float))), "sphk_bodies_get_pose")
+        return out
+
+    def body_local(self) -> torch.Tensor:
+        """(n_boundary, 4) carried {r_k, group} in the current boundary order (group 0: static, b + 1: body b)."""
+        out = torch.zeros((self.boundary.n, 4), dtype=torch.float32, device=self.device)
+        check(self.L.sphk_bodies_get_local(self.ctx, _ptr(out)), "sphk_bodies_get_local")
+        return out
+
     def search_fluid(self):
         p = self.fluid.abi()
         check(self.L.sphk_neighbor_search(self.ctx, 0, C.byref(p), _ptr(self.cs_fluid)), "sphk_neighbor_search(f)")
@@ -482,6 +507,8 @@ class SphkOps:
         return True
 
     def step(self):                  # SPHSystem.cu:129-158 (no host sync here; callers time with CUDA events)
+        if self.n_bodies:            # bodies move before the fluid search, as in SPHSystem::step
+            self.bodies_step()
         self.search_fluid()
         if self.use_list:            # (the C++ layer builds the list lazily in the first sweep; same kernel)
             self.set_use_list(True, 150 if self.solver == "pbd" else 0)
@@ -519,7 +546,10 @@ class SphkSystem(SphkOps):
     reference constructor including its implicit first step (Q3)."""
 
     def __init__(self, scene, device="cuda:0", use_list: bool | None = None, list_capacity: int | None = None,
-                 step0: bool = True):
+                 step0: bool = True, bodies=None):
+        """bodies: kinematic rigid bodies (DESIGN.md section 2.3), a list of dicts with "points" (k, 3) body coordinates,
+        "position" (3,), "orientation" (x, y, z, w) unit quaternion, "linear_velocity" (3,), "angular_velocity" (3,) in the
+        world frame.  Their particles follow the static boundary set; every step() moves them before the fluid search."""
         self.L = capi.sphk()
         self.p = scene.params
         self.device = torch.device(device)
@@ -531,6 +561,18 @@ class SphkSystem(SphkOps):
         else:
             self.fluid = ParticleSet(scene.fluid, self.device)
             self.boundary = ParticleSet(scene.boundary, self.device)
+        bodies = list(bodies or [])
+        self.n_bodies = len(bodies)
+        if bodies:                   # static set + the bodies' particles (placed by the first boundary search)
+            n_static = self.boundary.n
+            pts = [np.asarray(b["points"], np.float32).reshape(-1, 3) for b in bodies]
+            local = torch.from_numpy(np.concatenate(pts, 0)).to(self.device)
+            self.boundary = ParticleSet(torch.cat([self.boundary.pos, local], 0).contiguous(), self.device)
+            begin = np.concatenate([[0], np.cumsum([len(q) for q in pts])]) + n_static
+            self._body_begin = (C.c_int * (self.n_bodies + 1))(*[int(x) for x in begin])
+            self._body_local = np.ascontiguousarray(local.cpu().numpy())
+            self._body_pose = np.array([[*b["position"], *b["orientation"]] for b in bodies], np.float32)
+            self.body_motion = np.array([[*b["linear_velocity"], *b["angular_velocity"]] for b in bodies], np.float32)
         nc = self.p.ncells
         self.cs_fluid = torch.zeros(nc + 1, dtype=torch.int32, device=self.device)
         self.cs_boundary = torch.zeros(nc + 1, dtype=torch.int32, device=self.device)
@@ -549,7 +591,13 @@ class SphkSystem(SphkOps):
         self._scene = None
         self._G = (C.c_float * 3)(*[float(x) for x in self.p.gravity])
         self._space = (C.c_float * 3)(*[float(x) for x in self.p.space])
-        # SPHSystem.cu:68-76
+        if self.n_bodies:
+            p = self.boundary.abi()
+            fp = lambda a: a.ctypes.data_as(C.POINTER(C.c_float))  # noqa: E731
+            check(self.L.sphk_bodies_init(self.ctx, C.byref(p), C.c_int(int(self._body_begin[0])), C.c_int(self.n_bodies),
+                                          self._body_begin, fp(self._body_local), fp(self._body_pose), fp(self.body_motion)),
+                  "sphk_bodies_init")
+        # SPHSystem.cu:68-76 (with bodies the boundary search also places them at their initial pose)
         self.search_boundary()
         self.boundary_mass()
         check(self.L.sphk_fill(self.ctx, _ptr(self.fluid.mass), C.c_int(n), C.c_float(self.p.m0)), "sphk_fill")

@@ -4,6 +4,8 @@
 // construction; :131-134 SPHSystem construction; :302 step; vbo.cu:48 accessor use) and nothing
 // else.  It is deliberately written ONLY against names the reference headers export, so that it
 // builds unchanged on top of either engine (this repo's headers, or /root/reference/src).
+#include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <iostream>
 #include <vector>
@@ -62,9 +64,14 @@ static std::vector<float3> to_float3(const float* xyz, int n) {
     return v;
 }
 
-extern "C" sph_app* sph_app_create(const float* fluid_xyz, int n_fluid,
-                                   const float* boundary_xyz, int n_boundary,
-                                   const sph_app_params* p) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+struct body_list {};
+#else
+using body_list = std::vector<sphb200::KinematicBody>;
+#endif
+
+static sph_app* create(const float* fluid_xyz, int n_fluid, const float* boundary_xyz, int n_boundary, const sph_app_params* p,
+                       const body_list* bodies) {
     if (!fluid_xyz || !boundary_xyz || !p || n_fluid <= 0 || n_boundary <= 0) return nullptr;
     auto fluidParticles = std::make_shared<SPHParticles>(to_float3(fluid_xyz, n_fluid));
     auto boundaryParticles = std::make_shared<SPHParticles>(to_float3(boundary_xyz, n_boundary));
@@ -87,18 +94,87 @@ extern "C" sph_app* sph_app_create(const float* fluid_xyz, int n_fluid,
     }
     auto* app = new sph_app;
     app->solver = pSolver.get();
-    app->system = std::make_shared<SPHSystem>(
-        fluidParticles, boundaryParticles, pSolver,
-        make_float3(p->space[0], p->space[1], p->space[2]), p->cell_length, p->radius, p->dt, p->m0,
-        p->rho0, p->rho_boundary, p->stiff, p->visc, p->surface_tension, p->air_pressure,
-        make_float3(p->gravity[0], p->gravity[1], p->gravity[2]),
-        make_int3(p->cell_size[0], p->cell_size[1], p->cell_size[2]));
+    const float3 space = make_float3(p->space[0], p->space[1], p->space[2]), G = make_float3(p->gravity[0], p->gravity[1], p->gravity[2]);
+    const int3 cells = make_int3(p->cell_size[0], p->cell_size[1], p->cell_size[2]);
+#ifndef SPH_APP_REFERENCE_ENGINE
+    if (bodies)
+        app->system = std::make_shared<SPHSystem>(fluidParticles, boundaryParticles, pSolver, space, p->cell_length, p->radius, p->dt,
+                                                  p->m0, p->rho0, p->rho_boundary, p->stiff, p->visc, p->surface_tension,
+                                                  p->air_pressure, G, cells, *bodies);
+    else
+#endif
+        app->system = std::make_shared<SPHSystem>(fluidParticles, boundaryParticles, pSolver, space, p->cell_length, p->radius, p->dt,
+                                                  p->m0, p->rho0, p->rho_boundary, p->stiff, p->visc, p->surface_tension,
+                                                  p->air_pressure, G, cells);
+    (void)bodies;
     if (cudaDeviceSynchronize() != cudaSuccess) {
         std::fprintf(stderr, "sph_app_create: %s\n", cudaGetErrorString(cudaGetLastError()));
         delete app;
         return nullptr;
     }
     return app;
+}
+
+extern "C" sph_app* sph_app_create(const float* fluid_xyz, int n_fluid, const float* boundary_xyz, int n_boundary,
+                                   const sph_app_params* p) {
+    return create(fluid_xyz, n_fluid, boundary_xyz, n_boundary, p, nullptr);
+}
+
+extern "C" sph_app* sph_app_create_with_bodies(const float* fluid_xyz, int n_fluid, const float* boundary_xyz, int n_boundary,
+                                               int n_bodies, const int* body_begin, const float* body_xyz, const float* pose,
+                                               const float* motion, const sph_app_params* p) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)fluid_xyz; (void)n_fluid; (void)boundary_xyz; (void)n_boundary; (void)n_bodies; (void)body_begin; (void)body_xyz;
+    (void)pose; (void)motion; (void)p;
+    return nullptr;
+#else
+    if (n_bodies < 0 || (n_bodies > 0 && (!body_begin || !body_xyz || !pose || !motion)) || (n_bodies > 0 && body_begin[0] != 0))
+        return nullptr;
+    body_list bodies(static_cast<size_t>(n_bodies));
+    for (int b = 0; b < n_bodies; ++b) {
+        if (body_begin[b + 1] < body_begin[b]) return nullptr;
+        auto& k = bodies[b];
+        k.points = to_float3(body_xyz + 3 * static_cast<size_t>(body_begin[b]), body_begin[b + 1] - body_begin[b]);
+        const float* P = pose + 7 * b;
+        const float* M = motion + 6 * b;
+        k.position = make_float3(P[0], P[1], P[2]);
+        k.orientation = make_float4(P[3], P[4], P[5], P[6]);
+        k.linearVelocity = make_float3(M[0], M[1], M[2]);
+        k.angularVelocity = make_float3(M[3], M[4], M[5]);
+    }
+    sph_app* app = create(fluid_xyz, n_fluid, boundary_xyz, n_boundary, p, &bodies);
+    if (app && app->system->bodyCount() != n_bodies) { delete app; return nullptr; }   // sphk_bodies_init refused them
+    return app;
+#endif
+}
+
+extern "C" int sph_app_set_body_motion(sph_app* app, int body, const float* linear_velocity, const float* angular_velocity) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)body; (void)linear_velocity; (void)angular_velocity;
+    return 1;
+#else
+    if (!app || !linear_velocity || !angular_velocity || body < 0 || body >= app->system->bodyCount()) return 1;
+    for (int a = 0; a < 3; ++a)
+        if (!std::isfinite(linear_velocity[a]) || !std::isfinite(angular_velocity[a])) return 1;
+    app->system->setBodyMotion(body, make_float3(linear_velocity[0], linear_velocity[1], linear_velocity[2]),
+                               make_float3(angular_velocity[0], angular_velocity[1], angular_velocity[2]));
+    return 0;
+#endif
+}
+
+extern "C" int sph_app_body_pose(sph_app* app, int body, float* pose) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)body; (void)pose;
+    return 1;
+#else
+    if (!app || !pose || body < 0 || body >= app->system->bodyCount()) return 1;
+    float3 c;
+    float4 q;
+    app->system->getBodyPose(body, c, q);
+    const float v[7] = {c.x, c.y, c.z, q.x, q.y, q.z, q.w};
+    std::copy(v, v + 7, pose);
+    return 0;
+#endif
 }
 
 extern "C" void sph_app_destroy(sph_app* app) { delete app; }
@@ -257,6 +333,15 @@ extern "C" int sph_app_set_option(sph_app* app, int option, int value) {
     case 3: app->system->setStepGraph(value != 0); return 0;
     default: return 1;
     }
+#endif
+}
+
+extern "C" int sph_app_step_graph_active(sph_app* app) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app;
+    return -1;
+#else
+    return app->system->stepGraphActive() ? 1 : 0;
 #endif
 }
 

@@ -6,6 +6,7 @@
 #include <algorithm>
 #include <cstdlib>
 #include <limits>
+#include <numeric>
 
 using sphb200::check;
 
@@ -453,8 +454,30 @@ SPHSystem::SPHSystem(std::shared_ptr<SPHParticles>& fluidParticles, std::shared_
                      const float sphRhoBoundary, const float sphStiff, const float sphVisc,
                      const float sphSurfaceTensionIntensity, const float sphAirPressure, const float3 sphG,
                      const int3 cellSize)
+    : SPHSystem(fluidParticles, boundaryParticles, solver, spaceSize, sphCellLength, sphSmoothingRadius, dt, sphM0, sphRho0,
+                sphRhoBoundary, sphStiff, sphVisc, sphSurfaceTensionIntensity, sphAirPressure, sphG, cellSize, {}) {}
+
+// the caller's static boundary set followed by the bodies' particles (placed on the host here only to give the arrays a
+// value: the first boundary search places them on the device)
+static std::shared_ptr<SPHParticles> withBodies(std::shared_ptr<SPHParticles>&& boundary,
+                                                const std::vector<sphb200::KinematicBody>& bodies) {
+    if (bodies.empty()) return std::move(boundary);
+    std::vector<float3> all(boundary->size());
+    CUDA_CALL(cudaMemcpy(all.data(), boundary->getPosPtr(), sizeof(float3) * all.size(), cudaMemcpyDeviceToHost));
+    for (const auto& b : bodies)
+        for (const float3& r : b.points) all.push_back(make_float3(b.position.x + r.x, b.position.y + r.y, b.position.z + r.z));
+    boundary.reset();
+    return std::make_shared<SPHParticles>(all);
+}
+
+SPHSystem::SPHSystem(std::shared_ptr<SPHParticles>& fluidParticles, std::shared_ptr<SPHParticles>& boundaryParticles,
+                     std::shared_ptr<BaseSolver>& solver, const float3 spaceSize, const float sphCellLength,
+                     const float sphSmoothingRadius, const float dt, const float sphM0, const float sphRho0,
+                     const float sphRhoBoundary, const float sphStiff, const float sphVisc,
+                     const float sphSurfaceTensionIntensity, const float sphAirPressure, const float3 sphG,
+                     const int3 cellSize, const std::vector<sphb200::KinematicBody>& bodies)
     // the caller's three shared_ptrs are moved from, as in the reference (SPHSystem.cu:50-51)
-    : _fluids(std::move(fluidParticles)), _boundaries(std::move(boundaryParticles)), _solver(std::move(solver)),
+    : _fluids(std::move(fluidParticles)), _boundaries(withBodies(std::move(boundaryParticles), bodies)), _solver(std::move(solver)),
       cellStartFluid(cellSize.x * cellSize.y * cellSize.z + 1), cellStartBoundary(cellSize.x * cellSize.y * cellSize.z + 1),
       _spaceSize(spaceSize), _sphSmoothingRadius(sphSmoothingRadius), _sphCellLength(sphCellLength), _dt(dt),
       _sphRho0(sphRho0), _sphRhoBoundary(sphRhoBoundary), _sphStiff(sphStiff), _sphG(sphG), _sphVisc(sphVisc),
@@ -466,7 +489,26 @@ SPHSystem::SPHSystem(std::shared_ptr<SPHParticles>& fluidParticles, std::shared_
     CUDA_CALL(cudaEventCreate(&_evStop));
     if (const char* g = std::getenv("SPHK_STEP_GRAPH")) _graphEnabled = g[0] != '0';
     if (!_engine->ok()) return;
-    // SPHSystem.cu:68-76
+    if (!bodies.empty()) {
+        const int nStatic = boundarySize() - static_cast<int>(std::accumulate(
+            bodies.begin(), bodies.end(), size_t(0), [](size_t a, const sphb200::KinematicBody& b) { return a + b.points.size(); }));
+        std::vector<int> begin{nStatic};
+        std::vector<float> local, pose, motion;
+        for (const auto& b : bodies) {
+            begin.push_back(begin.back() + static_cast<int>(b.points.size()));
+            for (const float3& r : b.points) local.insert(local.end(), {r.x, r.y, r.z});
+            pose.insert(pose.end(), {b.position.x, b.position.y, b.position.z, b.orientation.x, b.orientation.y, b.orientation.z,
+                                     b.orientation.w});
+            motion.insert(motion.end(), {b.linearVelocity.x, b.linearVelocity.y, b.linearVelocity.z, b.angularVelocity.x,
+                                         b.angularVelocity.y, b.angularVelocity.z});
+        }
+        const sphk_particles bp = _boundaries->abi();
+        const int rc = sphk_bodies_init(_engine->ctx(), &bp, nStatic, static_cast<int>(bodies.size()), begin.data(),
+                                        local.data(), pose.data(), motion.data());
+        check(rc, "sphk_bodies_init");
+        if (rc == 0) _bodyMotion = motion;
+    }
+    // SPHSystem.cu:68-76 (with bodies the boundary search also places them at their initial pose)
     neighborSearch(_boundaries, cellStartBoundary);
     computeBoundaryMass();
     check(sphk_fill(_engine->ctx(), _fluids->getMassPtr(), fluidSize(), sphM0), "sphk_fill");
@@ -496,6 +538,35 @@ void SPHSystem::neighborSearch(const std::shared_ptr<SPHParticles>& particles, D
     // the fluid search re-packs the records from the API arrays: edits made behind the engine's back
     // (Particles::advect, raw pointer writes) are absorbed here, no separate sphk_refresh is needed
     if (which == 0) _engine->shadowsStale = false;
+}
+
+void SPHSystem::searchForStep() {
+    if (!_bodyMotion.empty()) {
+        const sphk_particles b = _boundaries->abi();
+        check(sphk_bodies_step(_engine->ctx(), &b, cellStartBoundary.addr(), _dt), "sphk_bodies_step");
+    }
+    neighborSearch(_fluids, cellStartFluid);
+}
+
+void SPHSystem::setBodyMotion(int body, float3 linearVelocity, float3 angularVelocity) {
+    if (body < 0 || body >= bodyCount()) { printf("setBodyMotion: no body %d (the system has %d)\n", body, bodyCount()); return; }
+    if (!_engine->ok()) return;
+    std::vector<float> motion = _bodyMotion;
+    const float m[6] = {linearVelocity.x, linearVelocity.y, linearVelocity.z, angularVelocity.x, angularVelocity.y, angularVelocity.z};
+    std::copy(m, m + 6, motion.begin() + 6 * body);
+    const int rc = sphk_bodies_set_motion(_engine->ctx(), motion.data());   // refuses non-finite values: the motion is kept
+    check(rc, "sphk_bodies_set_motion");
+    if (rc == 0) _bodyMotion = motion;
+}
+
+void SPHSystem::getBodyPose(int body, float3& position, float4& orientation) const {
+    if (body < 0 || body >= bodyCount()) { printf("getBodyPose: no body %d (the system has %d)\n", body, bodyCount()); return; }
+    std::vector<float> pose(7 * static_cast<size_t>(bodyCount()));
+    if (!_engine->ok()) return;
+    check(sphk_bodies_get_pose(_engine->ctx(), pose.data()), "sphk_bodies_get_pose");
+    const float* P = pose.data() + 7 * body;
+    position = make_float3(P[0], P[1], P[2]);
+    orientation = make_float4(P[3], P[4], P[5], P[6]);
 }
 
 // SPHSystem.cu:129-158
@@ -545,7 +616,7 @@ float SPHSystem::step() {
         if (capture) captured = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
         bool ok = false;
         try {
-            neighborSearch(_fluids, cellStartFluid);
+            searchForStep();
             _solver->step(_fluids, _boundaries, cellStartFluid, cellStartBoundary, _spaceSize, _cellSize, _sphCellLength,
                           _sphSmoothingRadius, _dt, _sphRho0, _sphRhoBoundary, _sphStiff, _sphVisc, _sphG,
                           _sphSurfaceTensionIntensity, _sphAirPressure);
@@ -567,7 +638,7 @@ float SPHSystem::step() {
                 _graphExec = nullptr;
                 _graphEnabled = false;                          // capture refused (e.g. a library call): stay on plain launches
                 printf("SPHSystem: step graph capture failed, continuing with plain launches\n");
-                neighborSearch(_fluids, cellStartFluid);
+                searchForStep();
                 try {
                     _solver->step(_fluids, _boundaries, cellStartFluid, cellStartBoundary, _spaceSize, _cellSize,
                                   _sphCellLength, _sphSmoothingRadius, _dt, _sphRho0, _sphRhoBoundary, _sphStiff, _sphVisc,

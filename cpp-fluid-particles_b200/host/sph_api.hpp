@@ -65,6 +65,16 @@ private:
     sphk_ctx* ctx_ = nullptr;
     cudaStream_t stream_ = nullptr;
 };
+
+// addition: a kinematic rigid body (DESIGN.md section 2.3).  Its boundary particles are `points` in body coordinates; the
+// system moves them every step by the prescribed motion (the fluid pushes back on nothing: one-way coupling).
+struct KinematicBody {
+    std::vector<float3> points;     // r_k, body coordinates
+    float3 position;                // centre c, world frame
+    float4 orientation;             // unit quaternion q = (x, y, z, w): vector part in x, y, z, scalar part in w
+    float3 linearVelocity;          // V, world frame
+    float3 angularVelocity;         // Omega (rad/s), world frame, about the centre
+};
 }  // namespace sphb200
 
 // ---- DArray.h:21-54 ---------------------------------------------------------------------------
@@ -344,6 +354,15 @@ public:
               std::shared_ptr<BaseSolver>& solver, float3 spaceSize, float sphCellLength, float sphSmoothingRadius,
               float dt, float sphM0, float sphRho0, float sphRhoBoundary, float sphStiff, float sphVisc,
               float sphSurfaceTensionIntensity, float sphAirPressure, float3 sphG, int3 cellSize);
+    // addition: the same system with kinematic rigid bodies.  The boundary set becomes the caller's (static) boundary
+    // particles followed by the bodies' particles, in the order given: getBoundaries() and boundarySize() include the body
+    // particles.  Every step() moves the bodies (pose update, placement, boundary search) before the fluid search.  An empty
+    // vector is the constructor above.
+    SPHSystem(std::shared_ptr<SPHParticles>& fluidParticles, std::shared_ptr<SPHParticles>& boundaryParticles,
+              std::shared_ptr<BaseSolver>& solver, float3 spaceSize, float sphCellLength, float sphSmoothingRadius,
+              float dt, float sphM0, float sphRho0, float sphRhoBoundary, float sphStiff, float sphVisc,
+              float sphSurfaceTensionIntensity, float sphAirPressure, float3 sphG, int3 cellSize,
+              const std::vector<sphb200::KinematicBody>& bodies);
     SPHSystem(const SPHSystem&) = delete;
     SPHSystem& operator=(const SPHSystem&) = delete;
     ~SPHSystem() noexcept;
@@ -362,6 +381,12 @@ public:
     const DArray<int>& getCellStartBoundary() const { return cellStartBoundary; }
     const std::shared_ptr<sphb200::Engine>& engine() const { return _engine; }
     void setStepGraph(bool on);   // replay each step as one CUDA graph when the solver allows it (default on)
+    bool stepGraphActive() const { return _graphExec != nullptr; }   // the next step replays a captured graph
+    // kinematic bodies: a new motion takes effect at the next step() (an asynchronous copy; a captured step graph stays
+    // valid).  getBodyPose synchronises.  Both print and ignore an out-of-range body index.
+    int bodyCount() const { return static_cast<int>(_bodyMotion.size() / 6); }
+    void setBodyMotion(int body, float3 linearVelocity, float3 angularVelocity);
+    void getBodyPose(int body, float3& position, float4& orientation) const;
 
 private:
     std::shared_ptr<SPHParticles> _fluids;
@@ -392,7 +417,9 @@ private:
     bool solverIsGraphSafe() const;
     unsigned int solverConfigEpoch() const;
     void dropStepGraph();
+    std::vector<float> _bodyMotion;       // host copy of all bodies' motions (6 floats each); empty: no bodies
     void computeBoundaryMass();
+    void searchForStep();                 // bodies (if any), then the fluid search
     void neighborSearch(const std::shared_ptr<SPHParticles>& particles, DArray<int>& cellStart);
 };
 

@@ -282,8 +282,12 @@ class SlabSystem(SphkOps):
 
     HISTORY = {"dfsph": 1, "wcsph": 0, "pbd": 3}      # extra floats per particle that migrate with it
 
-    def __init__(self, scene, rank: int, world: int, device, capacity_factor: float = 1.6, group=None, cut_skew: int = 0):
-        """cut_skew: shifts the interior cuts by that many planes off the balanced position (tests of the re-balancing)."""
+    def __init__(self, scene, rank: int, world: int, device, capacity_factor: float = 1.6, group=None, cut_skew: int = 0,
+                 bodies=None):
+        """cut_skew: shifts the interior cuts by that many planes off the balanced position (tests of the re-balancing).
+        Kinematic bodies (engine.SphkSystem's `bodies`) are single-GPU only: every rank would have to hold every body."""
+        if bodies:
+            raise ValueError("kinematic bodies are not supported on slab ranks (single-GPU engine.SphkSystem only)")
         self.L = capi.sphk()
         self.p = scene.params
         self.rank, self.world = rank, world

@@ -71,9 +71,24 @@ int   sph_app_wait(sph_app* app);
  * reference's host loop with one error sum read back per iteration), 2 = fused sweeps (default on), 3 = step graph. */
 int   sph_app_dfsph_iterations(sph_app* app, int* divergence_iters, int* density_iters);
 int   sph_app_set_option(sph_app* app, int option, int value);
+/* 1 when the next step replays a captured step graph, 0 when it launches kernels one by one, -1 on the reference build */
+int   sph_app_step_graph_active(sph_app* app);
 /* Vorticity confinement of strength eps >= 0 in every following step (BasicSPHSolver::setVorticityConfinement; 0 = off,
  * the default).  No reference counterpart: returns 1 on the reference build, and for eps < 0 or NaN. */
 int   sph_app_set_vorticity(sph_app* app, float eps);
+/* Kinematic rigid bodies (SPHSystem's constructor with a vector of sphb200::KinematicBody; DESIGN.md section 2.3).  No
+ * reference counterpart: NULL / 1 on the reference build.  Body b is the points body_xyz[body_begin[b] .. body_begin[b+1])
+ * (body coordinates; body_begin[0] = 0), pose[7 b ..] = {cx, cy, cz, qx, qy, qz, qw} (quaternion scalar part last),
+ * motion[6 b ..] = {Vx, Vy, Vz, Ox, Oy, Oz} in the world frame.  The boundary set of the system is the static boundary_xyz
+ * followed by the bodies' particles (sph_app_boundary_size and sph_app_download_boundary include them).  n_bodies = 0 is
+ * sph_app_create.  NULL on failure, including bodies the engine refuses (more than 64, non-finite pose or motion). */
+sph_app* sph_app_create_with_bodies(const float* fluid_xyz, int n_fluid, const float* boundary_xyz, int n_boundary,
+                                    int n_bodies, const int* body_begin, const float* body_xyz, const float* pose,
+                                    const float* motion, const sph_app_params* params);
+/* new motion of one body from the next step on (SPHSystem::setBodyMotion); 1 for a bad index or non-finite values */
+int   sph_app_set_body_motion(sph_app* app, int body, const float* linear_velocity_xyz, const float* angular_velocity_xyz);
+/* current pose of one body, float[7] as above (synchronises) */
+int   sph_app_body_pose(sph_app* app, int body, float* pose);
 /* Name of the engine underneath: "reference-cuda" or "b200-native". */
 const char* sph_app_engine(void);
 

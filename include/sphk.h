@@ -134,7 +134,8 @@ int sphk_neighbor_search(sphk_ctx* ctx, int which, const sphk_particles* p, int*
  * (fluidPosLast, width 3), which re-sort with particle2cell as keys and rely on sort stability. */
 int sphk_permute(sphk_ctx* ctx, float* array, int width, int n);
 
-/* Re-packs the shadows from the API arrays without re-sorting (after caller-side edits). */
+/* Re-packs the shadows from the API arrays without re-sorting (after caller-side edits).  Boundary records take the
+ * boundary velocities of body particles when bodies are defined (sphk_bodies_init); static records keep v = 0. */
 int sphk_refresh(sphk_ctx* ctx, const sphk_scene* scene);
 
 /* computeBoundaryMass_CUDA, SPHSystem.cu:79-112: mass_b = rhoB / max(eps, sum_k W(|x_b - x_k|)). */
@@ -257,6 +258,37 @@ int sphk_fused_viscosity_surface_vorticity(sphk_ctx* ctx, const sphk_scene* s, f
  * in one sweep, omega from the velocities before XSPH.  No reference counterpart. */
 int sphk_fused_pbd_xsph_vorticity(sphk_ctx* ctx, const sphk_scene* s, float c, float rho0, float* color_grad_or_null,
                                   float rho_boundary, float* omega, float* omega_norm);
+
+/* ---- kinematic rigid bodies (no reference counterpart; DESIGN.md section 2.3) ---------------------------------------------
+ * A body is a rigid set of boundary particles given in body coordinates r_k, with a pose (centre c, unit quaternion q) and
+ * a motion (linear velocity V, angular velocity Omega, both in the world frame).  Poses and motions live in device memory.
+ * Layouts: pose = {cx, cy, cz, qx, qy, qz, qw} (scalar part LAST) per body, motion = {Vx, Vy, Vz, Ox, Oy, Oz} per body.
+ *
+ * sphk_bodies_init declares that the boundary slots [n_static, n) of the set that has NOT been searched yet belong to
+ * n_bodies bodies (1..SPHK_MAX_BODIES = 64): body b owns slots [body_begin[b], body_begin[b+1]) with body_begin[0] = n_static,
+ * body_begin[n_bodies] = boundary->n, non-decreasing; local_xyz holds r_k of slots n_static.. (host float3[n - n_static]).
+ * pose and motion are host arrays (a non-unit quaternion is normalised, a zero one refused).  boundary->vel is required.
+ * From then on every boundary search (sphk_neighbor_search(which = 1) too) places the body particles at their pose
+ * (x_k = c + R(q) r_k, v_k = V + Omega x (x_k - c) into boundary->pos / vel), and carries the mass and {r_k, group} of every
+ * particle with it; boundary records carry v_k for body particles and 0 for the static set.  sphk_boundary_mass sums
+ * over the particle's own group only (the static set, or its body): m_b = rho_B / max(eps, sum_{k in group} W_bk).
+ * Call it before the first boundary search (SPHK_ERR_STATE otherwise, and on a second call).  Synchronises.
+ * A body particle that leaves the grid gets the out-of-grid cell (Q8) and stops interacting; nothing guards against it. */
+int sphk_bodies_init(sphk_ctx* ctx, const sphk_particles* boundary, int n_static, int n_bodies, const int* body_begin,
+                     const float* local_xyz, const float* pose, const float* motion);
+/* New motions of all bodies (host float[6 * n_bodies]), enqueued on the stream as an ordinary copy: it takes effect at the
+ * next sphk_bodies_step and does not change the launch sequence (a captured step graph stays valid).  The caller's buffer
+ * may be reused on return (waits only while the previous change is still in the context's staging buffer). */
+int sphk_bodies_set_motion(sphk_ctx* ctx, const float* motion_host);
+/* One step of every body, before the fluid search: pose update (c += dt V; q = normalize(dq (x) q), dq the rotation by
+ * |Omega| dt about Omega), placement, and the boundary search that carries mass and body frame (invalidates the lists as
+ * a boundary search does).  dt > 0 and finite.  SPHK_ERR_STATE before sphk_bodies_init and the first boundary search. */
+int sphk_bodies_step(sphk_ctx* ctx, const sphk_particles* boundary, int* cell_start_boundary, float dt);
+/* current poses (host float[7 * n_bodies]); synchronises */
+int sphk_bodies_get_pose(sphk_ctx* ctx, float* pose_host);
+/* introspection: the carried {r_k, group} of every boundary slot in the current (sorted) order, device float4[n] (group
+ * 0 = static, b + 1 = body b) */
+int sphk_bodies_get_local(sphk_ctx* ctx, float* local_out);
 
 /* Builds the per-step neighbour list now (sweeps otherwise build it lazily on first use). */
 int sphk_build_neighbor_list(sphk_ctx* ctx, const sphk_scene* s);
