@@ -9,15 +9,21 @@
 //
 //   sph_headless [--solver sph|dfsph|pbd] [--frames N] [--box L | --box LX LY LZ] [--block NX NY NZ] [--origin X Y Z]
 //                [--dt DT] [--iters K] [--vorticity EPS] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] [--ranks N [--rank R --rendezvous DIR]]
-//                [--bullets K] [--stir OMEGA]
+//                [--bullets K] [--stir OMEGA] [--float REL]
 // --vorticity EPS turns on vorticity confinement of strength EPS (BasicSPHSolver::setVorticityConfinement) after the
 // constructor's step 0, for every solver and with --ranks.
 // --stir OMEGA adds one kinematic body (SPHSystem's constructor with a KinematicBody): a flat vertical paddle through the
 // centre of the fluid block, rotating about y at OMEGA rad/s.  It is two layers of the boundary lattice's spacing thick
 // (normal along z), 60 % of the block's x extent wide and as tall as the block; fluid lattice points within one spacing of
 // it are dropped.  Single GPU only.
+// --float REL adds one dynamic body instead (a KinematicBody with mass > 0, two-way coupled): a hollow cube of side about
+// 0.1, its faces sampled at the boundary lattice's spacing, at the centre of the fluid block, initially at rest.  Its mass
+// is REL * m0 / spacing^3 * V with V = (extent + boundary spacing)^3, the volume its particles stand for (the fluid's mass
+// per unit volume is m0 / spacing^3, DESIGN.md section 2.4), and its moments those of a solid cube of that mass and side.  Fluid lattice points within one spacing of it are dropped.  Single GPU
+// only, and not together with --stir.
 // --emit-scene writes the generated scene (PREFIX.fluid.f32, PREFIX.boundary.f32; with --stir also PREFIX.body.f32, the
-// paddle's points in body coordinates, and PREFIX.body_state.f32 = pose {c, q = (x, y, z, w)} + motion {V, Omega}) and
+// paddle's points in body coordinates, and PREFIX.body_state.f32 = pose {c, q = (x, y, z, w)} + motion {V, Omega}; with
+// --float the same for the cube and PREFIX.body_dyn.f32 = {M, Ix, Iy, Iz}) and
 // exits: needs no GPU, lets a test compare this generator with the python one the benchmarks use, or rebuild the scene.
 // --ranks N runs the same scene on N GPUs through SlabSPHSystem (host/sph_slab.hpp: the class API sharded by x-slabs):
 // without --rank the process forks one child per GPU (rank r on device r) and a fresh rendezvous directory; with
@@ -65,6 +71,8 @@ struct Options {
     float vorticity = 0.0f;                   // --vorticity EPS: vorticity confinement from frame 1 on (0: off)
     bool stir = false;                        // --stir OMEGA: a paddle rotating about y at OMEGA rad/s
     float stirOmega = 0.0f;
+    bool floating = false;                    // --float REL: a free cube of relative density REL
+    float floatRel = 0.0f;
     int bullets = 0;                          // test aid: this many top-layer particles start at ~3 cell planes per step
     int ranks = 1, rank = -1;                 // --ranks N: SlabSPHSystem on N GPUs; --rank R: this process is rank R
     std::string rendezvous;
@@ -84,6 +92,7 @@ bool parse(int argc, char** argv, Options& o) {
         else if (a == "--bullets" && need(i, 1)) o.bullets = std::atoi(argv[++i]);
         else if (a == "--vorticity" && need(i, 1)) o.vorticity = static_cast<float>(std::atof(argv[++i]));
         else if (a == "--stir" && need(i, 1)) { o.stir = true; o.stirOmega = static_cast<float>(std::atof(argv[++i])); }
+        else if (a == "--float" && need(i, 1)) { o.floating = true; o.floatRel = static_cast<float>(std::atof(argv[++i])); }
         else if (a == "--ranks" && need(i, 1)) o.ranks = std::atoi(argv[++i]);
         else if (a == "--rank" && need(i, 1)) o.rank = std::atoi(argv[++i]);
         else if (a == "--rendezvous" && need(i, 1)) o.rendezvous = argv[++i];
@@ -105,6 +114,11 @@ bool parse(int argc, char** argv, Options& o) {
     if (o.ranks < 1 || o.rank >= o.ranks || (o.rank >= 0 && o.ranks > 1 && o.rendezvous.empty())) return false;
     if (o.stir && (o.ranks > 1 || !std::isfinite(o.stirOmega))) {
         std::fprintf(stderr, "sph_headless: --stir runs on one GPU only (kinematic bodies are not supported with --ranks)\n");
+        return false;
+    }
+    if (o.floating && (o.ranks > 1 || o.stir || !(o.floatRel > 0.0f) || !std::isfinite(o.floatRel))) {
+        std::fprintf(stderr, "sph_headless: --float REL needs REL > 0, runs on one GPU only (bodies are not supported with --ranks) "
+                             "and not together with --stir\n");
         return false;
     }
     return o.frames >= 0 && o.vorticity >= 0.0f && o.block[0] > 0 && o.block[1] > 0 && o.block[2] > 0 &&
@@ -156,6 +170,30 @@ sphb200::KinematicBody paddle(const Options& o, float spacing, float boundarySpa
     b.orientation = make_float4(0.0f, 0.0f, 0.0f, 1.0f);
     b.linearVelocity = make_float3(0.0f, 0.0f, 0.0f);
     b.angularVelocity = make_float3(0.0f, o.stirOmega, 0.0f);
+    return b;
+}
+
+constexpr float kSphM0 = 76.596750762082e-6f;   // the fluid particle mass m0, main.cpp
+
+// --float: the hollow cube (body coordinates, centred on the block's centre, at rest), mass and moments of a solid cube
+sphb200::KinematicBody floating_cube(const Options& o, float spacing, float boundarySpacing) {
+    sphb200::KinematicBody b;
+    const float sb = boundarySpacing;
+    const int n = std::max(2, static_cast<int>(std::lround(0.1f / sb)) + 1);
+    for (int i = 0; i < n; ++i)
+        for (int j = 0; j < n; ++j)
+            for (int k = 0; k < n; ++k)
+                if (i == 0 || j == 0 || k == 0 || i == n - 1 || j == n - 1 || k == n - 1)
+                    b.points.push_back(make_float3((i - 0.5f * (n - 1)) * sb, (j - 0.5f * (n - 1)) * sb, (k - 0.5f * (n - 1)) * sb));
+    const float ex = spacing * (o.block[0] - 1), ey = spacing * (o.block[1] - 1);
+    b.position = make_float3(o.origin[0] + 0.5f * ex, o.origin[1] + 0.5f * ey, o.origin[2] + 0.5f * spacing * (o.block[2] - 1));
+    b.orientation = make_float4(0.0f, 0.0f, 0.0f, 1.0f);
+    b.linearVelocity = make_float3(0.0f, 0.0f, 0.0f);
+    b.angularVelocity = make_float3(0.0f, 0.0f, 0.0f);
+    const float side = n * sb;           // the volume its particles stand for: (extent + spacing)^3
+    b.mass = o.floatRel * (kSphM0 / (spacing * spacing * spacing)) * side * side * side;
+    const float I = b.mass * side * side / 6.0f;
+    b.inertia = make_float3(I, I, I);
     return b;
 }
 
@@ -227,7 +265,7 @@ int main(int argc, char** argv) {
     Options o;
     if (!parse(argc, argv, o)) {
         std::fprintf(stderr, "usage: sph_headless [--solver sph|dfsph|pbd] [--frames N] [--box L | LX LY LZ] [--block NX NY NZ] "
-                             "[--origin X Y Z] [--dt DT] [--iters K] [--vorticity EPS] [--stir OMEGA] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] "
+                             "[--origin X Y Z] [--dt DT] [--iters K] [--vorticity EPS] [--stir OMEGA | --float REL] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] "
                              "[--ranks N [--rank R --rendezvous DIR]]\n");
         return 2;
     }
@@ -242,21 +280,22 @@ int main(int argc, char** argv) {
     const float boundarySpacing = 0.99f * spaceSize.x / float(2 * cellSize.x - 1);
     std::vector<sphb200::KinematicBody> bodies;
     std::vector<float3> fluidPoints = fluid_block(o, sphSpacing);
-    if (o.stir) {
-        bodies.push_back(paddle(o, sphSpacing, boundarySpacing));
-        fluidPoints = clear_of(fluidPoints, bodies[0], boundarySpacing);
-    }
+    if (o.stir) bodies.push_back(paddle(o, sphSpacing, boundarySpacing));
+    if (o.floating) bodies.push_back(floating_cube(o, sphSpacing, boundarySpacing));
+    if (!bodies.empty()) fluidPoints = clear_of(fluidPoints, bodies[0], boundarySpacing);
     if (!o.emitScene.empty()) {
         const int3 cells = cellSize;
         bool ok = write_floats(o.emitScene + ".fluid.f32", flat(fluidPoints)) &&
                   write_floats(o.emitScene + ".boundary.f32", flat(boundary_shell(cells, spaceSize)));
-        if (ok && o.stir) {
+        if (ok && !bodies.empty()) {
             const auto& b = bodies[0];
             ok = write_floats(o.emitScene + ".body.f32", flat(b.points)) &&
                  write_floats(o.emitScene + ".body_state.f32",
                               {b.position.x, b.position.y, b.position.z, b.orientation.x, b.orientation.y, b.orientation.z, b.orientation.w,
                                b.linearVelocity.x, b.linearVelocity.y, b.linearVelocity.z, b.angularVelocity.x, b.angularVelocity.y,
                                b.angularVelocity.z});
+            if (ok && o.floating)
+                ok = write_floats(o.emitScene + ".body_dyn.f32", {b.mass, b.inertia.x, b.inertia.y, b.inertia.z});
         }
         std::printf("{\"cells\": [%d, %d, %d]}\n", cells.x, cells.y, cells.z);
         return ok ? 0 : 5;
@@ -309,7 +348,7 @@ int main(int argc, char** argv) {
     const float dt = o.dt > 0.0f ? o.dt : (wcsph ? 0.001f : 0.004f);
     const float sphRho0 = 1.0f;
     const float sphRhoBoundary = 1.4f * sphRho0;
-    const float sphM0 = 76.596750762082e-6f;
+    const float sphM0 = kSphM0;
     const float sphStiff = 10.0f;
     const float3 sphG = make_float3(0.0f, -9.8f, 0.0f);
     const float sphVisc = 5e-4f;
@@ -337,7 +376,7 @@ int main(int argc, char** argv) {
                                                 dt, sphM0, sphRho0, sphRhoBoundary, sphStiff, sphVisc, sphSurfaceTensionIntensity,
                                                 sphAirPressure, sphG, cellSize, boot);
         if (!pSlab->ok()) { std::fprintf(stderr, "sph_headless: rank %d: SlabSPHSystem did not come up\n", o.rank); return 4; }
-    } else if (o.stir) {
+    } else if (!bodies.empty()) {
         pSystem = std::make_shared<SPHSystem>(fluidParticles, boundaryParticles, pSolver, spaceSize, sphCellLength, sphSmoothingRadius,
                                               dt, sphM0, sphRho0, sphRhoBoundary, sphStiff, sphVisc, sphSurfaceTensionIntensity,
                                               sphAirPressure, sphG, cellSize, bodies);

@@ -31,18 +31,27 @@ SPHK_FUNCTIONS = [
     "sphk_mg_exchange_ints", "sphk_mg_exchange_ints_async", "sphk_mg_plane_ranges", "sphk_mg_halo_device", "sphk_mg_check_async", "sphk_set_active_range_device", "sphk_mg_allreduce_sum", "sphk_mg_exchange_slices", "sphk_mg_halo", "sphk_mg_check", "sphk_mg_stats",
     "sphk_strays_block_floats", "sphk_strays_collect", "sphk_strays_append", "sphk_mg_strays_route", "sphk_strays_counts",
     "sphk_bodies_init", "sphk_bodies_set_motion", "sphk_bodies_step", "sphk_bodies_get_pose", "sphk_bodies_get_local",
+    "sphk_bodies_set_dynamics", "sphk_bodies_react", "sphk_bodies_integrate", "sphk_bodies_set_body_motion",
+    "sphk_bodies_get_motion", "sphk_bodies_get_impulse",
 ]
 SPH_APP_FUNCTIONS = [
     "sph_app_create", "sph_app_destroy", "sph_app_step", "sph_app_fluid_size", "sph_app_boundary_size",
     "sph_app_download_fluid", "sph_app_download_boundary", "sph_app_upload_fluid", "sph_app_engine",
     "sph_app_submit", "sph_app_wait", "sph_app_dfsph_iterations", "sph_app_set_option", "sph_app_set_vorticity",
     "sph_app_create_with_bodies", "sph_app_set_body_motion", "sph_app_body_pose", "sph_app_step_graph_active",
+    "sph_app_create_with_dynamic_bodies", "sph_app_body_motion", "sph_app_body_impulse",
 ]
 
 OPT_NEIGHBOR_LIST, OPT_LIST_CAPACITY, OPT_LIST_SKIN, OPT_SIMPLE_LIST_BUILD, OPT_TILE, OPT_STAGED_LIST_BUILD, OPT_PATCH = 1, 2, 5, 6, 9, 10, 11
 # tile-list geometry of csrc/sphk_internal.cuh (SPHK_BLOCK, SPHK_TILE_WINS, SPHK_TILE_CAP): sphk_get_tile_lists copies
 # TILE_WINDOWS windows per tile of TILE_PARTICLES particles; a tile whose windows exceed TILE_CAP records walks the cells
 TILE_PARTICLES, TILE_WINDOWS, TILE_CAP = 128, 18, 1535
+
+
+def body_mass_inertia(bodies) -> np.ndarray:
+    """{M, Ix, Iy, Iz} per body from the body dicts' optional "mass" (default 0: kinematic) and "inertia" (default 0)."""
+    return np.ascontiguousarray([[float(b.get("mass", 0.0)), *[float(x) for x in b.get("inertia", (0.0, 0.0, 0.0))]]
+                                 for b in bodies], np.float32).reshape(-1, 4)
 
 
 class SphkGrid(C.Structure):
@@ -103,6 +112,7 @@ def app_lib(path: str = LIBHOST):
         L = _load(path)
         L.sph_app_create.restype = C.c_void_p
         L.sph_app_create_with_bodies.restype = C.c_void_p
+        L.sph_app_create_with_dynamic_bodies.restype = C.c_void_p
         L.sph_app_step.restype = C.c_float
         L.sph_app_engine.restype = C.c_char_p
         L.sph_app_destroy.restype = None
@@ -137,8 +147,9 @@ class SphApp:
     CUDA build oracle/_ref/libsphref.so -- the facade source is the same file for both."""
 
     def __init__(self, scene, lib_path: str = LIBHOST, bodies=None):
-        """bodies: kinematic rigid bodies in engine.SphkSystem's format (sph_app_create_with_bodies); their particles follow
-        the static boundary set, so nB counts them."""
+        """bodies: rigid bodies in engine.SphkSystem's format (sph_app_create_with_bodies; with a "mass" key on any body,
+        sph_app_create_with_dynamic_bodies: dynamics are declared when some mass is > 0, as in engine.SphkSystem); their
+        particles follow the static boundary set, so nB counts them."""
         self.L = app_lib(lib_path)
         self.scene = scene
         fl = np.ascontiguousarray(scene.fluid, np.float32)
@@ -152,10 +163,14 @@ class SphApp:
             pose = np.ascontiguousarray([[*b["position"], *b["orientation"]] for b in bodies], np.float32).reshape(-1, 7)
             motion = np.ascontiguousarray([[*b["linear_velocity"], *b["angular_velocity"]] for b in bodies], np.float32).reshape(-1, 6)
             self.nB += xyz.shape[0]
-            self.h = self.L.sph_app_create_with_bodies(fl.ctypes.data_as(C.c_void_p), C.c_int(self.nF), bd.ctypes.data_as(C.c_void_p),
-                                                       C.c_int(bd.shape[0]), C.c_int(len(bodies)), begin.ctypes.data_as(C.c_void_p),
-                                                       xyz.ctypes.data_as(C.c_void_p), pose.ctypes.data_as(C.c_void_p),
-                                                       motion.ctypes.data_as(C.c_void_p), C.byref(prm))
+            args = [fl.ctypes.data_as(C.c_void_p), C.c_int(self.nF), bd.ctypes.data_as(C.c_void_p), C.c_int(bd.shape[0]),
+                    C.c_int(len(bodies)), begin.ctypes.data_as(C.c_void_p), xyz.ctypes.data_as(C.c_void_p),
+                    pose.ctypes.data_as(C.c_void_p), motion.ctypes.data_as(C.c_void_p)]
+            if any("mass" in b for b in bodies):
+                mi = body_mass_inertia(bodies)
+                self.h = self.L.sph_app_create_with_dynamic_bodies(*args, mi.ctypes.data_as(C.c_void_p), C.byref(prm))
+            else:
+                self.h = self.L.sph_app_create_with_bodies(*args, C.byref(prm))
         else:
             self.h = self.L.sph_app_create(fl.ctypes.data_as(C.c_void_p), C.c_int(self.nF), bd.ctypes.data_as(C.c_void_p),
                                            C.c_int(self.nB), C.byref(prm))
@@ -246,6 +261,20 @@ class SphApp:
         out = np.zeros(7, np.float32)
         if self.L.sph_app_body_pose(self.h, C.c_int(body), out.ctypes.data_as(C.c_void_p)):
             raise RuntimeError("sph_app_body_pose failed (reference engine or bad index)")
+        return out
+
+    def body_motion(self, body: int) -> np.ndarray:
+        """{Vx, Vy, Vz, Ox, Oy, Oz} of one body (the integrated motion of a dynamic body)."""
+        out = np.zeros(6, np.float32)
+        if self.L.sph_app_body_motion(self.h, C.c_int(body), out.ctypes.data_as(C.c_void_p)):
+            raise RuntimeError("sph_app_body_motion failed (reference engine or bad index)")
+        return out
+
+    def body_impulse(self, body: int) -> np.ndarray:
+        """{J, H} the fluid gave one body over the last step (two-way coupled systems; zero otherwise)."""
+        out = np.zeros(6, np.float32)
+        if self.L.sph_app_body_impulse(self.h, C.c_int(body), out.ctypes.data_as(C.c_void_p)):
+            raise RuntimeError("sph_app_body_impulse failed (reference engine or bad index)")
         return out
 
     def close(self):

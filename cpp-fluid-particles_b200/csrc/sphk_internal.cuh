@@ -64,7 +64,17 @@ struct BodyState {
     float* snapMass = nullptr;       // device [capB]: pre-sort snapshot of the boundary mass
     float* stage = nullptr;          // pinned [6 * SPHK_MAX_BODIES]: staging of sphk_bodies_set_motion
     cudaEvent_t staged = nullptr;    // the copy out of `stage` has been done
+    int* decl = nullptr;             // device [capB]: declaration slot of every particle, carried by the search like local[]
+    int* snapDecl = nullptr;         // device [capB]: pre-sort snapshot of decl
+    int* begin = nullptr;            // device [nBodies + 1]: body_begin of sphk_bodies_init (declaration slots)
+    float box[6 * SPHK_MAX_BODIES] = {};   // host: body-frame bounding box of each body's r_k, {lo.xyz, hi.xyz}
+    bool stepped = false;            // sphk_bodies_step has run
+    // two-way coupling (sphk_bodies_set_dynamics; DESIGN.md section 2.4)
+    float* dyn = nullptr;            // device [SPHK_DYN * nBodies]: M, I.xyz, box lo.xyz, box hi.xyz, clamp box hi.xyz
+    double* acc = nullptr;           // device [6 * (n - nStatic)]: {J, H} of every body particle, summed over the step's reactions
+    float* impulse = nullptr;        // device [6 * nBodies]: {J, H} of the last integrated step
 };
+#define SPHK_DYN 16                  // floats per body in BodyState::dyn
 __device__ __forceinline__ float body_group(float4 local) { return local.w; }
 
 struct sphk_ctx {

@@ -638,17 +638,59 @@ extern "C" int sphk_get_permutation(sphk_ctx* c, int* perm_out, int n) {
 // {r_k, group} of each particle with it (the reference leaves boundary masses in place, Q2: they are computed once, after
 // the one search) and keeps the body velocities in the records; the static set keeps v = 0.
 
+__device__ void pose_rotate(float* P, double wx, double wy, double wz, double w, float dt);
+
+// R(q) as a row-major 3x3 matrix in double
+__device__ void quat_matrix(const float* q, double R[9]) {
+    const double x = q[0], y = q[1], z = q[2], w = q[3];
+    R[0] = 1.0 - 2.0 * (y * y + z * z); R[1] = 2.0 * (x * y - z * w);       R[2] = 2.0 * (x * z + y * w);
+    R[3] = 2.0 * (x * y + z * w);       R[4] = 1.0 - 2.0 * (x * x + z * z); R[5] = 2.0 * (y * z - x * w);
+    R[6] = 2.0 * (x * z - y * w);       R[7] = 2.0 * (y * z + x * w);       R[8] = 1.0 - 2.0 * (x * x + y * y);
+}
+
+// Wall contact of a dynamic body (DESIGN.md section 2.4): the 8 corners of its body-frame bounding box at the new pose must lie
+// in the box the fluid is clamped to, [0, 0.99 space] per axis.  The centre moves back by the largest penetration of each axis
+// and the outward component of V is zeroed (inelastic, frictionless; no torque).
+__device__ void body_contact(float* P, float* V, const float* D) {
+    double R[9];
+    quat_matrix(P + 3, R);
+    double lo[3] = {1e300, 1e300, 1e300}, hi[3] = {-1e300, -1e300, -1e300};
+    for (int k = 0; k < 8; ++k) {
+        const double r[3] = {D[(k & 1) ? 7 : 4], D[(k & 2) ? 8 : 5], D[(k & 4) ? 9 : 6]};
+        for (int a = 0; a < 3; ++a) {
+            const double x = P[a] + R[3 * a] * r[0] + R[3 * a + 1] * r[1] + R[3 * a + 2] * r[2];
+            lo[a] = fmin(lo[a], x); hi[a] = fmax(hi[a], x);
+        }
+    }
+    for (int a = 0; a < 3; ++a) {
+        if (lo[a] < 0.0) {
+            P[a] = static_cast<float>(P[a] - lo[a]);
+            V[a] = fmaxf(V[a], 0.f);
+        } else if (hi[a] > D[10 + a]) {
+            P[a] = static_cast<float>(P[a] - (hi[a] - D[10 + a]));
+            V[a] = fminf(V[a], 0.f);
+        }
+    }
+}
+
 // One thread per body.  The update is evaluated in double from the float pose and rounded once: with -use_fast_math the
-// float sin / cos would be the approximate intrinsics.
-__global__ void k_bodies_pose(float* __restrict__ pose, const float* __restrict__ motion, int nBodies, float dt) {
+// float sin / cos would be the approximate intrinsics.  dyn (sphk_bodies_set_dynamics, else null): dynamic bodies then
+// meet the walls.
+__global__ void k_bodies_pose(float* __restrict__ pose, float* __restrict__ motion, int nBodies, float dt,
+                              const float* __restrict__ dyn) {
     const int b = blockIdx.x * blockDim.x + threadIdx.x;
     if (b >= nBodies) return;
     float* P = pose + 7 * b;
-    const float* M = motion + 6 * b;
+    float* M = motion + 6 * b;
     for (int a = 0; a < 3; ++a) P[a] = __fadd_rn(P[a], __fmul_rn(dt, M[a]));
     const double wx = M[3], wy = M[4], wz = M[5];
     const double w = sqrt(wx * wx + wy * wy + wz * wz);
-    if (w == 0.0) return;                                   // dq = identity: q stays bit for bit
+    if (w != 0.0) pose_rotate(P, wx, wy, wz, w, dt);        // dq = identity otherwise: q stays bit for bit
+    if (dyn && dyn[SPHK_DYN * b] > 0.f) body_contact(P, M, dyn + SPHK_DYN * b);
+}
+
+// q <- normalize(dq (x) q) of k_bodies_pose
+__device__ void pose_rotate(float* P, double wx, double wy, double wz, double w, float dt) {
     const double h = 0.5 * w * static_cast<double>(dt), s = sin(h) / w;
     const double dx = s * wx, dy = s * wy, dz = s * wz, dw = cos(h);
     const double qx = P[3], qy = P[4], qz = P[5], qw = P[6];
@@ -667,12 +709,14 @@ __global__ void k_bodies_pose(float* __restrict__ pose, const float* __restrict_
 __global__ void __launch_bounds__(SPHK_BLOCK)
 k_bodies_place(const float4* __restrict__ local, const float* __restrict__ pose, const float* __restrict__ motion,
                const float* __restrict__ mass, int n, float* __restrict__ pos, float* __restrict__ vel,
-               float4* __restrict__ snapLocal, float* __restrict__ snapMass) {
+               float4* __restrict__ snapLocal, float* __restrict__ snapMass, const int* __restrict__ decl,
+               int* __restrict__ snapDecl) {
     const int i = blockIdx.x * SPHK_BLOCK + threadIdx.x;
     if (i >= n) return;
     const float4 l = local[i];
     snapLocal[i] = l;
     snapMass[i] = mass[i];
+    snapDecl[i] = decl[i];
     const int g = static_cast<int>(body_group(l));
     if (g == 0) return;
     const float* P = pose + 7 * (g - 1);
@@ -695,7 +739,8 @@ k_bodies_place(const float4* __restrict__ local, const float* __restrict__ pose,
 __global__ void __launch_bounds__(SPHK_BLOCK)
 k_bodies_gather(const int* __restrict__ idxSorted, const float4* __restrict__ snapPos, const float4* __restrict__ snapVel,
                 const float* __restrict__ snapMass, const float4* __restrict__ snapLocal, int n, float* __restrict__ pos,
-                float* __restrict__ vel, float* __restrict__ mass, float4* __restrict__ local, Rec rec) {
+                float* __restrict__ vel, float* __restrict__ mass, float4* __restrict__ local, Rec rec,
+                const int* __restrict__ snapDecl, int* __restrict__ decl) {
     const int s = blockIdx.x * SPHK_BLOCK + threadIdx.x;
     if (s >= n) return;
     const int src = idxSorted[s];
@@ -706,15 +751,57 @@ k_bodies_gather(const int* __restrict__ idxSorted, const float4* __restrict__ sn
     store3(vel, s, xyz(v));
     mass[s] = m;
     local[s] = l;
+    decl[s] = snapDecl[src];
     if (body_group(l) == 0.f) v = make_float4(0.f, 0.f, 0.f, 0.f);
     v.w = m;
     p.w = m;
     rec_store(rec + s, p, v);
 }
 
+// End of step of every body (DESIGN.md section 2.4), one block per body.  The block sums the {J, H} its particles gathered over
+// the step's reactions in a fixed shape (strided partials, then a tree; deterministic) and clears them.  Thread 0 reports
+// them and, for a dynamic body (M > 0), updates the motion in double, rounded once:
+//   V += J / M + dt G;  L = R diag(I) R^T Omega + H;  Omega = R diag(1/I) R^T L   (R from the current pose)
+#define SPHK_INTEGRATE_THREADS 256
+__global__ void __launch_bounds__(SPHK_INTEGRATE_THREADS)
+k_bodies_integrate(const int* __restrict__ begin, int nStatic, double* __restrict__ acc, const float* __restrict__ pose,
+                   float* __restrict__ motion, const float* __restrict__ dyn, float* __restrict__ impulse, float dt, float3 G) {
+    __shared__ double red[6][SPHK_INTEGRATE_THREADS];
+    const int b = blockIdx.x, t = threadIdx.x;
+    const int k0 = begin[b] - nStatic, k1 = begin[b + 1] - nStatic;
+    double s[6] = {0.0, 0.0, 0.0, 0.0, 0.0, 0.0};
+    for (int k = k0 + t; k < k1; k += SPHK_INTEGRATE_THREADS)
+        for (int q = 0; q < 6; ++q) { s[q] += acc[6 * static_cast<size_t>(k) + q]; acc[6 * static_cast<size_t>(k) + q] = 0.0; }
+    for (int q = 0; q < 6; ++q) red[q][t] = s[q];
+    __syncthreads();
+    for (int w = SPHK_INTEGRATE_THREADS / 2; w > 0; w >>= 1) {
+        if (t < w)
+            for (int q = 0; q < 6; ++q) red[q][t] += red[q][t + w];
+        __syncthreads();
+    }
+    if (t != 0) return;
+    const double J[3] = {red[0][0], red[1][0], red[2][0]}, H[3] = {red[3][0], red[4][0], red[5][0]};
+    for (int q = 0; q < 3; ++q) { impulse[6 * b + q] = static_cast<float>(J[q]); impulse[6 * b + 3 + q] = static_cast<float>(H[q]); }
+    const float* D = dyn + SPHK_DYN * b;
+    const double M = D[0];
+    if (!(M > 0.0)) return;                                  // held: kinematic, the reaction is only reported
+    float* Mo = motion + 6 * b;
+    const double g[3] = {G.x, G.y, G.z};
+    for (int a = 0; a < 3; ++a) Mo[a] = static_cast<float>(Mo[a] + J[a] / M + static_cast<double>(dt) * g[a]);
+    double R[9];
+    quat_matrix(pose + 7 * b + 3, R);
+    const double I[3] = {D[1], D[2], D[3]}, W[3] = {Mo[3], Mo[4], Mo[5]};
+    double wb[3], L[3], lb[3];
+    for (int a = 0; a < 3; ++a) wb[a] = R[a] * W[0] + R[3 + a] * W[1] + R[6 + a] * W[2];              // R^T Omega
+    for (int a = 0; a < 3; ++a) L[a] = R[3 * a] * I[0] * wb[0] + R[3 * a + 1] * I[1] * wb[1] + R[3 * a + 2] * I[2] * wb[2] + H[a];
+    for (int a = 0; a < 3; ++a) lb[a] = (R[a] * L[0] + R[3 + a] * L[1] + R[6 + a] * L[2]) / I[a];    // diag(1/I) R^T L
+    for (int a = 0; a < 3; ++a) Mo[3 + a] = static_cast<float>(R[3 * a] * lb[0] + R[3 * a + 1] * lb[1] + R[3 * a + 2] * lb[2]);
+}
+
 static void sphk_bodies_release(BodyState* b) {
     if (!b) return;
     cudaFree(b->pose); cudaFree(b->motion); cudaFree(b->local); cudaFree(b->snapLocal); cudaFree(b->snapMass);
+    cudaFree(b->decl); cudaFree(b->snapDecl); cudaFree(b->begin); cudaFree(b->dyn); cudaFree(b->acc); cudaFree(b->impulse);
     if (b->stage) cudaFreeHost(b->stage);
     if (b->staged) cudaEventDestroy(b->staged);
     delete b;
@@ -726,14 +813,15 @@ static int sphk_bodies_search(sphk_ctx* c, const sphk_particles* p, int* cell_st
     if (!p->vel || n != B->n) return SPHK_ERR_INVALID;      // the set declared by sphk_bodies_init
     cudaStream_t st = c->stream;
     k_bodies_place<<<sphk_blocks(n), SPHK_BLOCK, 0, st>>>(B->local, B->pose, B->motion, p->mass, n, p->pos, p->vel,
-                                                         B->snapLocal, B->snapMass);
+                                                         B->snapLocal, B->snapMass, B->decl, B->snapDecl);
     k_hash_snapshot<<<sphk_blocks(n), SPHK_BLOCK, 0, st>>>(p->pos, p->vel, n, c->cellLength, c->cs, c->org, p->particle2cell,
                                                           c->keys, c->idx, c->snapA, c->snapB);
     size_t tb = c->cubTempBytes;
     SPHK_CUDA_TRY(cub::DeviceRadixSort::SortPairs(c->cubTemp, tb, c->keys, c->keysSorted, c->idx, c->idxSorted, n, 0,
                                                   c->endBit, st));
     k_bodies_gather<<<sphk_blocks(n), SPHK_BLOCK, 0, st>>>(c->idxSorted, c->snapA, c->snapB, B->snapMass, B->snapLocal, n,
-                                                          p->pos, p->vel, p->mass, B->local, c->rec + c->capF);
+                                                          p->pos, p->vel, p->mass, B->local, c->rec + c->capF, B->snapDecl,
+                                                          B->decl);
     k_cell_start<<<sphk_blocks(c->ncells + 1), SPHK_BLOCK, 0, st>>>(c->keysSorted, n, c->ncells, cell_start);
     c->launches += 4 + 4;
     c->nB = n; c->boundarySearched = true; c->listEpoch = ~0ull; c->permValid = false;
@@ -777,12 +865,29 @@ extern "C" int sphk_bodies_init(sphk_ctx* c, const sphk_particles* boundary, int
     BodyState* B = new (std::nothrow) BodyState;
     if (!B) return SPHK_ERR_ALLOC;
     B->nBodies = n_bodies; B->nStatic = n_static; B->n = n;
+    for (int b = 0; b < n_bodies; ++b) {                     // body-frame bounding boxes (wall contact of dynamic bodies)
+        float* box = B->box + 6 * b;
+        for (int a = 0; a < 3; ++a) { box[a] = 0.f; box[3 + a] = 0.f; }
+        for (int k = body_begin[b]; k < body_begin[b + 1]; ++k)
+            for (int a = 0; a < 3; ++a) {
+                const float r = local_xyz[3 * static_cast<size_t>(k - n_static) + a];
+                if (k == body_begin[b] || r < box[a]) box[a] = r;
+                if (k == body_begin[b] || r > box[3 + a]) box[3 + a] = r;
+            }
+    }
+    std::vector<int> decl(static_cast<size_t>(n));
+    for (int k = 0; k < n; ++k) decl[k] = k;
     const size_t cap = static_cast<size_t>(c->capB);
     cudaError_t e = dalloc(&B->pose, 7 * static_cast<size_t>(n_bodies));
     if (e == cudaSuccess) e = dalloc(&B->motion, 6 * static_cast<size_t>(n_bodies));
     if (e == cudaSuccess) e = dalloc(&B->local, cap);
     if (e == cudaSuccess) e = dalloc(&B->snapLocal, cap);
     if (e == cudaSuccess) e = dalloc(&B->snapMass, cap);
+    if (e == cudaSuccess) e = dalloc(&B->decl, cap);
+    if (e == cudaSuccess) e = dalloc(&B->snapDecl, cap);
+    if (e == cudaSuccess) e = dalloc(&B->begin, static_cast<size_t>(n_bodies) + 1);
+    if (e == cudaSuccess) e = cudaMemcpy(B->decl, decl.data(), sizeof(int) * decl.size(), cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaMemcpy(B->begin, body_begin, sizeof(int) * (n_bodies + 1), cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaMallocHost(reinterpret_cast<void**>(&B->stage), sizeof(float) * 6 * SPHK_MAX_BODIES);
     if (e == cudaSuccess) e = cudaEventCreateWithFlags(&B->staged, cudaEventDisableTiming);
     if (e == cudaSuccess) e = cudaMemcpy(B->pose, q.data(), sizeof(float) * q.size(), cudaMemcpyHostToDevice);
@@ -813,10 +918,87 @@ extern "C" int sphk_bodies_step(sphk_ctx* c, const sphk_particles* boundary, int
     if (!(dt > 0.f) || !all_finite(&dt, 1)) return SPHK_ERR_INVALID;
     if (!c->bodies || !c->boundarySearched) return SPHK_ERR_STATE;
     if (boundary->n != c->nB) return SPHK_ERR_STATE;
-    const BodyState* B = c->bodies;
-    k_bodies_pose<<<1, SPHK_MAX_BODIES, 0, c->stream>>>(B->pose, B->motion, B->nBodies, dt);
+    BodyState* B = c->bodies;
+    k_bodies_pose<<<1, SPHK_MAX_BODIES, 0, c->stream>>>(B->pose, B->motion, B->nBodies, dt, B->dyn);
     c->launches++;
+    B->stepped = true;
     return sphk_bodies_search(c, boundary, cell_start_boundary);
+}
+
+extern "C" int sphk_bodies_set_dynamics(sphk_ctx* c, const float* mass_inertia, const float space[3]) {
+    if (!c || !mass_inertia || !space) return SPHK_ERR_INVALID;
+    if (!c->bodies) return SPHK_ERR_STATE;
+    BodyState* B = c->bodies;
+    if (!all_finite(mass_inertia, 4 * B->nBodies) || !all_finite(space, 3)) return SPHK_ERR_INVALID;
+    for (int a = 0; a < 3; ++a)
+        if (!(space[a] > 0.f)) return SPHK_ERR_INVALID;
+    for (int b = 0; b < B->nBodies; ++b) {
+        const float* m = mass_inertia + 4 * b;
+        if (!(m[0] >= 0.f) || m[1] < 0.f || m[2] < 0.f || m[3] < 0.f) return SPHK_ERR_INVALID;
+        if (m[0] > 0.f && !(m[1] > 0.f && m[2] > 0.f && m[3] > 0.f)) return SPHK_ERR_INVALID;
+    }
+    if (B->dyn || B->stepped) return SPHK_ERR_STATE;        // once, before the first sphk_bodies_step
+    std::vector<float> dyn(static_cast<size_t>(SPHK_DYN) * B->nBodies, 0.f);
+    for (int b = 0; b < B->nBodies; ++b) {
+        float* D = dyn.data() + SPHK_DYN * b;
+        for (int a = 0; a < 4; ++a) D[a] = mass_inertia[4 * b + a];
+        for (int a = 0; a < 6; ++a) D[4 + a] = B->box[6 * b + a];
+        for (int a = 0; a < 3; ++a) D[10 + a] = space[a] * .99f;     // the fluid's clamp box (k_advect's clamp_axis)
+    }
+    const size_t nk = static_cast<size_t>(B->n - B->nStatic);
+    cudaError_t e = dalloc(&B->dyn, dyn.size());
+    if (e == cudaSuccess) e = dalloc(&B->acc, 6 * nk);
+    if (e == cudaSuccess) e = dalloc(&B->impulse, 6 * static_cast<size_t>(B->nBodies));
+    if (e == cudaSuccess) e = cudaMemcpy(B->dyn, dyn.data(), sizeof(float) * dyn.size(), cudaMemcpyHostToDevice);
+    if (e != cudaSuccess) {
+        cudaFree(B->dyn); cudaFree(B->acc); cudaFree(B->impulse);
+        B->dyn = nullptr; B->acc = nullptr; B->impulse = nullptr;
+        cudaGetLastError();
+        return e == cudaErrorMemoryAllocation ? SPHK_ERR_ALLOC : static_cast<int>(e);
+    }
+    return SPHK_OK;
+}
+
+extern "C" int sphk_bodies_integrate(sphk_ctx* c, float dt, const float G[3]) {
+    if (!c || !G) return SPHK_ERR_INVALID;
+    if (!(dt > 0.f) || !all_finite(&dt, 1) || !all_finite(G, 3)) return SPHK_ERR_INVALID;
+    if (!c->bodies || !c->bodies->dyn) return SPHK_ERR_STATE;
+    const BodyState* B = c->bodies;
+    k_bodies_integrate<<<B->nBodies, SPHK_INTEGRATE_THREADS, 0, c->stream>>>(B->begin, B->nStatic, B->acc, B->pose, B->motion,
+                                                                             B->dyn, B->impulse, dt, make_float3(G[0], G[1], G[2]));
+    c->launches++;
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+extern "C" int sphk_bodies_set_body_motion(sphk_ctx* c, int body, const float motion[6]) {
+    if (!c || !motion) return SPHK_ERR_INVALID;
+    if (!c->bodies) return SPHK_ERR_STATE;
+    BodyState* B = c->bodies;
+    if (body < 0 || body >= B->nBodies || !all_finite(motion, 6)) return SPHK_ERR_INVALID;
+    SPHK_CUDA_TRY(cudaEventSynchronize(B->staged));         // the staging buffer is shared with sphk_bodies_set_motion
+    std::memcpy(B->stage + 6 * body, motion, sizeof(float) * 6);
+    SPHK_CUDA_TRY(cudaMemcpyAsync(B->motion + 6 * body, B->stage + 6 * body, sizeof(float) * 6, cudaMemcpyHostToDevice, c->stream));
+    SPHK_CUDA_TRY(cudaEventRecord(B->staged, c->stream));
+    return SPHK_OK;
+}
+
+extern "C" int sphk_bodies_get_motion(sphk_ctx* c, float* motion_host) {
+    if (!c || !motion_host) return SPHK_ERR_INVALID;
+    if (!c->bodies) return SPHK_ERR_STATE;
+    SPHK_CUDA_TRY(cudaMemcpyAsync(motion_host, c->bodies->motion, sizeof(float) * 6 * c->bodies->nBodies, cudaMemcpyDeviceToHost,
+                                  c->stream));
+    SPHK_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    return SPHK_OK;
+}
+
+extern "C" int sphk_bodies_get_impulse(sphk_ctx* c, float* impulse_host) {
+    if (!c || !impulse_host) return SPHK_ERR_INVALID;
+    if (!c->bodies || !c->bodies->dyn) return SPHK_ERR_STATE;
+    SPHK_CUDA_TRY(cudaMemcpyAsync(impulse_host, c->bodies->impulse, sizeof(float) * 6 * c->bodies->nBodies, cudaMemcpyDeviceToHost,
+                                  c->stream));
+    SPHK_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    return SPHK_OK;
 }
 
 extern "C" int sphk_bodies_get_pose(sphk_ctx* c, float* pose_host) {

@@ -1341,6 +1341,66 @@ extern "C" int sphk_pbd_delta_pos_apply(sphk_ctx* c, const sphk_scene* s, const 
     return SPHK_OK;
 }
 
+// ---- two-way coupled bodies: the fluid's reaction on them (DESIGN.md section 2.4) ---------------------------------------------
+// One thread per boundary slot; body particles only.  Walks the fluid cells within `reach` cells of the particle with the
+// fluid cell ranges of the search and forms each pair term as the fluid sweep forms it, g = (m_k s_i) (d gradWfactor),
+// d = x_i - x_k (the fluid particle received c m_i g).  The body particle gathers -c m_i g and its moment about the body's
+// centre into its own declaration slot of acc, in double (no atomics: every slot has one writer, sums are in walk order).
+__global__ void __launch_bounds__(SPHK_BLOCK)
+k_bodies_react(const DevScene s, const float* __restrict__ massF, const float4* __restrict__ local, const int* __restrict__ decl,
+               const float* __restrict__ pose, int nB, int nStatic, int reach, float coef, double* __restrict__ acc) {
+    if (s.pred && *s.pred == 0) return;     // a device-controlled loop has ended: its sweeps did not run
+    const int kb = blockIdx.x * SPHK_BLOCK + threadIdx.x;
+    if (kb >= nB) return;
+    const int g = static_cast<int>(body_group(local[kb]));
+    if (g == 0) return;
+    const float4 pk = rec_lo(s.rec + s.bOff + kb);          // {x_k, m_k}
+    const float3 xk = xyz(pk);
+    const float mk = pk.w;
+    const int cx = cell_coord(pk.x, s.cellLength) - s.org.x, cy = cell_coord(pk.y, s.cellLength) - s.org.y,
+              cz = cell_coord(pk.z, s.cellLength) - s.org.z;
+    if (cx < 0 || cx >= s.cs.x || cy < 0 || cy >= s.cs.y || cz < 0 || cz >= s.cs.z) return;   // off the grid: no interaction
+    const int zlo = max(cz - reach, 0), zhi = min(cz + reach, s.cs.z - 1);
+    const double cc = coef;
+    double F[3] = {0.0, 0.0, 0.0};
+#pragma unroll 1
+    for (int x = max(cx - reach, 0); x <= min(cx + reach, s.cs.x - 1); ++x)
+#pragma unroll 1
+        for (int y = max(cy - reach, 0); y <= min(cy + reach, s.cs.y - 1); ++y) {
+            const int c0 = (x * s.cs.y + y) * s.cs.z;
+            const int end = s.csF[c0 + zhi + 1];
+            for (int j = s.csF[c0 + zlo]; j < end; ++j) {
+                const float4 lo = rec_lo(s.rec + j);
+                const float3 d = xyz(lo) - xk;
+                const float r2 = dot3(d, d);
+                if (r2 > s.k.r2cut) continue;
+                const float3 t = (mk * lo.w) * (d * grad_w_factor(sqrtf(r2), s.k));
+                const double f = -cc * static_cast<double>(massF[j]);
+                F[0] += f * t.x; F[1] += f * t.y; F[2] += f * t.z;
+            }
+        }
+    const float* P = pose + 7 * (g - 1);
+    const double rx = static_cast<double>(xk.x) - P[0], ry = static_cast<double>(xk.y) - P[1], rz = static_cast<double>(xk.z) - P[2];
+    double* A = acc + 6 * static_cast<size_t>(decl[kb] - nStatic);
+    A[0] += F[0]; A[1] += F[1]; A[2] += F[2];
+    A[3] += ry * F[2] - rz * F[1]; A[4] += rz * F[0] - rx * F[2]; A[5] += rx * F[1] - ry * F[0];
+}
+
+extern "C" int sphk_bodies_react(sphk_ctx* c, const sphk_scene* s, float coef) {
+    SPHK_CHECK_SCENE(c, s);
+    if (!s->fluid.mass || !(coef - coef == 0.f)) return SPHK_ERR_INVALID;
+    if (!c->bodies || !c->bodies->acc || !c->boundarySearched || s->boundary.n != c->nB) return SPHK_ERR_STATE;
+    if (c->actCount >= 0 || c->rangeDev) return SPHK_ERR_STATE;    // slab ranks: bodies are single-context only
+    const BodyState* B = c->bodies;
+    // positions moved since the search (PBD corrections): a fluid particle within R of x_k may be listed two cells away
+    const int reach = c->posDirty ? 2 : 1;
+    k_bodies_react<<<sphk_blocks(c->nB), SPHK_BLOCK, 0, c->stream>>>(dev_scene(c, s), s->fluid.mass, B->local, B->decl, B->pose,
+                                                                    c->nB, B->nStatic, reach, coef, B->acc);
+    c->launches++;
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
 extern "C" int sphk_pbd_velocity_from_positions(sphk_ctx* c, const sphk_scene* s, const float* pos_last, float dt) {
     SPHK_CHECK_SCENE(c, s);
     if (!pos_last) return SPHK_ERR_INVALID;

@@ -153,10 +153,40 @@ class SphkOps:
         check(self.L.sphk_bodies_step(self.ctx, C.byref(p), _ptr(self.cs_boundary), C.c_float(self.p.dt)), "sphk_bodies_step")
 
     def set_body_motion(self, body: int, linear_velocity, angular_velocity):
-        """New motion of one body from the next step on (an asynchronous copy, like SPHSystem::setBodyMotion)."""
-        self.body_motion[body] = [*linear_velocity, *angular_velocity]
-        m = np.ascontiguousarray(self.body_motion, np.float32)
-        check(self.L.sphk_bodies_set_motion(self.ctx, m.ctypes.data_as(C.POINTER(C.c_float))), "sphk_bodies_set_motion")
+        """New motion of one body from the next step on (an asynchronous copy, like SPHSystem::setBodyMotion); the other
+        bodies keep their device-side (for dynamic bodies: integrated) motion."""
+        m = np.ascontiguousarray([*linear_velocity, *angular_velocity], np.float32)
+        check(self.L.sphk_bodies_set_body_motion(self.ctx, C.c_int(body), m.ctypes.data_as(C.POINTER(C.c_float))),
+              "sphk_bodies_set_body_motion")
+        self.body_motion[body] = m
+
+    # ---- two-way coupled bodies (DESIGN.md section 2.4) -----------------------------------------------------------------
+    bodies_dynamic = False
+
+    def bodies_react(self, c):
+        """The bodies' reaction to the sweep just run (sphk_bodies_react); nothing without dynamic bodies."""
+        if self.bodies_dynamic:
+            check(self.L.sphk_bodies_react(self.ctx, self._s(), C.c_float(float(c))), "sphk_bodies_react")
+
+    def bodies_integrate(self):
+        if self.bodies_dynamic:
+            check(self.L.sphk_bodies_integrate(self.ctx, C.c_float(self.p.dt), self._G), "sphk_bodies_integrate")
+
+    def current_body_motion(self) -> np.ndarray:
+        """(n_bodies, 6) motions {V, Omega} on the device (the integrated ones for dynamic bodies; the attribute body_motion
+        is the host copy of the prescribed motions); synchronises."""
+        out = np.zeros((self.n_bodies, 6), np.float32)
+        check(self.L.sphk_bodies_get_motion(self.ctx, out.ctypes.data_as(C.POINTER(C.c_float))), "sphk_bodies_get_motion")
+        return out
+
+    def body_impulse(self) -> np.ndarray:
+        """(n_bodies, 6) {J, H} the fluid gave each body over the last step (H about the body's centre; zero without dynamic
+        bodies, as SPHSystem::getBodyImpulse); synchronises."""
+        out = np.zeros((self.n_bodies, 6), np.float32)
+        if not self.bodies_dynamic:
+            return out
+        check(self.L.sphk_bodies_get_impulse(self.ctx, out.ctypes.data_as(C.POINTER(C.c_float))), "sphk_bodies_get_impulse")
+        return out
 
     def body_pose(self) -> np.ndarray:
         """(n_bodies, 7) poses {c, q = (x, y, z, w)}; synchronises."""
@@ -412,6 +442,7 @@ class SphkOps:
         self.pressure()
         self.sync_array(self.fluid.density); self.sync_array(self.fluid.pressure)
         self.pressure_force()
+        self.bodies_react(-np.float32(self.p.dt))
         self.advect()
 
     def step_dfsph(self):            # DFSPHSolver.cu:33-72
@@ -428,6 +459,7 @@ class SphkOps:
         total, it = 3.4e38, 0        # correctDivergenceError :331-363
         while (it < 1 or total > self.div_thr * n * rho0) and it < self.max_iter:
             self._run(self.dfsph_div_correct, "vel")
+            self.bodies_react(1.0)
             it += 1
             if it == self.max_iter:  # the loop ends whatever the error is, and nothing reads it again: dead sweep
                 break
@@ -456,10 +488,13 @@ class SphkOps:
         total, it = 3.4e38, 0        # project :160-210
         self.permute(self.warm, 1)
         self._run(lambda: self.dfsph_den_correct(self.warm), "vel")
+        inv_dt = np.float32(1.0) / np.float32(self.p.dt)
+        self.bodies_react(inv_dt)
         self._run(lambda: self.dfsph_den_error(False), "scalar", self.kappa)
         self.copy(self.warm, self.kappa)
         while (it < 2 or total > self.den_thr * n * rho0) and it < self.max_iter:
             self._run(self.dfsph_den_correct, "vel")
+            self.bodies_react(inv_dt)
             self._run(lambda: self.dfsph_den_error(True), "scalar", self.kappa)
             it += 1
             if it >= 2 and self.den_thr >= 0:
@@ -474,8 +509,10 @@ class SphkOps:
             return False
         self.set_use_list(self.use_list, 150 if self.use_list else 0)   # skin list: positions move inside the step
         self.permute(self.pos_last, 3)
+        c = np.float32(1.0) / (np.float32(self.p.rho0) * np.float32(self.p.dt))
         for _ in range(self.max_iter):
             self._run(self.pbd_density_lambda, "scalar", self.lam)
+            self.bodies_react(c)     # before the positions move: the pairs of this correction
             self.pbd_delta_pos_apply(); self.sync_positions()
         self.pbd_velocity_from_positions()
         vort = self.vorticity_eps > 0
@@ -516,9 +553,11 @@ class SphkOps:
         if self.solver == "dfsph":
             self.step_dfsph()
         elif self.solver == "pbd":
-            self.step_pbd()
+            if not self.step_pbd():
+                return           # the "throwing" first call: no sweep ran, nothing to integrate (as in SPHSystem::step)
         else:
             self.step_wcsph()
+        self.bodies_integrate()
 
     def state(self) -> dict:
         self.synchronize()
@@ -547,9 +586,12 @@ class SphkSystem(SphkOps):
 
     def __init__(self, scene, device="cuda:0", use_list: bool | None = None, list_capacity: int | None = None,
                  step0: bool = True, bodies=None):
-        """bodies: kinematic rigid bodies (DESIGN.md section 2.3), a list of dicts with "points" (k, 3) body coordinates,
+        """bodies: rigid bodies (DESIGN.md sections 2.3, 2.4), a list of dicts with "points" (k, 3) body coordinates,
         "position" (3,), "orientation" (x, y, z, w) unit quaternion, "linear_velocity" (3,), "angular_velocity" (3,) in the
-        world frame.  Their particles follow the static boundary set; every step() moves them before the fluid search."""
+        world frame, and optionally "mass" (> 0: dynamic, two-way coupled; default 0: kinematic, and held -- its reaction reported --
+        when another body is dynamic) and "inertia" (3,) principal
+        moments about the centre in the axes of "points".  Masses are in the fluid's units, m0 / spacing^3 per unit volume
+        (not rho0).  Their particles follow the static boundary set; every step() moves them before the fluid search."""
         self.L = capi.sphk()
         self.p = scene.params
         self.device = torch.device(device)
@@ -597,6 +639,10 @@ class SphkSystem(SphkOps):
             check(self.L.sphk_bodies_init(self.ctx, C.byref(p), C.c_int(int(self._body_begin[0])), C.c_int(self.n_bodies),
                                           self._body_begin, fp(self._body_local), fp(self._body_pose), fp(self.body_motion)),
                   "sphk_bodies_init")
+            mi = capi.body_mass_inertia(bodies)
+            if (mi[:, 0] > 0).any():     # as SPHSystem: held bodies (mass 0) then report their reaction too
+                check(self.L.sphk_bodies_set_dynamics(self.ctx, fp(mi), self._space), "sphk_bodies_set_dynamics")
+                self.bodies_dynamic = True
         # SPHSystem.cu:68-76 (with bodies the boundary search also places them at their initial pose)
         self.search_boundary()
         self.boundary_mass()

@@ -120,17 +120,15 @@ extern "C" sph_app* sph_app_create(const float* fluid_xyz, int n_fluid, const fl
     return create(fluid_xyz, n_fluid, boundary_xyz, n_boundary, p, nullptr);
 }
 
-extern "C" sph_app* sph_app_create_with_bodies(const float* fluid_xyz, int n_fluid, const float* boundary_xyz, int n_boundary,
-                                               int n_bodies, const int* body_begin, const float* body_xyz, const float* pose,
-                                               const float* motion, const sph_app_params* p) {
-#ifdef SPH_APP_REFERENCE_ENGINE
-    (void)fluid_xyz; (void)n_fluid; (void)boundary_xyz; (void)n_boundary; (void)n_bodies; (void)body_begin; (void)body_xyz;
-    (void)pose; (void)motion; (void)p;
-    return nullptr;
-#else
+#ifndef SPH_APP_REFERENCE_ENGINE
+// the bodies of sph_app_create_with_bodies / _with_dynamic_bodies (mass_inertia: null = all kinematic)
+static sph_app* create_with_bodies(const float* fluid_xyz, int n_fluid, const float* boundary_xyz, int n_boundary, int n_bodies,
+                                   const int* body_begin, const float* body_xyz, const float* pose, const float* motion,
+                                   const float* mass_inertia, const sph_app_params* p) {
     if (n_bodies < 0 || (n_bodies > 0 && (!body_begin || !body_xyz || !pose || !motion)) || (n_bodies > 0 && body_begin[0] != 0))
         return nullptr;
     body_list bodies(static_cast<size_t>(n_bodies));
+    bool dynamic = false;
     for (int b = 0; b < n_bodies; ++b) {
         if (body_begin[b + 1] < body_begin[b]) return nullptr;
         auto& k = bodies[b];
@@ -141,10 +139,44 @@ extern "C" sph_app* sph_app_create_with_bodies(const float* fluid_xyz, int n_flu
         k.orientation = make_float4(P[3], P[4], P[5], P[6]);
         k.linearVelocity = make_float3(M[0], M[1], M[2]);
         k.angularVelocity = make_float3(M[3], M[4], M[5]);
+        if (mass_inertia) {
+            const float* D = mass_inertia + 4 * b;
+            k.mass = D[0];
+            k.inertia = make_float3(D[1], D[2], D[3]);
+            dynamic = dynamic || D[0] > 0.0f;
+        }
     }
     sph_app* app = create(fluid_xyz, n_fluid, boundary_xyz, n_boundary, p, &bodies);
-    if (app && app->system->bodyCount() != n_bodies) { delete app; return nullptr; }   // sphk_bodies_init refused them
+    // sphk_bodies_init or sphk_bodies_set_dynamics refused them
+    if (app && (app->system->bodyCount() != n_bodies || app->system->bodiesDynamic() != dynamic)) { delete app; return nullptr; }
     return app;
+}
+#endif
+
+extern "C" sph_app* sph_app_create_with_bodies(const float* fluid_xyz, int n_fluid, const float* boundary_xyz, int n_boundary,
+                                               int n_bodies, const int* body_begin, const float* body_xyz, const float* pose,
+                                               const float* motion, const sph_app_params* p) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)fluid_xyz; (void)n_fluid; (void)boundary_xyz; (void)n_boundary; (void)n_bodies; (void)body_begin; (void)body_xyz;
+    (void)pose; (void)motion; (void)p;
+    return nullptr;
+#else
+    return create_with_bodies(fluid_xyz, n_fluid, boundary_xyz, n_boundary, n_bodies, body_begin, body_xyz, pose, motion, nullptr, p);
+#endif
+}
+
+extern "C" sph_app* sph_app_create_with_dynamic_bodies(const float* fluid_xyz, int n_fluid, const float* boundary_xyz,
+                                                       int n_boundary, int n_bodies, const int* body_begin, const float* body_xyz,
+                                                       const float* pose, const float* motion, const float* mass_inertia,
+                                                       const sph_app_params* p) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)fluid_xyz; (void)n_fluid; (void)boundary_xyz; (void)n_boundary; (void)n_bodies; (void)body_begin; (void)body_xyz;
+    (void)pose; (void)motion; (void)mass_inertia; (void)p;
+    return nullptr;
+#else
+    if (!mass_inertia) return nullptr;
+    return create_with_bodies(fluid_xyz, n_fluid, boundary_xyz, n_boundary, n_bodies, body_begin, body_xyz, pose, motion,
+                              mass_inertia, p);
 #endif
 }
 
@@ -176,6 +208,25 @@ extern "C" int sph_app_body_pose(sph_app* app, int body, float* pose) {
     return 0;
 #endif
 }
+
+static int body_pair(sph_app* app, int body, float* out, bool impulse) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)body; (void)out; (void)impulse;
+    return 1;
+#else
+    if (!app || !out || body < 0 || body >= app->system->bodyCount()) return 1;
+    float3 a, b;
+    if (impulse) app->system->getBodyImpulse(body, a, b);
+    else app->system->getBodyMotion(body, a, b);
+    const float v[6] = {a.x, a.y, a.z, b.x, b.y, b.z};
+    std::copy(v, v + 6, out);
+    return 0;
+#endif
+}
+
+extern "C" int sph_app_body_motion(sph_app* app, int body, float* motion) { return body_pair(app, body, motion, false); }
+
+extern "C" int sph_app_body_impulse(sph_app* app, int body, float* impulse) { return body_pair(app, body, impulse, true); }
 
 extern "C" void sph_app_destroy(sph_app* app) { delete app; }
 

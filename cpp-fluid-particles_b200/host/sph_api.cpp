@@ -70,6 +70,7 @@ bool BasicSPHSolver::beginStep(std::shared_ptr<SPHParticles>& fluids, const std:
     current_.abi.cell_start_fluid = cellStartFluid.addr();
     current_.abi.cell_start_boundary = cellStartBoundary.addr();
     current_.abi.radius = radius;
+    reacting_ = eng->bodiesDynamic;
     check(sphk_set_option(current_.ctx, SPHK_OPT_NEIGHBOR_LIST, neighborList ? 1 : 0), "sphk_set_option");
     check(sphk_set_option(current_.ctx, SPHK_OPT_LIST_SKIN, listSkinPermille), "sphk_set_option");
     if (eng->shadowsStale) { check(sphk_refresh(current_.ctx, &current_.abi), "sphk_refresh"); eng->shadowsStale = false; }
@@ -95,6 +96,7 @@ void BasicSPHSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shar
         check(sphk_pressure(current_.ctx, &current_.abi, rho0, stiff), "sphk_pressure");
         produced(0, fluids->getDensityPtr(), 1); produced(0, fluids->getPressurePtr(), 1);
         check(sphk_pressure_force(current_.ctx, &current_.abi, dt), "sphk_pressure_force");
+        react(-dt);
     } else {
         if (vorticityOn()) vorticity(rho0);
         diffuse(fluids, cellStartFluid, cellSize, cellLength, rho0, radius, visc, dt);
@@ -189,6 +191,7 @@ void BasicSPHSolver::project(std::shared_ptr<SPHParticles>&, const std::shared_p
     check(sphk_pressure(current_.ctx, &current_.abi, rho0, stiff), "sphk_pressure");
     produced(0, current_.abi.fluid.density, 1); produced(0, current_.abi.fluid.pressure, 1);
     check(sphk_pressure_force(current_.ctx, &current_.abi, dt), "sphk_pressure_force");
+    react(-dt);
 }
 
 // :211-225
@@ -269,6 +272,7 @@ int DFSPHSolver::correctDivergenceError(float rho0, float dt, float errorThresho
         check(sphk_loop_begin(ctx, 0, 1, maxIter_, errorThreshold * num * rho0, 1), "sphk_loop_begin");
         for (int k = 0; k < maxIter_; ++k) {
             check(sphk_dfsph_div_correct(ctx, &current_.abi, bufferFloat.addr()), "sphk_dfsph_div_correct");
+            react(1.0f);
             check(sphk_dfsph_div_error(ctx, &current_.abi, alpha.addr(), error.addr(), bufferFloat.addr(), dt, rho0),
                   "sphk_dfsph_div_error");
             check(sphk_loop_next(ctx, 0, error.addr(), num), "sphk_loop_next");
@@ -278,6 +282,7 @@ int DFSPHSolver::correctDivergenceError(float rho0, float dt, float errorThresho
     }
     while ((iter < 1 || totalError > errorThreshold * thresholdCount * rho0) && iter < maxIter_) {
         check(sphk_dfsph_div_correct(ctx, &current_.abi, bufferFloat.addr()), "sphk_dfsph_div_correct");
+        react(1.0f);
         produced(1, current_.abi.fluid.vel, 3);
         ++iter;
         // After the last permitted iteration the loop ends whatever the error is, and nothing reads this error, stiffness or
@@ -305,6 +310,7 @@ int DFSPHSolver::project(std::shared_ptr<SPHParticles>& fluids, const std::share
     check(sphk_permute(ctx, denWarmStiff.addr(), 1, num), "sphk_permute");
     // (ghost particles carry their warm stiffness with them: it travels with the candidates and is permuted with the rest)
     check(sphk_dfsph_den_correct(ctx, &current_.abi, denWarmStiff.addr(), dt), "sphk_dfsph_den_correct");
+    react(1.0f / dt);
     produced(1, current_.abi.fluid.vel, 3);
     check(sphk_dfsph_den_error(ctx, &current_.abi, alpha.addr(), error.addr(), bufferFloat.addr(), dt, rho0, nullptr),
           "sphk_dfsph_den_error");
@@ -315,6 +321,7 @@ int DFSPHSolver::project(std::shared_ptr<SPHParticles>& fluids, const std::share
         check(sphk_loop_begin(ctx, 1, 2, maxIter_, errorThreshold * num * rho0, 2), "sphk_loop_begin");
         for (int k = 0; k < maxIter_; ++k) {
             check(sphk_dfsph_den_correct(ctx, &current_.abi, bufferFloat.addr(), dt), "sphk_dfsph_den_correct");
+            react(1.0f / dt);
             check(sphk_dfsph_den_error(ctx, &current_.abi, alpha.addr(), error.addr(), bufferFloat.addr(), dt, rho0,
                                        denWarmStiff.addr()),
                   "sphk_dfsph_den_error");                                                // + :199-203 fused
@@ -325,6 +332,7 @@ int DFSPHSolver::project(std::shared_ptr<SPHParticles>& fluids, const std::share
     }
     while ((iter < 2 || totalError > errorThreshold * thresholdCount * rho0) && iter < maxIter_) {
         check(sphk_dfsph_den_correct(ctx, &current_.abi, bufferFloat.addr(), dt), "sphk_dfsph_den_correct");
+        react(1.0f / dt);
         produced(1, current_.abi.fluid.vel, 3);
         check(sphk_dfsph_den_error(ctx, &current_.abi, alpha.addr(), error.addr(), bufferFloat.addr(), dt, rho0,
                                    denWarmStiff.addr()),
@@ -373,6 +381,7 @@ void PBDSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shared_pt
     // displacement on the device and falls back to the cell walk if the corrections ever exceed skin/2
     if (!beginStep(fluids, boundaries, cellStartFluid, cellStartBoundary, radius, true, 150)) return;
     updateNeighborhood(fluids);
+    reactCoef_ = 1.0f / (rho0 * dt);
     project(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, cellSize, spaceSize, cellLength, radius, maxIter);
     check(sphk_pbd_velocity_from_positions(current_.ctx, &current_.abi, reinterpret_cast<float*>(fluidPosLast.addr()), dt),
           "sphk_pbd_velocity_from_positions");
@@ -436,6 +445,7 @@ int PBDSolver::project(std::shared_ptr<SPHParticles>&, const std::shared_ptr<SPH
         check(sphk_pbd_density_lambda(current_.ctx, &current_.abi, bufferFloat.addr(), rho0, relaxation),
               "sphk_pbd_density_lambda");
         produced(2, bufferFloat.addr(), 1);
+        react(reactCoef_);      // before the positions move: the pairs of this correction
         check(sphk_pbd_delta_pos_apply(current_.ctx, &current_.abi, bufferFloat.addr(),
                                        reinterpret_cast<float*>(bufferFloat3.addr()), rho0, sp),
               "sphk_pbd_delta_pos_apply");
@@ -507,6 +517,15 @@ SPHSystem::SPHSystem(std::shared_ptr<SPHParticles>& fluidParticles, std::shared_
                                         local.data(), pose.data(), motion.data());
         check(rc, "sphk_bodies_init");
         if (rc == 0) _bodyMotion = motion;
+        const bool dynamic = std::any_of(bodies.begin(), bodies.end(), [](const sphb200::KinematicBody& b) { return b.mass > 0.0f; });
+        if (rc == 0 && dynamic) {
+            std::vector<float> mi;
+            for (const auto& b : bodies) mi.insert(mi.end(), {b.mass, b.inertia.x, b.inertia.y, b.inertia.z});
+            const float sp[3] = {spaceSize.x, spaceSize.y, spaceSize.z};
+            const int rd = sphk_bodies_set_dynamics(_engine->ctx(), mi.data(), sp);
+            check(rd, "sphk_bodies_set_dynamics");
+            _bodiesDynamic = _engine->bodiesDynamic = rd == 0;
+        }
     }
     // SPHSystem.cu:68-76 (with bodies the boundary search also places them at their initial pose)
     neighborSearch(_boundaries, cellStartBoundary);
@@ -548,15 +567,41 @@ void SPHSystem::searchForStep() {
     neighborSearch(_fluids, cellStartFluid);
 }
 
+// the end of a step with dynamic bodies (after the solver's last reaction, inside a captured step graph)
+void SPHSystem::integrateBodies() {
+    if (!_bodiesDynamic) return;
+    const float g[3] = {_sphG.x, _sphG.y, _sphG.z};
+    check(sphk_bodies_integrate(_engine->ctx(), _dt, g), "sphk_bodies_integrate");
+}
+
 void SPHSystem::setBodyMotion(int body, float3 linearVelocity, float3 angularVelocity) {
     if (body < 0 || body >= bodyCount()) { printf("setBodyMotion: no body %d (the system has %d)\n", body, bodyCount()); return; }
     if (!_engine->ok()) return;
-    std::vector<float> motion = _bodyMotion;
     const float m[6] = {linearVelocity.x, linearVelocity.y, linearVelocity.z, angularVelocity.x, angularVelocity.y, angularVelocity.z};
-    std::copy(m, m + 6, motion.begin() + 6 * body);
-    const int rc = sphk_bodies_set_motion(_engine->ctx(), motion.data());   // refuses non-finite values: the motion is kept
-    check(rc, "sphk_bodies_set_motion");
-    if (rc == 0) _bodyMotion = motion;
+    // this body only: the host copy of a dynamic body's motion is stale, the device holds the integrated one
+    const int rc = sphk_bodies_set_body_motion(_engine->ctx(), body, m);   // refuses non-finite values: the motion is kept
+    check(rc, "sphk_bodies_set_body_motion");
+    if (rc == 0) std::copy(m, m + 6, _bodyMotion.begin() + 6 * body);
+}
+
+void SPHSystem::getBodyMotion(int body, float3& linearVelocity, float3& angularVelocity) const {
+    if (body < 0 || body >= bodyCount()) { printf("getBodyMotion: no body %d (the system has %d)\n", body, bodyCount()); return; }
+    std::vector<float> motion(6 * static_cast<size_t>(bodyCount()));
+    if (!_engine->ok()) return;
+    check(sphk_bodies_get_motion(_engine->ctx(), motion.data()), "sphk_bodies_get_motion");
+    const float* M = motion.data() + 6 * body;
+    linearVelocity = make_float3(M[0], M[1], M[2]);
+    angularVelocity = make_float3(M[3], M[4], M[5]);
+}
+
+void SPHSystem::getBodyImpulse(int body, float3& linearImpulse, float3& angularImpulse) const {
+    if (body < 0 || body >= bodyCount()) { printf("getBodyImpulse: no body %d (the system has %d)\n", body, bodyCount()); return; }
+    std::vector<float> imp(6 * static_cast<size_t>(bodyCount()), 0.0f);
+    if (!_engine->ok()) return;
+    if (_bodiesDynamic) check(sphk_bodies_get_impulse(_engine->ctx(), imp.data()), "sphk_bodies_get_impulse");
+    const float* I = imp.data() + 6 * body;
+    linearImpulse = make_float3(I[0], I[1], I[2]);
+    angularImpulse = make_float3(I[3], I[4], I[5]);
 }
 
 void SPHSystem::getBodyPose(int body, float3& position, float4& orientation) const {
@@ -620,6 +665,7 @@ float SPHSystem::step() {
             _solver->step(_fluids, _boundaries, cellStartFluid, cellStartBoundary, _spaceSize, _cellSize, _sphCellLength,
                           _sphSmoothingRadius, _dt, _sphRho0, _sphRhoBoundary, _sphStiff, _sphVisc, _sphG,
                           _sphSurfaceTensionIntensity, _sphAirPressure);
+            integrateBodies();
             ok = true;
         } catch (const char* s) {
             std::cout << s << "\n";
@@ -643,6 +689,7 @@ float SPHSystem::step() {
                     _solver->step(_fluids, _boundaries, cellStartFluid, cellStartBoundary, _spaceSize, _cellSize,
                                   _sphCellLength, _sphSmoothingRadius, _dt, _sphRho0, _sphRhoBoundary, _sphStiff, _sphVisc,
                                   _sphG, _sphSurfaceTensionIntensity, _sphAirPressure);
+                    integrateBodies();
                 } catch (const char* s) {
                     std::cout << s << "\n";
                 } catch (...) {

@@ -61,19 +61,25 @@ public:
     cudaStream_t stream() const { return stream_; }
     bool ok() const { return ctx_ != nullptr; }
     bool shadowsStale = false;   // set when a caller moved particles behind the engine's back
+    bool bodiesDynamic = false;  // set by SPHSystem: the solvers follow every reacting sweep with sphk_bodies_react
 private:
     sphk_ctx* ctx_ = nullptr;
     cudaStream_t stream_ = nullptr;
 };
 
-// addition: a kinematic rigid body (DESIGN.md section 2.3).  Its boundary particles are `points` in body coordinates; the
-// system moves them every step by the prescribed motion (the fluid pushes back on nothing: one-way coupling).
+// addition: a rigid body (DESIGN.md sections 2.3, 2.4).  Its boundary particles are `points` in body coordinates; the
+// system moves them every step.  With mass = 0 (the default) the motion is prescribed (a kinematic body).  With mass > 0
+// the fluid pushes back: the body is integrated under the fluid's force and torque and gravity, and meets the walls.
+// Mass units: the fluid's mass per unit volume is m0 / spacing^3 (about 9.57 in the reference's scenes), not rho0, so a
+// body of relative density REL and volume V has mass = REL * m0 / spacing^3 * V.
 struct KinematicBody {
-    std::vector<float3> points;     // r_k, body coordinates
-    float3 position;                // centre c, world frame
+    std::vector<float3> points;     // r_k, body coordinates (the principal axes of a dynamic body)
+    float3 position;                // centre c, world frame (the centre of mass of a dynamic body)
     float4 orientation;             // unit quaternion q = (x, y, z, w): vector part in x, y, z, scalar part in w
     float3 linearVelocity;          // V, world frame
     float3 angularVelocity;         // Omega (rad/s), world frame, about the centre
+    float mass = 0;                 // M > 0: dynamic (two-way coupled); 0: kinematic
+    float3 inertia = {0, 0, 0};     // principal moments about the centre, body axes (all > 0 when mass > 0)
 };
 }  // namespace sphb200
 
@@ -250,6 +256,9 @@ protected:
     float* omegaNormBuffer() const { return omegaNorm_->addr(); }
     void vorticity(float rho0);
     void confine(const std::shared_ptr<SPHParticles>& fluids, float rho0, float dt);
+    // two-way coupled bodies: the reaction of the sweep just run, with its c (sphk_bodies_react); nothing without dynamic bodies
+    void react(float c) { if (reacting_) sphb200::check(sphk_bodies_react(current_.ctx, &current_.abi, c), "sphk_bodies_react"); }
+    bool reacting_ = false;
 private:
     DArray<float3> bufferFloat3;   // viscosity deltaV, then colour gradient (BasicSPHSolver.h:43)
     DArray<float3> bufferColorGrad;   // addition: the fused viscosity+surface sweep needs both at once
@@ -337,6 +346,7 @@ protected:
                          float cellLength, float rho0, float radius, float visc);
 private:
     void updateNeighborhood(const std::shared_ptr<SPHParticles>& particles);
+    float reactCoef_ = 0.0f;       // 1 / (rho0 dt) of the step in flight: c of the position-correction reaction
     bool posLastInitialized = false;
     const int maxIter;
     const float xSPH_c;
@@ -387,6 +397,12 @@ public:
     int bodyCount() const { return static_cast<int>(_bodyMotion.size() / 6); }
     void setBodyMotion(int body, float3 linearVelocity, float3 angularVelocity);
     void getBodyPose(int body, float3& position, float4& orientation) const;
+    // two-way coupled bodies (any body with mass > 0): the current motion (the integrated one for a dynamic body), and the
+    // {J, H} the fluid gave a body over the last step (held bodies included; zero without dynamic bodies).  Both synchronise
+    // and print and ignore an out-of-range body index.
+    void getBodyMotion(int body, float3& linearVelocity, float3& angularVelocity) const;
+    void getBodyImpulse(int body, float3& linearImpulse, float3& angularImpulse) const;
+    bool bodiesDynamic() const { return _bodiesDynamic; }   // the dynamics were declared (false if the engine refused them)
 
 private:
     std::shared_ptr<SPHParticles> _fluids;
@@ -418,8 +434,10 @@ private:
     unsigned int solverConfigEpoch() const;
     void dropStepGraph();
     std::vector<float> _bodyMotion;       // host copy of all bodies' motions (6 floats each); empty: no bodies
+    bool _bodiesDynamic = false;          // some body has mass > 0: sphk_bodies_integrate ends every step
     void computeBoundaryMass();
     void searchForStep();                 // bodies (if any), then the fluid search
+    void integrateBodies();               // sphk_bodies_integrate at the end of a step with dynamic bodies
     void neighborSearch(const std::shared_ptr<SPHParticles>& particles, DArray<int>& cellStart);
 };
 

@@ -89,6 +89,19 @@ sph_app* sph_app_create_with_bodies(const float* fluid_xyz, int n_fluid, const f
 int   sph_app_set_body_motion(sph_app* app, int body, const float* linear_velocity_xyz, const float* angular_velocity_xyz);
 /* current pose of one body, float[7] as above (synchronises) */
 int   sph_app_body_pose(sph_app* app, int body, float* pose);
+/* Two-way coupled rigid bodies (DESIGN.md section 2.4): sph_app_create_with_bodies plus mass_inertia[4 b ..] = {M, Ix, Iy, Iz}
+ * per body (sphb200::KinematicBody::mass and ::inertia; principal moments about the centre in the axes of body_xyz).  M > 0
+ * makes a body dynamic (the fluid pushes it; gravity and wall contact apply) and needs I > 0; M = 0 keeps it kinematic and
+ * its reaction is still reported.  Masses are in the fluid's units: m0 / spacing^3 per unit volume (not rho0).  NULL on the
+ * reference build and when the engine refuses the bodies or their dynamics. */
+sph_app* sph_app_create_with_dynamic_bodies(const float* fluid_xyz, int n_fluid, const float* boundary_xyz, int n_boundary,
+                                            int n_bodies, const int* body_begin, const float* body_xyz, const float* pose,
+                                            const float* motion, const float* mass_inertia, const sph_app_params* params);
+/* current motion of one body, float[6] = {V, Omega} (the integrated one for a dynamic body); synchronises */
+int   sph_app_body_motion(sph_app* app, int body, float* motion);
+/* {Jx, Jy, Jz, Hx, Hy, Hz}: the impulse and angular impulse about the centre the fluid gave one body over the last step
+ * (zero without dynamic bodies); synchronises */
+int   sph_app_body_impulse(sph_app* app, int body, float* impulse);
 /* Name of the engine underneath: "reference-cuda" or "b200-native". */
 const char* sph_app_engine(void);
 

@@ -290,6 +290,41 @@ int sphk_bodies_get_pose(sphk_ctx* ctx, float* pose_host);
  * 0 = static, b + 1 = body b) */
 int sphk_bodies_get_local(sphk_ctx* ctx, float* local_out);
 
+/* ---- two-way coupled bodies (no reference counterpart; DESIGN.md section 2.4) ------------------------------------------------
+ * The fluid pushes back on bodies: every sweep whose boundary term changes fluid momentum, c m_i m_k s_i gradW(x_i - x_k) for
+ * a fluid particle i and a body particle k, is followed by sphk_bodies_react with its c; the body gathers the opposite
+ * impulse J and its moment H about the body's centre.  sphk_bodies_integrate then moves the dynamic bodies at the end of the
+ * step.
+ *
+ * sphk_bodies_set_dynamics declares the bodies' masses and principal moments, mass_inertia = {M, Ix, Iy, Iz} per body (host
+ * float[4 * n_bodies]), the moments about the centre in body axes (the axes of r_k).  M > 0 makes a body dynamic and needs
+ * I > 0; M = 0 keeps it kinematic ("held"), its reaction is still gathered and reported (a force sensor).  Mass units are
+ * those of the fluid's momentum: a fluid particle of mass m0 stands for a volume spacing^3, so the fluid's mass per unit
+ * volume is m0 / spacing^3 (about 9.57 in the reference's scenes), NOT rho0; a body of relative density REL and volume V has
+ * M = REL * m0 / spacing^3 * V.  space = the domain size: dynamic bodies stay inside the fluid's clamp box
+ * [0, 0.99 space] per axis (the corners of the body-frame bounding box of r_k; the centre is moved back and the outward
+ * velocity zeroed at each pose update; no friction, no torque; bodies pass through each other).  Call it once, after
+ * sphk_bodies_init and before the first sphk_bodies_step (SPHK_ERR_STATE otherwise).  Synchronises.
+ * A system that never calls it launches nothing new. */
+int sphk_bodies_set_dynamics(sphk_ctx* ctx, const float* mass_inertia, const float space[3]);
+/* Gathers the reaction of the sweep just run, per body particle, from the fluid records' scalar s_i and positions and the
+ * fluid masses (scene->fluid.mass):  c = -dt after sphk_pressure_force; 1 after sphk_dfsph_div_correct; 1/dt after
+ * sphk_dfsph_den_correct (warm start included); 1/(rho0 dt) between sphk_pbd_density_lambda and sphk_pbd_delta_pos_apply.
+ * Returns at once inside a device-controlled loop that has ended, like the sweeps.  Reads the records only.  SPHK_ERR_STATE
+ * before sphk_bodies_set_dynamics and under an active range (slab ranks). */
+int sphk_bodies_react(sphk_ctx* ctx, const sphk_scene* scene, float c);
+/* End of step: the gathered {J, H} of every body become the reported impulse (sphk_bodies_get_impulse) and are cleared; a
+ * dynamic body's motion becomes V += J / M + dt G, Omega = (R diag(I) R^T)^-1 (R diag(I) R^T Omega + H), R from the current
+ * pose.  The next sphk_bodies_step moves it.  dt > 0, G finite. */
+int sphk_bodies_integrate(sphk_ctx* ctx, float dt, const float G[3]);
+/* New motion {V, Omega} of one body (host float[6]), enqueued like sphk_bodies_set_motion; the other bodies keep their
+ * device-side motion (the integrated one, for dynamic bodies). */
+int sphk_bodies_set_body_motion(sphk_ctx* ctx, int body, const float motion[6]);
+/* current motions (host float[6 * n_bodies]); synchronises */
+int sphk_bodies_get_motion(sphk_ctx* ctx, float* motion_host);
+/* {Jx, Jy, Jz, Hx, Hy, Hz} per body of the last integrated step (host float[6 * n_bodies]; J / dt is the mean force); synchronises */
+int sphk_bodies_get_impulse(sphk_ctx* ctx, float* impulse_host);
+
 /* Builds the per-step neighbour list now (sweeps otherwise build it lazily on first use). */
 int sphk_build_neighbor_list(sphk_ctx* ctx, const sphk_scene* s);
 
