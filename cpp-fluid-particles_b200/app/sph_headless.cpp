@@ -9,9 +9,12 @@
 //
 //   sph_headless [--solver sph|dfsph|pbd] [--frames N] [--box L | --box LX LY LZ] [--block NX NY NZ] [--origin X Y Z]
 //                [--dt DT] [--iters K] [--vorticity EPS] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] [--ranks N [--rank R --rendezvous DIR]]
-//                [--bullets K] [--stir OMEGA] [--float REL]
+//                [--bullets K] [--stir OMEGA] [--float REL] [--implicit-viscosity NU]
 // --vorticity EPS turns on vorticity confinement of strength EPS (BasicSPHSolver::setVorticityConfinement) after the
 // constructor's step 0, for every solver and with --ranks.
+// --implicit-viscosity NU turns on the implicit viscosity solve (BasicSPHSolver::setImplicitViscosity) with nu = nu_boundary = NU
+// after the constructor's step 0, for every solver: walls and a --stir paddle drag the fluid (no-slip).  Single GPU only, and not
+// together with --float (the viscous wall force is not part of a dynamic body's reaction).
 // --stir OMEGA adds one kinematic body (SPHSystem's constructor with a KinematicBody): a flat vertical paddle through the
 // centre of the fluid block, rotating about y at OMEGA rad/s.  It is two layers of the boundary lattice's spacing thick
 // (normal along z), 60 % of the block's x extent wide and as tall as the block; fluid lattice points within one spacing of
@@ -69,6 +72,7 @@ struct Options {
     std::string dump, emitScene;
     bool quiet = false;
     float vorticity = 0.0f;                   // --vorticity EPS: vorticity confinement from frame 1 on (0: off)
+    float implicitNu = 0.0f;                  // --implicit-viscosity NU: implicit viscosity from frame 1 on (0: off)
     bool stir = false;                        // --stir OMEGA: a paddle rotating about y at OMEGA rad/s
     float stirOmega = 0.0f;
     bool floating = false;                    // --float REL: a free cube of relative density REL
@@ -91,6 +95,7 @@ bool parse(int argc, char** argv, Options& o) {
         else if (a == "--quiet") o.quiet = true;
         else if (a == "--bullets" && need(i, 1)) o.bullets = std::atoi(argv[++i]);
         else if (a == "--vorticity" && need(i, 1)) o.vorticity = static_cast<float>(std::atof(argv[++i]));
+        else if (a == "--implicit-viscosity" && need(i, 1)) o.implicitNu = static_cast<float>(std::atof(argv[++i]));
         else if (a == "--stir" && need(i, 1)) { o.stir = true; o.stirOmega = static_cast<float>(std::atof(argv[++i])); }
         else if (a == "--float" && need(i, 1)) { o.floating = true; o.floatRel = static_cast<float>(std::atof(argv[++i])); }
         else if (a == "--ranks" && need(i, 1)) o.ranks = std::atoi(argv[++i]);
@@ -119,6 +124,14 @@ bool parse(int argc, char** argv, Options& o) {
     if (o.floating && (o.ranks > 1 || o.stir || !(o.floatRel > 0.0f) || !std::isfinite(o.floatRel))) {
         std::fprintf(stderr, "sph_headless: --float REL needs REL > 0, runs on one GPU only (bodies are not supported with --ranks) "
                              "and not together with --stir\n");
+        return false;
+    }
+    if (!(o.implicitNu >= 0.0f) || !std::isfinite(o.implicitNu)) {
+        std::fprintf(stderr, "sph_headless: --implicit-viscosity NU needs a finite NU >= 0\n");
+        return false;
+    }
+    if (o.implicitNu > 0.0f && (o.ranks > 1 || o.floating)) {
+        std::fprintf(stderr, "sph_headless: --implicit-viscosity runs on one GPU only (not with --ranks) and not together with --float\n");
         return false;
     }
     return o.frames >= 0 && o.vorticity >= 0.0f && o.block[0] > 0 && o.block[1] > 0 && o.block[2] > 0 &&
@@ -265,7 +278,7 @@ int main(int argc, char** argv) {
     Options o;
     if (!parse(argc, argv, o)) {
         std::fprintf(stderr, "usage: sph_headless [--solver sph|dfsph|pbd] [--frames N] [--box L | LX LY LZ] [--block NX NY NZ] "
-                             "[--origin X Y Z] [--dt DT] [--iters K] [--vorticity EPS] [--stir OMEGA | --float REL] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] "
+                             "[--origin X Y Z] [--dt DT] [--iters K] [--vorticity EPS] [--implicit-viscosity NU] [--stir OMEGA | --float REL] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] "
                              "[--ranks N [--rank R --rendezvous DIR]]\n");
         return 2;
     }
@@ -391,6 +404,7 @@ int main(int argc, char** argv) {
     }
 
     if (o.vorticity > 0.0f) basicSolver->setVorticityConfinement(o.vorticity);
+    if (o.implicitNu > 0.0f) basicSolver->setImplicitViscosity(o.implicitNu, o.implicitNu);
 
     if (o.bullets > 0) {
         const int hit = slab ? shoot(o, sphSpacing, dt, pSlab->getFluids(), static_cast<size_t>(pSlab->ownedBegin()), static_cast<size_t>(pSlab->size()))

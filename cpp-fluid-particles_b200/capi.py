@@ -33,13 +33,16 @@ SPHK_FUNCTIONS = [
     "sphk_bodies_init", "sphk_bodies_set_motion", "sphk_bodies_step", "sphk_bodies_get_pose", "sphk_bodies_get_local",
     "sphk_bodies_set_dynamics", "sphk_bodies_react", "sphk_bodies_integrate", "sphk_bodies_set_body_motion",
     "sphk_bodies_get_motion", "sphk_bodies_get_impulse",
+    "sphk_implicit_viscosity_work_floats", "sphk_implicit_viscosity", "sphk_implicit_viscosity_stats", "sphk_visc_implicit_setup",
+    "sphk_visc_implicit_matvec",
 ]
 SPH_APP_FUNCTIONS = [
     "sph_app_create", "sph_app_destroy", "sph_app_step", "sph_app_fluid_size", "sph_app_boundary_size",
     "sph_app_download_fluid", "sph_app_download_boundary", "sph_app_upload_fluid", "sph_app_engine",
     "sph_app_submit", "sph_app_wait", "sph_app_dfsph_iterations", "sph_app_set_option", "sph_app_set_vorticity",
     "sph_app_create_with_bodies", "sph_app_set_body_motion", "sph_app_body_pose", "sph_app_step_graph_active",
-    "sph_app_create_with_dynamic_bodies", "sph_app_body_motion", "sph_app_body_impulse",
+    "sph_app_create_with_dynamic_bodies", "sph_app_body_motion", "sph_app_body_impulse", "sph_app_set_implicit_viscosity",
+    "sph_app_viscosity_stats",
 ]
 
 OPT_NEIGHBOR_LIST, OPT_LIST_CAPACITY, OPT_LIST_SKIN, OPT_SIMPLE_LIST_BUILD, OPT_TILE, OPT_STAGED_LIST_BUILD, OPT_PATCH = 1, 2, 5, 6, 9, 10, 11
@@ -98,6 +101,7 @@ def sphk():
         L.sphk_launch_count.restype = C.c_longlong
         L.sphk_scene_boundary_count.restype = C.c_longlong
         L.sphk_strays_block_floats.restype = C.c_longlong
+        L.sphk_implicit_viscosity_work_floats.restype = C.c_longlong
         L.sphk_destroy.restype = None
         L.sphk_mg_destroy.restype = None
         _sphk = L
@@ -244,6 +248,18 @@ class SphApp:
         """Vorticity confinement of strength eps in every following step (0: off).  Not on the reference engine."""
         if self.L.sph_app_set_vorticity(self.h, C.c_float(eps)):
             raise RuntimeError("sph_app_set_vorticity failed (reference engine, or eps < 0)")
+
+    def set_implicit_viscosity(self, nu: float, nu_boundary: float = 0.0, tol: float = 1e-4, max_iter: int = 20):
+        """Implicit viscosity in every following step (nu = 0: off).  Not on the reference engine."""
+        if self.L.sph_app_set_implicit_viscosity(self.h, C.c_float(nu), C.c_float(nu_boundary), C.c_float(tol), C.c_int(max_iter)):
+            raise RuntimeError("sph_app_set_implicit_viscosity failed (reference engine or invalid values)")
+
+    def viscosity_stats(self):
+        """(iterations, relative residual) of the last implicit viscosity solve."""
+        it, res = C.c_int(0), C.c_float(0.0)
+        if self.L.sph_app_viscosity_stats(self.h, C.byref(it), C.byref(res)):
+            raise RuntimeError("sph_app_viscosity_stats failed (reference engine)")
+        return int(it.value), float(res.value)
 
     def set_body_motion(self, body: int, linear_velocity, angular_velocity):
         """New motion of one kinematic body from the next step on.  Not on the reference engine."""

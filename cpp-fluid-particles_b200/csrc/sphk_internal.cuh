@@ -128,6 +128,7 @@ struct sphk_ctx {
     const int* lastCsB = nullptr;
     long long launches = 0;
     BodyState* bodies = nullptr;     // non-null after sphk_bodies_init
+    float* viscStats = nullptr;      // [2] device: {iterations (int bits), |r|_M / |b|_M} of the last sphk_implicit_viscosity
 };
 
 struct DevScene {

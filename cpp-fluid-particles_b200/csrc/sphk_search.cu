@@ -210,6 +210,7 @@ extern "C" int sphk_create(sphk_ctx** out, int max_fluid, int max_boundary, cons
     if (e == cudaSuccess) e = dalloc(&c->tmpF, 3 * static_cast<size_t>(max_fluid));
     if (e == cudaSuccess) e = dalloc(&c->partial, 1024);
     if (e == cudaSuccess) e = dalloc(&c->loops, 2);
+    if (e == cudaSuccess) e = dalloc(&c->viscStats, 2);
     if (e == cudaSuccess) e = dalloc(&c->cnt, static_cast<size_t>(max_fluid));
     if (e == cudaSuccess) e = dalloc(&c->tileWin, (static_cast<size_t>(max_fluid) / SPHK_BLOCK + 1) * SPHK_TILE_WINS);
     if (e == cudaSuccess) {
@@ -241,7 +242,7 @@ extern "C" void sphk_destroy(sphk_ctx* c) {
     if (!c) return;
     cudaFree(c->keys); cudaFree(c->keysSorted); cudaFree(c->idx); cudaFree(c->idxSorted);
     cudaFree(c->snapA); cudaFree(c->snapB); cudaFree(c->rec.a); cudaFree(c->rec.b); cudaFree(c->massRange); cudaFree(c->dispMax); cudaFree(c->cellFlag);
-    cudaFree(c->tmpF); cudaFree(c->partial); cudaFree(c->loops); cudaFree(c->cnt); cudaFree(c->nbr); cudaFree(c->cubTemp); cudaFree(c->tileWin);
+    cudaFree(c->tmpF); cudaFree(c->partial); cudaFree(c->loops); cudaFree(c->viscStats); cudaFree(c->cnt); cudaFree(c->nbr); cudaFree(c->cubTemp); cudaFree(c->tileWin);
     if (c->pinned) cudaFreeHost(c->pinned);
     sphk_bodies_release(c->bodies);
     delete c;

@@ -372,6 +372,69 @@ struct OpVorticityConfinement {
     }
 };
 
+// ---- implicit viscosity (no reference counterpart; Weiler, Koschier, Brand & Bender 2018; DESIGN.md section 2.5) -------------
+// Pair coefficient c_ij = -10 nu V_j g(r) / (r^2 + 0.01 R^2), g = grad_w_factor <= 0 (so c_ij >= 0), V_j = m_j / rho0; a boundary
+// pair takes nu_b and m_b / rho_B.  `nuV` = nu V_j.  m_i c_ij = m_j c_ji: the system is self-adjoint in the mass inner product.
+__device__ __forceinline__ float visc_coef(float nuV, float r2, const KConst& k) {
+    return -10.0f * nuV * grad_w_factor(sqrtf(r2), k) / (r2 + 0.01f * k.R * k.R);
+}
+// symmetric 3x3 matrices as 6 floats {xx, yy, zz, xy, xz, yz}
+__device__ __forceinline__ float3 sym_apply(const float* __restrict__ S, int i, float3 p) {
+    const float* a = S + 6 * static_cast<size_t>(i);
+    return f3(a[0] * p.x + a[3] * p.y + a[4] * p.z, a[3] * p.x + a[1] * p.y + a[5] * p.z, a[4] * p.x + a[5] * p.y + a[2] * p.z);
+}
+
+// D_i = I + dt sum_j c_ij d d^T (fluid and boundary neighbours), b_i = v*_i + dt sum_b c_ib d (d . v_b) (v_b = the boundary
+// record's velocity: 0, or a kinematic body's v_k); Dinv (when non-null) = D_i^-1 by cofactors (D_i is symmetric, eigenvalues >= 1)
+struct OpViscImplicitSetup {
+    float* D; float* Dinv; float* b; float nuRho, nuBRho, dt;     // nu / rho0, nu_b / rho_B
+    static constexpr bool kFluidOnly = false, kHi = true;
+    struct Acc {
+        float s[6]; float3 bb; float3 vi;
+        template <class F> __device__ void sums(F f) { for (int k = 0; k < 6; ++k) f(s[k]); f(bb.x); f(bb.y); f(bb.z); }
+    };
+    __device__ void begin(Acc& a, int, float4, float4 hi, const DevScene&) const {
+        for (int k = 0; k < 6; ++k) a.s[k] = 0.f;
+        a.bb = f3(0, 0, 0); a.vi = xyz(hi);
+    }
+    __device__ void pair(Acc& a, int, int, bool isB, float3 d, float r2, float mj, float4, float4 hi, const DevScene& s) const {
+        const float c = visc_coef(mj * (isB ? nuBRho : nuRho), r2, s.k);
+        const float3 cd = c * d;
+        a.s[0] += cd.x * d.x; a.s[1] += cd.y * d.y; a.s[2] += cd.z * d.z;
+        a.s[3] += cd.x * d.y; a.s[4] += cd.x * d.z; a.s[5] += cd.y * d.z;
+        if (isB) a.bb += dot3(d, xyz(hi)) * cd;
+    }
+    __device__ void end(Acc& a, int i, float4, float4, const DevScene&) const {
+        float m[6];
+        for (int k = 0; k < 6; ++k) m[k] = dt * a.s[k];
+        m[0] += 1.0f; m[1] += 1.0f; m[2] += 1.0f;
+        float* out = D + 6 * static_cast<size_t>(i);
+        for (int k = 0; k < 6; ++k) out[k] = m[k];
+        store3(b, i, a.vi + dt * a.bb);
+        if (!Dinv) return;
+        const float c00 = m[1] * m[2] - m[5] * m[5], c11 = m[0] * m[2] - m[4] * m[4], c22 = m[0] * m[1] - m[3] * m[3];
+        const float c01 = m[4] * m[5] - m[3] * m[2], c02 = m[3] * m[5] - m[1] * m[4], c12 = m[3] * m[4] - m[0] * m[5];
+        const float inv = 1.0f / (m[0] * c00 + m[3] * c01 + m[4] * c02);
+        float* o = Dinv + 6 * static_cast<size_t>(i);
+        o[0] = c00 * inv; o[1] = c11 * inv; o[2] = c22 * inv; o[3] = c01 * inv; o[4] = c02 * inv; o[5] = c12 * inv;
+    }
+};
+
+// (A p)_i = D_i p_i - dt sum_j c_ij d (d . p_j), fluid neighbours only; p = the velocity slots of the fluid records (B.xyz; the
+// solve keeps its CG direction there, so every path -- tile staging of B included -- gathers p with the record and B.w stays m)
+struct OpViscImplicitMatvec {
+    const float* D; float* Ap; float nuRho, dt;
+    static constexpr bool kFluidOnly = true, kHi = true;
+    struct Acc { float3 a; template <class F> __device__ void sums(F f) { f(a.x); f(a.y); f(a.z); } };
+    __device__ void begin(Acc& a, int, float4, float4, const DevScene&) const { a.a = f3(0, 0, 0); }
+    __device__ void pair(Acc& a, int, int, bool, float3 d, float r2, float mj, float4, float4 hi, const DevScene& s) const {
+        a.a += (visc_coef(mj * nuRho, r2, s.k) * dot3(d, xyz(hi))) * d;
+    }
+    __device__ void end(Acc& a, int i, float4, float4 hi, const DevScene&) const {
+        store3(Ap, i, sym_apply(D, i, xyz(hi)) - dt * a.a);
+    }
+};
+
 // =================================================================================================
 // Sweep drivers
 // =================================================================================================
@@ -1620,6 +1683,248 @@ extern "C" int sphk_fused_pbd_xsph_vorticity(sphk_ctx* c, const sphk_scene* s, f
     const int b = (c->actCount < 0 || c->rangeDev) ? 0 : c->actBegin, e = (c->actCount < 0 || c->rangeDev) ? c->nF : c->actBegin + c->actCount;
     if (e > b) k_commit_vel<<<sphk_blocks(e - b), SPHK_BLOCK, 0, c->stream>>>(tmp, c->rec, s->fluid.vel, b, e, c->rangeDev);
     c->launches++;
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+// ---- implicit viscosity: preconditioned CG in the mass inner product, loop control on the device ------------------------------
+// Workspace (caller-owned floats): ViscCg | 3 x SPHK_VISC_PARTS double partials | D[6n] | Dinv[6n] | r[3n] | z[3n] | Ap[3n].
+// The iterate x lives in the API velocity array, the direction p in the velocity slots of the fluid records.  Every kernel of
+// the loop returns at once when the loop has ended, so max_iter iterations are enqueued as a fixed launch sequence (a captured
+// step graph replays it).  Dot products are m_i-weighted, accumulated in double, in a fixed shape (bit-reproducible).
+struct ViscCg {
+    int active, iters, maxIter, pad;
+    double tol2, bb, rz, rr, alpha, beta;
+};
+#define SPHK_VISC_HEAD 64                    // floats reserved for ViscCg
+#define SPHK_VISC_PARTS 1024                 // blocks of the element-wise reductions, at most
+#define SPHK_VISC_RED 256                    // threads of the element-wise kernels
+static_assert(sizeof(ViscCg) <= SPHK_VISC_HEAD * sizeof(float), "ViscCg exceeds its head");
+
+// fixed-shape sum of K doubles over a block of SPHK_VISC_RED threads; thread 0 receives the totals
+template <int K> __device__ __forceinline__ void visc_block_sum(double (&v)[K]) {
+    __shared__ double sm[K][SPHK_VISC_RED / 32];
+    for (int k = 0; k < K; ++k) {
+        double t = v[k];
+        for (int o = 16; o > 0; o >>= 1) t += __shfl_xor_sync(0xffffffffu, t, o);
+        if ((threadIdx.x & 31) == 0) sm[k][threadIdx.x >> 5] = t;
+    }
+    __syncthreads();
+    if (threadIdx.x == 0)
+        for (int k = 0; k < K; ++k) {
+            double t = 0.0;
+            for (int w = 0; w < SPHK_VISC_RED / 32; ++w) t += sm[k][w];
+            v[k] = t;
+        }
+}
+template <int K> __device__ __forceinline__ void visc_store_partials(double (&v)[K], double* __restrict__ part) {
+    visc_block_sum(v);
+    if (threadIdx.x == 0)
+        for (int k = 0; k < K; ++k) part[k * SPHK_VISC_PARTS + blockIdx.x] = v[k];
+}
+// one block: the K totals of m partials
+template <int K> __device__ __forceinline__ void visc_sum_partials(const double* __restrict__ part, int m, double (&v)[K]) {
+    for (int k = 0; k < K; ++k) {
+        v[k] = 0.0;
+        for (int b = threadIdx.x; b < m; b += SPHK_VISC_RED) v[k] += part[k * SPHK_VISC_PARTS + b];
+    }
+    visc_block_sum(v);
+}
+__device__ __forceinline__ double mdot(float m, float3 a, float3 b) {
+    return static_cast<double>(m) * (static_cast<double>(a.x) * b.x + static_cast<double>(a.y) * b.y + static_cast<double>(a.z) * b.z);
+}
+
+// r = b - A x0 (b arrives in r, A x0 in Ap; x0 = v* = the records' velocity, copied to the API array), z = Dinv r, p = z;
+// partials {<b,b>, <r,z>, <r,r>}
+__global__ void __launch_bounds__(SPHK_VISC_RED)
+k_visc_init(Rec rec, float* __restrict__ vel, float* __restrict__ r, const float* __restrict__ Ap, const float* __restrict__ Dinv,
+            float* __restrict__ z, int n, double* __restrict__ part) {
+    double acc[3] = {0.0, 0.0, 0.0};
+    for (int i = blockIdx.x * SPHK_VISC_RED + threadIdx.x; i < n; i += gridDim.x * SPHK_VISC_RED) {
+        const float4 hi = rec_hi(rec + i);
+        store3(vel, i, xyz(hi));
+        const float3 b = load3(r, i), ri = b - load3(Ap, i), zi = sym_apply(Dinv, i, ri);
+        store3(r, i, ri); store3(z, i, zi);
+        rec_set_vel(rec + i, zi);
+        acc[0] += mdot(hi.w, b, b); acc[1] += mdot(hi.w, ri, zi); acc[2] += mdot(hi.w, ri, ri);
+    }
+    visc_store_partials(acc, part);
+}
+// the loop test before the first iteration: converged (|r|_M <= tol |b|_M, a fluid at rest included) or <r,z>_M = 0
+__global__ void __launch_bounds__(SPHK_VISC_RED) k_visc_init_finish(ViscCg* st, const double* __restrict__ part, int m, double tol2,
+                                                                     int maxIter) {
+    double v[3];
+    visc_sum_partials(part, m, v);
+    if (threadIdx.x != 0) return;
+    st->tol2 = tol2; st->maxIter = maxIter; st->iters = 0;
+    st->bb = v[0]; st->rz = v[1]; st->rr = v[2]; st->alpha = 0.0; st->beta = 0.0;
+    st->active = (v[2] <= tol2 * v[0] || v[1] == 0.0) ? 0 : 1;
+}
+// partials of <p, Ap>
+__global__ void __launch_bounds__(SPHK_VISC_RED)
+k_visc_alpha_partial(const ViscCg* st, Rec rec, const float* __restrict__ Ap, int n, double* __restrict__ part) {
+    if (!st->active) return;
+    double acc[1] = {0.0};
+    for (int i = blockIdx.x * SPHK_VISC_RED + threadIdx.x; i < n; i += gridDim.x * SPHK_VISC_RED) {
+        const float4 hi = rec_hi(rec + i);
+        acc[0] += mdot(hi.w, xyz(hi), load3(Ap, i));
+    }
+    visc_store_partials(acc, part);
+}
+// alpha = <r,z> / <p,Ap> (a non-positive <p,Ap> -- breakdown -- ends the loop)
+__global__ void __launch_bounds__(SPHK_VISC_RED) k_visc_alpha_finish(ViscCg* st, const double* __restrict__ part, int m) {
+    if (!st->active) return;
+    double v[1];
+    visc_sum_partials(part, m, v);
+    if (threadIdx.x != 0) return;
+    if (!(v[0] > 0.0)) { st->active = 0; return; }
+    st->alpha = st->rz / v[0];
+}
+// x += alpha p, r -= alpha Ap, z = Dinv r; partials {<r,z>, <r,r>}
+__global__ void __launch_bounds__(SPHK_VISC_RED)
+k_visc_update(const ViscCg* st, Rec rec, float* __restrict__ vel, float* __restrict__ r, const float* __restrict__ Ap,
+              const float* __restrict__ Dinv, float* __restrict__ z, int n, double* __restrict__ part) {
+    if (!st->active) return;
+    const float a = static_cast<float>(st->alpha);
+    double acc[2] = {0.0, 0.0};
+    for (int i = blockIdx.x * SPHK_VISC_RED + threadIdx.x; i < n; i += gridDim.x * SPHK_VISC_RED) {
+        const float4 hi = rec_hi(rec + i);
+        store3(vel, i, load3(vel, i) + a * xyz(hi));
+        const float3 ri = load3(r, i) - a * load3(Ap, i), zi = sym_apply(Dinv, i, ri);
+        store3(r, i, ri); store3(z, i, zi);
+        acc[0] += mdot(hi.w, ri, zi); acc[1] += mdot(hi.w, ri, ri);
+    }
+    visc_store_partials(acc, part);
+}
+// ++iters; the loop ends when |r|_M <= tol |b|_M, <r,z>_M = 0 or iters = max_iter; else beta = <r,z>_new / <r,z>
+__global__ void __launch_bounds__(SPHK_VISC_RED) k_visc_beta_finish(ViscCg* st, const double* __restrict__ part, int m) {
+    if (!st->active) return;
+    double v[2];
+    visc_sum_partials(part, m, v);
+    if (threadIdx.x != 0) return;
+    const int it = st->iters + 1;
+    st->iters = it;
+    st->rr = v[1];
+    if (v[1] <= st->tol2 * st->bb || v[0] == 0.0 || it >= st->maxIter) { st->active = 0; return; }
+    st->beta = v[0] / st->rz;
+    st->rz = v[0];
+}
+// p = z + beta p
+__global__ void __launch_bounds__(SPHK_VISC_RED) k_visc_direction(const ViscCg* st, Rec rec, const float* __restrict__ z, int n) {
+    if (!st->active) return;
+    const float beta = static_cast<float>(st->beta);
+    for (int i = blockIdx.x * SPHK_VISC_RED + threadIdx.x; i < n; i += gridDim.x * SPHK_VISC_RED)
+        rec_set_vel(rec + i, load3(z, i) + beta * xyz(rec_hi(rec + i)));
+}
+// the solve's outcome into the context's own memory (the workspace is the caller's and may be gone when the stats are read)
+__global__ void k_visc_report(const ViscCg* st, float* out) {
+    out[0] = __int_as_float(st->iters);
+    out[1] = st->bb > 0.0 ? static_cast<float>(sqrt(st->rr / st->bb)) : 0.0f;
+}
+// the records' velocity slots <- a float3 array (a test's direction p; the solution at the end of the solve)
+__global__ void __launch_bounds__(SPHK_BLOCK) k_visc_set_rec_vel(Rec rec, const float* __restrict__ v, int n) {
+    const int i = blockIdx.x * SPHK_BLOCK + threadIdx.x;
+    if (i < n) rec_set_vel(rec + i, load3(v, i));
+}
+
+static int visc_blocks(int n) {
+    const int b = (n + SPHK_VISC_RED * 8 - 1) / (SPHK_VISC_RED * 8);
+    return b < 1 ? 1 : (b > SPHK_VISC_PARTS ? SPHK_VISC_PARTS : b);
+}
+static bool finite_nonneg(float x) { return x >= 0.f && x - x == 0.f; }
+static int check_visc(const sphk_ctx* c, float nu, float dt, float rho0) {
+    if (!finite_nonneg(nu) || !finite_nonneg(dt) || !(rho0 > 0.f)) return SPHK_ERR_INVALID;
+    if (c->actCount >= 0 || c->rangeDev) return SPHK_ERR_STATE;      // slab ranks: the solve needs global dot products
+    return SPHK_OK;
+}
+static bool aliases(const void* a, const sphk_scene* s) {
+    return a == s->fluid.pos || a == s->fluid.vel || a == s->fluid.mass || a == s->fluid.density || a == s->fluid.pressure;
+}
+
+extern "C" long long sphk_implicit_viscosity_work_floats(int n) {
+    if (n < 0) return -1;
+    return SPHK_VISC_HEAD + 2LL * 3 * SPHK_VISC_PARTS + 21LL * n;
+}
+
+extern "C" int sphk_implicit_viscosity(sphk_ctx* c, const sphk_scene* s, float* work, float nu, float nu_boundary, float dt, float rho0,
+                                       float rho_boundary, float tol, int max_iter) {
+    SPHK_CHECK_SCENE(c, s);
+    if (!work || aliases(work, s) || !finite_nonneg(nu_boundary) || !(rho_boundary > 0.f) || !(tol > 0.f) || max_iter < 1 ||
+        max_iter > SPHK_IMPLICIT_VISCOSITY_MAX_ITER)
+        return SPHK_ERR_INVALID;
+    const int rc0 = check_visc(c, nu, dt, rho0);
+    if (rc0 != SPHK_OK) return rc0;
+    // the viscous force on a dynamic body is not part of its reaction (sphk_bodies_react): the momentum would not balance
+    if (nu_boundary > 0.f && c->bodies && c->bodies->acc) return SPHK_ERR_STATE;
+    const int n = c->nF;
+    ViscCg* st = reinterpret_cast<ViscCg*>(work);
+    double* part = reinterpret_cast<double*>(work + SPHK_VISC_HEAD);
+    float* D = work + SPHK_VISC_HEAD + 2 * 3 * SPHK_VISC_PARTS;
+    float *Dinv = D + 6LL * n, *r = Dinv + 6LL * n, *z = r + 3LL * n, *Ap = z + 3LL * n;
+    const float nuRho = nu / rho0, nuBRho = nu_boundary / rho_boundary;
+    float* vel = s->fluid.vel;
+    int rc = run_sweep(c, s, OpViscImplicitSetup{D, Dinv, r, nuRho, nuBRho, dt});          // b -> r
+    if (rc != SPHK_OK) return rc;
+    const OpViscImplicitMatvec mv{D, Ap, nuRho, dt};
+    rc = run_sweep(c, s, mv);                                                                // A v*
+    if (rc != SPHK_OK) return rc;
+    const int m = visc_blocks(n);
+    k_visc_init<<<m, SPHK_VISC_RED, 0, c->stream>>>(c->rec, vel, r, Ap, Dinv, z, n, part);
+    k_visc_init_finish<<<1, SPHK_VISC_RED, 0, c->stream>>>(st, part, m, static_cast<double>(tol) * tol, max_iter);
+    c->launches += 2;
+    const int* outer = c->pred;
+    c->pred = &st->active;
+    for (int k = 0; k < max_iter && rc == SPHK_OK; ++k) {
+        rc = run_sweep(c, s, mv);
+        k_visc_alpha_partial<<<m, SPHK_VISC_RED, 0, c->stream>>>(st, c->rec, Ap, n, part);
+        k_visc_alpha_finish<<<1, SPHK_VISC_RED, 0, c->stream>>>(st, part, m);
+        k_visc_update<<<m, SPHK_VISC_RED, 0, c->stream>>>(st, c->rec, vel, r, Ap, Dinv, z, n, part);
+        k_visc_beta_finish<<<1, SPHK_VISC_RED, 0, c->stream>>>(st, part, m);
+        k_visc_direction<<<m, SPHK_VISC_RED, 0, c->stream>>>(st, c->rec, z, n);
+        c->launches += 5;
+    }
+    c->pred = outer;
+    if (n > 0) { k_visc_set_rec_vel<<<sphk_blocks(n), SPHK_BLOCK, 0, c->stream>>>(c->rec, vel, n); c->launches++; }   // records <- x
+    k_visc_report<<<1, 1, 0, c->stream>>>(st, c->viscStats);
+    c->launches++;
+    if (rc != SPHK_OK) return rc;
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+extern "C" int sphk_implicit_viscosity_stats(sphk_ctx* c, int* iterations, float* rel_residual) {
+    if (!c || !iterations) return SPHK_ERR_INVALID;
+    float h[2];
+    SPHK_CUDA_TRY(cudaMemcpyAsync(h, c->viscStats, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
+    SPHK_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    memcpy(iterations, &h[0], sizeof(int));
+    if (rel_residual) *rel_residual = h[1];
+    return SPHK_OK;
+}
+
+extern "C" int sphk_visc_implicit_setup(sphk_ctx* c, const sphk_scene* s, float* d_out, float* b_out, float nu, float nu_boundary,
+                                        float dt, float rho0, float rho_boundary) {
+    SPHK_CHECK_SCENE(c, s);
+    if (!d_out || !b_out || d_out == b_out || aliases(d_out, s) || aliases(b_out, s) || !finite_nonneg(nu_boundary) ||
+        !(rho_boundary > 0.f))
+        return SPHK_ERR_INVALID;
+    const int rc = check_visc(c, nu, dt, rho0);
+    if (rc != SPHK_OK) return rc;
+    return run_sweep(c, s, OpViscImplicitSetup{d_out, nullptr, b_out, nu / rho0, nu_boundary / rho_boundary, dt});
+}
+
+extern "C" int sphk_visc_implicit_matvec(sphk_ctx* c, const sphk_scene* s, const float* d_in, const float* p_in, float* ap_out,
+                                         float nu, float dt, float rho0) {
+    SPHK_CHECK_SCENE(c, s);
+    if (!d_in || !p_in || !ap_out || d_in == p_in || ap_out == d_in || ap_out == p_in || aliases(ap_out, s)) return SPHK_ERR_INVALID;
+    const int rc0 = check_visc(c, nu, dt, rho0);
+    if (rc0 != SPHK_OK) return rc0;
+    const int n = c->nF;
+    if (n > 0) k_visc_set_rec_vel<<<sphk_blocks(n), SPHK_BLOCK, 0, c->stream>>>(c->rec, p_in, n);
+    const int rc = run_sweep(c, s, OpViscImplicitMatvec{d_in, ap_out, nu / rho0, dt});
+    if (n > 0) k_visc_set_rec_vel<<<sphk_blocks(n), SPHK_BLOCK, 0, c->stream>>>(c->rec, s->fluid.vel, n);   // records <- API velocities
+    if (n > 0) c->launches += 2;
+    if (rc != SPHK_OK) return rc;
     SPHK_CUDA_TRY(cudaGetLastError());
     return SPHK_OK;
 }

@@ -79,6 +79,10 @@ class SphkOps:
 
     list_capacity = 96               # SPHK_OPT_LIST_CAPACITY of ctx (set_option keeps it current)
     vorticity_eps = 0.0              # vorticity confinement strength (BasicSPHSolver::setVorticityConfinement); 0: off
+    implicit_nu = 0.0                # implicit viscosity (BasicSPHSolver::setImplicitViscosity); 0: off
+    implicit_nu_boundary = 0.0
+    implicit_tol = 1e-4
+    implicit_max_iter = 20
 
     # ---- multi-GPU hooks ---------------------------------------------------------------------------------
     def sync_vel(self):
@@ -334,6 +338,40 @@ class SphkOps:
                                                    _ptr(self.buffer3) if with_color_grad else None, C.c_float(self.p.rho_boundary),
                                                    *self._vort_buffers()), "sphk_fused_pbd_xsph_vorticity")
 
+    # ---- implicit viscosity (no reference counterpart; DESIGN.md section 2.5) --------------------------------------------
+    def _visc_work(self):
+        if getattr(self, "visc_work", None) is None:   # allocated on first use, like the class layer's
+            n = self.buffer3.shape[0]
+            self.visc_work = torch.zeros(int(self.L.sphk_implicit_viscosity_work_floats(C.c_int(n))), dtype=torch.float32,
+                                         device=self.device)
+        return _ptr(self.visc_work)
+
+    def implicit_viscosity(self, nu=None, nu_boundary=None, tol=None, max_iter=None):
+        """The implicit viscosity solve with the attributes' settings (or the arguments)."""
+        a = lambda x, d: d if x is None else x  # noqa: E731
+        check(self.L.sphk_implicit_viscosity(self.ctx, self._s(), self._visc_work(), C.c_float(a(nu, self.implicit_nu)),
+                                             C.c_float(a(nu_boundary, self.implicit_nu_boundary)), C.c_float(self.p.dt),
+                                             C.c_float(self.p.rho0), C.c_float(self.p.rho_boundary),
+                                             C.c_float(a(tol, self.implicit_tol)), C.c_int(int(a(max_iter, self.implicit_max_iter)))),
+              "sphk_implicit_viscosity")
+
+    def implicit_viscosity_stats(self):
+        """(iterations, |r|_M / |b|_M) of the last solve; synchronises."""
+        it, res = C.c_int(0), C.c_float(0.0)
+        check(self.L.sphk_implicit_viscosity_stats(self.ctx, C.byref(it), C.byref(res)), "sphk_implicit_viscosity_stats")
+        return int(it.value), float(res.value)
+
+    def visc_implicit_setup(self, d_out, b_out, nu, nu_boundary):
+        """D_i (n, 6) and b_i (n, 3) of the solve into the given tensors (one sweep)."""
+        check(self.L.sphk_visc_implicit_setup(self.ctx, self._s(), _ptr(d_out), _ptr(b_out), C.c_float(nu), C.c_float(nu_boundary),
+                                              C.c_float(self.p.dt), C.c_float(self.p.rho0), C.c_float(self.p.rho_boundary)),
+              "sphk_visc_implicit_setup")
+
+    def visc_implicit_matvec(self, d_in, p_in, ap_out, nu):
+        """(A p)_i (n, 3) from D (n, 6) and p (n, 3) (one sweep)."""
+        check(self.L.sphk_visc_implicit_matvec(self.ctx, self._s(), _ptr(d_in), _ptr(p_in), _ptr(ap_out), C.c_float(nu),
+                                               C.c_float(self.p.dt), C.c_float(self.p.rho0)), "sphk_visc_implicit_matvec")
+
     def pressure(self):
         check(self.L.sphk_pressure(self.ctx, self._s(), C.c_float(self.p.rho0), C.c_float(self.p.stiff)), "sphk_pressure")
 
@@ -427,6 +465,8 @@ class SphkOps:
                 self.sync_scalar(self.omega_norm)
             else:
                 self._run(self.fused_viscosity_surface, "vel", split=False)
+            if self.implicit_nu > 0:
+                self._run(self.implicit_viscosity, "vel")
             if vort:
                 self._run(self.vorticity_confinement, "vel")
         else:
@@ -436,6 +476,8 @@ class SphkOps:
             if self._surface_enabled():  # handleSurface, :262-275
                 self._run(self.color_grad, "array", self.buffer3)
                 self._run(self.surface, "vel")
+            if self.implicit_nu > 0:
+                self._run(self.implicit_viscosity, "vel")
             if vort:
                 self._run(self.vorticity_confinement, "vel")
             self.density()
@@ -483,6 +525,8 @@ class SphkOps:
             if self._surface_enabled():
                 self._run(self.color_grad, "array", self.buffer3)
                 self._run(self.surface, "vel")
+        if self.implicit_nu > 0:     # after surface, before the density solve
+            self._run(self.implicit_viscosity, "vel")
         if vort:                     # after surface, before the density solve
             self._run(self.vorticity_confinement, "vel")
         total, it = 3.4e38, 0        # project :160-210
@@ -536,6 +580,8 @@ class SphkOps:
             if self._surface_enabled():
                 self._run(self.color_grad, "array", self.buffer3)
                 self._run(self.surface, "vel")
+        if self.implicit_nu > 0:     # after XSPH and surface, before gravity
+            self._run(self.implicit_viscosity, "vel")
         if vort:                     # after XSPH and surface, before gravity
             self._run(self.vorticity_confinement, "vel")
         self.gravity()

@@ -408,6 +408,34 @@ extern "C" int sph_app_set_vorticity(sph_app* app, float eps) {
 #endif
 }
 
+extern "C" int sph_app_set_implicit_viscosity(sph_app* app, float nu, float nu_boundary, float tol, int max_iter) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)nu; (void)nu_boundary; (void)tol; (void)max_iter;
+    return 1;
+#else
+    auto* b = dynamic_cast<BasicSPHSolver*>(app->solver);
+    if (!b || !(nu >= 0.0f) || !(nu_boundary >= 0.0f) || !std::isfinite(nu) || !std::isfinite(nu_boundary) || !(tol > 0.0f) ||
+        max_iter < 1 || max_iter > SPHK_IMPLICIT_VISCOSITY_MAX_ITER)
+        return 1;
+    if (nu_boundary > 0.0f && app->system->bodiesDynamic()) return 1;   // the viscous wall force is not part of the bodies' reaction
+    b->setImplicitViscosity(nu, nu_boundary, tol, max_iter);
+    return 0;
+#endif
+}
+
+extern "C" int sph_app_viscosity_stats(sph_app* app, int* iterations, float* rel_residual) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)iterations; (void)rel_residual;
+    return 1;
+#else
+    auto* b = dynamic_cast<BasicSPHSolver*>(app->solver);
+    if (!b) return 1;
+    if (iterations) *iterations = b->lastViscosityIterations();
+    if (rel_residual) *rel_residual = b->lastViscosityResidual();
+    return 0;
+#endif
+}
+
 extern "C" const char* sph_app_engine(void) {
 #ifdef SPH_APP_REFERENCE_ENGINE
     return "reference-cuda";

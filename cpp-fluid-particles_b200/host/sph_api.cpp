@@ -4,6 +4,7 @@
 #include "sph_api.hpp"
 
 #include <algorithm>
+#include <cmath>
 #include <cstdlib>
 #include <limits>
 #include <numeric>
@@ -92,6 +93,7 @@ void BasicSPHSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shar
         if (surface) produced(0, colorGradBuffer(), 3);
         diffuseAndSurface(rho0, rhoB, visc, dt, surfaceTensionIntensity, airPressure, surface, true);
         producedVel(fluids);
+        if (implicitViscosityOn()) implicitViscosity(fluids, rho0, rhoB, dt);
         if (vorticityOn()) confine(fluids, rho0, dt);
         check(sphk_pressure(current_.ctx, &current_.abi, rho0, stiff), "sphk_pressure");
         produced(0, fluids->getDensityPtr(), 1); produced(0, fluids->getPressurePtr(), 1);
@@ -104,6 +106,7 @@ void BasicSPHSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shar
         if (surface)
             handleSurface(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, rhoB, cellSize, cellLength, radius,
                           dt, surfaceTensionIntensity, airPressure);
+        if (implicitViscosityOn()) implicitViscosity(fluids, rho0, rhoB, dt);
         if (vorticityOn()) confine(fluids, rho0, dt);
         project(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, stiff, cellSize, cellLength, radius, dt);
     }
@@ -168,6 +171,40 @@ void BasicSPHSolver::confine(const std::shared_ptr<SPHParticles>& fluids, float 
           "sphk_vorticity_confinement");
     producedVel(fluids);
 }
+
+// addition (no reference counterpart): implicit viscosity, sphk.h
+void BasicSPHSolver::setImplicitViscosity(float nu, float nuBoundary, float tol, int maxIter) {
+    if (!(nu >= 0.0f) || !(nuBoundary >= 0.0f) || !(tol > 0.0f) || maxIter < 1 || maxIter > SPHK_IMPLICIT_VISCOSITY_MAX_ITER ||
+        !std::isfinite(nu) || !std::isfinite(nuBoundary)) {
+        printf("setImplicitViscosity: need nu >= 0, nuBoundary >= 0 (finite), tol > 0 and 1 <= maxIter <= %d (got %g, %g, %g, %d); "
+               "the setting is kept at %g, %g, %g, %d\n", SPHK_IMPLICIT_VISCOSITY_MAX_ITER, nu, nuBoundary, tol, maxIter, implNu_,
+               implNuB_, implTol_, implMaxIter_);
+        return;
+    }
+    if (nuBoundary > 0.0f && reacting_) {      // (known once the solver has stepped in its system: SPHSystem's constructor does)
+        printf("setImplicitViscosity: nuBoundary > 0 is not supported with dynamic bodies (the viscous wall force is not part of "
+               "their reaction); the setting is kept at %g, %g, %g, %d\n", implNu_, implNuB_, implTol_, implMaxIter_);
+        return;
+    }
+    if (nu > 0.0f && !viscWork_)
+        viscWork_ = std::make_unique<DArray<float>>(static_cast<unsigned int>(sphk_implicit_viscosity_work_floats(num_)));
+    if (nu != implNu_ || nuBoundary != implNuB_ || tol != implTol_ || maxIter != implMaxIter_) ++configEpoch_;
+    implNu_ = nu; implNuB_ = nuBoundary; implTol_ = tol; implMaxIter_ = maxIter;
+}
+
+void BasicSPHSolver::implicitViscosity(const std::shared_ptr<SPHParticles>& fluids, float rho0, float rhoB, float dt) {
+    check(sphk_implicit_viscosity(current_.ctx, &current_.abi, viscWork_->addr(), implNu_, implNuB_, dt, rho0, rhoB, implTol_,
+                                  implMaxIter_),
+          "sphk_implicit_viscosity");
+    producedVel(fluids);
+}
+
+void BasicSPHSolver::viscStats(int& iters, float& residual) const {
+    iters = 0; residual = 0.0f;
+    if (current_.ctx) check(sphk_implicit_viscosity_stats(current_.ctx, &iters, &residual), "sphk_implicit_viscosity_stats");
+}
+int BasicSPHSolver::lastViscosityIterations() const { int it; float r; viscStats(it, r); return it; }
+float BasicSPHSolver::lastViscosityResidual() const { int it; float r; viscStats(it, r); return r; }
 
 // :227-235
 void BasicSPHSolver::force(std::shared_ptr<SPHParticles>&, float dt, float3 G) {
@@ -248,6 +285,7 @@ void DFSPHSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shared_
             handleSurface(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, rhoB, cellSize, cellLength, radius,
                           dt, surfaceTensionIntensity, airPressure);
     }
+    if (implicitViscosityOn()) implicitViscosity(fluids, rho0, rhoB, dt);   // after surface, before the density solve
     if (vorticityOn()) confine(fluids, rho0, dt);      // after surface, before the density solve
     itDen_ = project(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, cellSize, cellLength, radius, dt,
                      densityErrorThreshold, maxIter);
@@ -412,6 +450,7 @@ void PBDSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shared_pt
             handleSurface(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, rhoB, cellSize, cellLength, radius,
                           dt, surfaceTensionIntensity, airPressure);
     }
+    if (implicitViscosityOn()) implicitViscosity(fluids, rho0, rhoB, dt);   // after XSPH and surface, before gravity
     if (vorticityOn()) confine(fluids, rho0, dt);      // after XSPH and surface, before gravity
     force(fluids, dt, G);
     predict(fluids, dt, spaceSize);

@@ -193,6 +193,18 @@ public:
     // the first enable.
     void setVorticityConfinement(float eps);
     float vorticityConfinement() const { return vortEps_; }
+    // addition: implicit viscosity (sphk_implicit_viscosity; DESIGN.md section 2.5) in every step, on top of the reference's
+    // explicit `visc` term: kinematic viscosity nu of the fluid and nuBoundary against walls and bodies (0: free slip), solved
+    // to |b - A v|_M <= tol |b|_M or maxIter CG iterations.  nu = 0 (default) = off, the reference's step.  nu or nuBoundary
+    // < 0 or NaN, tol <= 0 or NaN, maxIter outside [1, SPHK_IMPLICIT_VISCOSITY_MAX_ITER], and nuBoundary > 0 in a system with
+    // dynamic bodies are refused (printed, setting kept).  Every one of the maxIter iterations is enqueued (the ones after
+    // convergence return at once), so maxIter should stay near what the scene needs.  The workspace is allocated on the first
+    // enable.
+    void setImplicitViscosity(float nu, float nuBoundary = 0.0f, float tol = 1e-4f, int maxIter = 20);
+    float implicitViscosity() const { return implNu_; }
+    // iterations and final relative residual of the last solve (0 before the first); synchronise
+    int lastViscosityIterations() const;
+    float lastViscosityResidual() const;
     // addition: true when step() enqueues the same kernel sequence every call and never synchronises the host.
     // Only the three shipped solver types can say so: a user-derived solver (the reference API allows subclassing
     // BasicSPHSolver) has per-step host logic of its own, so it is never captured into a step graph.
@@ -256,6 +268,9 @@ protected:
     float* omegaNormBuffer() const { return omegaNorm_->addr(); }
     void vorticity(float rho0);
     void confine(const std::shared_ptr<SPHParticles>& fluids, float rho0, float dt);
+    // implicit viscosity: on when implNu_ > 0; runs where confine() would run, before it
+    bool implicitViscosityOn() const { return implNu_ > 0.0f; }
+    void implicitViscosity(const std::shared_ptr<SPHParticles>& fluids, float rho0, float rhoB, float dt);
     // two-way coupled bodies: the reaction of the sweep just run, with its c (sphk_bodies_react); nothing without dynamic bodies
     void react(float c) { if (reacting_) sphb200::check(sphk_bodies_react(current_.ctx, &current_.abi, c), "sphk_bodies_react"); }
     bool reacting_ = false;
@@ -266,6 +281,10 @@ private:
     float vortEps_ = 0.0f;
     std::unique_ptr<DArray<float3>> omega_;      // vorticity omega
     std::unique_ptr<DArray<float>> omegaNorm_;   // |omega|, the neighbour scalar of the confinement sweep
+    float implNu_ = 0.0f, implNuB_ = 0.0f, implTol_ = 1e-4f;
+    int implMaxIter_ = 20;
+    std::unique_ptr<DArray<float>> viscWork_;    // workspace of sphk_implicit_viscosity
+    void viscStats(int& iters, float& residual) const;
 };
 
 // ---- DFSPHSolver.h:20-64 ----------------------------------------------------------------------

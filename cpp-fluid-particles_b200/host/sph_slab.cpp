@@ -391,6 +391,10 @@ void SlabSPHSystem::beginStep() {
 
 float SlabSPHSystem::step() {
     if (!ok_) return 0.0f;
+    // implicit viscosity needs a global dot product per CG iteration and a halo of the direction before each product
+    const auto* known = dynamic_cast<const BasicSPHSolver*>(solver_.get());
+    if (known && known->implicitViscosity() > 0.0f)
+        throw std::runtime_error("SlabSPHSystem: implicit viscosity is not supported on slab ranks (single-GPU SPHSystem only)");
     cudaStream_t st = engine_->stream();
     CUDA_CALL(cudaEventRecord(evStart_, st));
     if (strayCap_ > 0 && haveRanges_ && comm_) collectStrays();

@@ -973,6 +973,16 @@ class SlabSystem(SphkOps):
         self.rebalanced += 1
         return True
 
+    # implicit viscosity needs a global dot product per CG iteration and a halo of the direction before each product
+    @property
+    def implicit_nu(self):
+        return 0.0
+
+    @implicit_nu.setter
+    def implicit_nu(self, nu):
+        if nu != 0.0:
+            raise ValueError("implicit viscosity is not supported on slab ranks (single-GPU engine.SphkSystem only)")
+
     def step(self):
         self._step_no += 1
         if self.stray_cap and self._ranges is not None:

@@ -76,6 +76,15 @@ int   sph_app_step_graph_active(sph_app* app);
 /* Vorticity confinement of strength eps >= 0 in every following step (BasicSPHSolver::setVorticityConfinement; 0 = off,
  * the default).  No reference counterpart: returns 1 on the reference build, and for eps < 0 or NaN. */
 int   sph_app_set_vorticity(sph_app* app, float eps);
+/* Implicit viscosity in every following step (BasicSPHSolver::setImplicitViscosity; DESIGN.md section 2.5): kinematic viscosity
+ * nu of the fluid and nu_boundary against walls and bodies, CG to |b - A v|_M <= tol |b|_M or max_iter iterations; nu = 0 = off
+ * (the default).  No reference counterpart: returns 1 on the reference build, for nu or nu_boundary < 0 or not finite,
+ * tol <= 0 or NaN, max_iter < 1 or > 1000 (SPHK_IMPLICIT_VISCOSITY_MAX_ITER), and for nu_boundary > 0 in a system with dynamic
+ * bodies (the setting is then kept). */
+int   sph_app_set_implicit_viscosity(sph_app* app, float nu, float nu_boundary, float tol, int max_iter);
+/* iterations and relative residual |r|_M / |b|_M of the last implicit viscosity solve (0, 0 before the first); synchronises;
+ * 1 on the reference build */
+int   sph_app_viscosity_stats(sph_app* app, int* iterations, float* rel_residual);
 /* Kinematic rigid bodies (SPHSystem's constructor with a vector of sphb200::KinematicBody; DESIGN.md section 2.3).  No
  * reference counterpart: NULL / 1 on the reference build.  Body b is the points body_xyz[body_begin[b] .. body_begin[b+1])
  * (body coordinates; body_begin[0] = 0), pose[7 b ..] = {cx, cy, cz, qx, qy, qz, qw} (quaternion scalar part last),

@@ -259,6 +259,40 @@ int sphk_fused_viscosity_surface_vorticity(sphk_ctx* ctx, const sphk_scene* s, f
 int sphk_fused_pbd_xsph_vorticity(sphk_ctx* ctx, const sphk_scene* s, float c, float rho0, float* color_grad_or_null,
                                   float rho_boundary, float* omega, float* omega_norm);
 
+/* ---- implicit viscosity (no reference counterpart: Weiler, Koschier, Brand & Bender 2018; DESIGN.md section 2.5) ------------
+ * Solves A v = b for the new fluid velocities, v* = the velocities entering the solve, d = x_i - x_j, g = the kernel gradient
+ * factor (gradW_ij = g d, g <= 0), R = support radius:
+ *   c_ij    = -10 nu V_j g / (r^2 + 0.01 R^2),  V_j = m_j / rho0   (boundary pairs: nu_boundary and m_b / rho_boundary)
+ *   (A v)_i = D_i v_i - dt sum_j c_ij d (d . v_j)                         (fluid neighbours)
+ *   D_i     = I + dt sum_j c_ij d d^T + dt sum_b c_ib d d^T
+ *   b_i     = v*_i + dt sum_b c_ib d (d . v_b)                            (v_b: 0, or a kinematic body's velocity)
+ * A is self-adjoint in <u,w>_M = sum m_i u_i . w_i with eigenvalues >= 1.  Preconditioned CG in that inner product with the
+ * block-Jacobi preconditioner D_i^-1, x0 = v*, m-weighted dot products in double in a fixed shape; the loop ends at the first
+ * of |b - A v|_M <= tol |b|_M, <r,z>_M = 0 (a fluid at rest comes out unchanged) and max_iter iterations.  The loop test runs on
+ * the device: max_iter iterations are enqueued, the ones after the end return at once (no host synchronisation; a step graph
+ * replays it).  The solution goes to the API velocities and the records.  `work` = caller-owned device floats,
+ * sphk_implicit_viscosity_work_floats(n) of them for n fluid particles (so nothing is allocated inside a captured step).
+ * SPHK_ERR_INVALID: NULL or aliased buffers, nu or nu_boundary < 0 / not finite, rho0 or rho_boundary <= 0, tol <= 0 or NaN,
+ * max_iter < 1 or > SPHK_IMPLICIT_VISCOSITY_MAX_ITER, dt < 0.  SPHK_ERR_STATE: an active range is set (slab ranks), or
+ * nu_boundary > 0 with dynamic bodies declared (sphk_bodies_set_dynamics: the viscous wall force is not part of their reaction).
+ * Every one of the max_iter iterations is enqueued (6 launches each, a matvec sweep over all particles among them) and a
+ * captured step graph holds them all; the ones after the end cost about 20-30 us each on the 2M-particle scenes, so max_iter
+ * should not be far above the iterations a scene needs (DESIGN.md section 2.5). */
+#define SPHK_IMPLICIT_VISCOSITY_MAX_ITER 1000
+long long sphk_implicit_viscosity_work_floats(int n);
+int sphk_implicit_viscosity(sphk_ctx* ctx, const sphk_scene* s, float* work, float nu, float nu_boundary, float dt, float rho0,
+                            float rho_boundary, float tol, int max_iter);
+/* iterations and final relative residual |r|_M / |b|_M of the last sphk_implicit_viscosity (0, 0 before the first), kept by the
+ * context (the workspace may be freed after the solve); synchronises */
+int sphk_implicit_viscosity_stats(sphk_ctx* ctx, int* iterations, float* rel_residual);
+/* The two sweeps of the solve, one call each (per-element tests): D_i (float[6n], {xx, yy, zz, xy, xz, yz}) and b_i (float3[n]);
+ * (A p)_i (float3[n]) from D (float[6n]) and p (float3[n]).  The matvec leaves the records' velocities as the API array holds
+ * them.  Same validation as sphk_implicit_viscosity. */
+int sphk_visc_implicit_setup(sphk_ctx* ctx, const sphk_scene* s, float* d_out, float* b_out, float nu, float nu_boundary, float dt,
+                             float rho0, float rho_boundary);
+int sphk_visc_implicit_matvec(sphk_ctx* ctx, const sphk_scene* s, const float* d_in, const float* p_in, float* ap_out, float nu,
+                              float dt, float rho0);
+
 /* ---- kinematic rigid bodies (no reference counterpart; DESIGN.md section 2.3) ---------------------------------------------
  * A body is a rigid set of boundary particles given in body coordinates r_k, with a pose (centre c, unit quaternion q) and
  * a motion (linear velocity V, angular velocity Omega, both in the world frame).  Poses and motions live in device memory.
