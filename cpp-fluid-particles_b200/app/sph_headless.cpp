@@ -9,7 +9,12 @@
 //
 //   sph_headless [--solver sph|dfsph|pbd] [--frames N] [--box L | --box LX LY LZ] [--block NX NY NZ] [--origin X Y Z]
 //                [--dt DT] [--iters K] [--vorticity EPS] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] [--ranks N [--rank R --rendezvous DIR]]
-//                [--bullets K] [--stir OMEGA] [--float REL] [--implicit-viscosity NU]
+//                [--bullets K] [--stir OMEGA] [--float REL] [--implicit-viscosity NU] [--tap SPEED] [--drain SIDE] [--capacity N]
+// --tap SPEED adds an emitter (SPHSystem's constructor with sphb200::OpenBoundaries, DESIGN.md section 2.6): an 8 x 8 nozzle at the
+// fluid spacing, centred above the block at 0.85 of the box height, pointing down, SPEED fast.  --drain SIDE adds a sink on the
+// floor: the box [0, SIDE] x [0, 0.05 L] x [0, SIDE] in the (0, 0, 0) corner of the clamp box.  --capacity N is the fluid set's
+// capacity (default: twice the initial count).  Single GPU only; they combine with --stir, --float, --vorticity and
+// --implicit-viscosity.  The JSON summary then reports fluid_count, emitted, removed and refused.
 // --vorticity EPS turns on vorticity confinement of strength EPS (BasicSPHSolver::setVorticityConfinement) after the
 // constructor's step 0, for every solver and with --ranks.
 // --implicit-viscosity NU turns on the implicit viscosity solve (BasicSPHSolver::setImplicitViscosity) with nu = nu_boundary = NU
@@ -24,7 +29,8 @@
 // is REL * m0 / spacing^3 * V with V = (extent + boundary spacing)^3, the volume its particles stand for (the fluid's mass
 // per unit volume is m0 / spacing^3, DESIGN.md section 2.4), and its moments those of a solid cube of that mass and side.  Fluid lattice points within one spacing of it are dropped.  Single GPU
 // only, and not together with --stir.
-// --emit-scene writes the generated scene (PREFIX.fluid.f32, PREFIX.boundary.f32; with --stir also PREFIX.body.f32, the
+// --emit-scene writes the generated scene (PREFIX.fluid.f32, PREFIX.boundary.f32; with --tap PREFIX.emitter.f32 = {origin,
+// direction, speed, spacing, width, height}; with --drain PREFIX.sink.f32 = {lo, hi}; with --stir also PREFIX.body.f32, the
 // paddle's points in body coordinates, and PREFIX.body_state.f32 = pose {c, q = (x, y, z, w)} + motion {V, Omega}; with
 // --float the same for the cube and PREFIX.body_dyn.f32 = {M, Ix, Iy, Iz}) and
 // exits: needs no GPU, lets a test compare this generator with the python one the benchmarks use, or rebuild the scene.
@@ -77,6 +83,9 @@ struct Options {
     float stirOmega = 0.0f;
     bool floating = false;                    // --float REL: a free cube of relative density REL
     float floatRel = 0.0f;
+    float tap = 0.0f;                         // --tap SPEED: an emitter above the block (0: none)
+    float drain = 0.0f;                       // --drain SIDE: a floor sink (0: none)
+    long long capacity = 0;                   // --capacity N: fluid capacity of an open system (0: twice the initial count)
     int bullets = 0;                          // test aid: this many top-layer particles start at ~3 cell planes per step
     int ranks = 1, rank = -1;                 // --ranks N: SlabSPHSystem on N GPUs; --rank R: this process is rank R
     std::string rendezvous;
@@ -98,6 +107,9 @@ bool parse(int argc, char** argv, Options& o) {
         else if (a == "--implicit-viscosity" && need(i, 1)) o.implicitNu = static_cast<float>(std::atof(argv[++i]));
         else if (a == "--stir" && need(i, 1)) { o.stir = true; o.stirOmega = static_cast<float>(std::atof(argv[++i])); }
         else if (a == "--float" && need(i, 1)) { o.floating = true; o.floatRel = static_cast<float>(std::atof(argv[++i])); }
+        else if (a == "--tap" && need(i, 1)) o.tap = static_cast<float>(std::atof(argv[++i]));
+        else if (a == "--drain" && need(i, 1)) o.drain = static_cast<float>(std::atof(argv[++i]));
+        else if (a == "--capacity" && need(i, 1)) o.capacity = std::atoll(argv[++i]);
         else if (a == "--ranks" && need(i, 1)) o.ranks = std::atoi(argv[++i]);
         else if (a == "--rank" && need(i, 1)) o.rank = std::atoi(argv[++i]);
         else if (a == "--rendezvous" && need(i, 1)) o.rendezvous = argv[++i];
@@ -132,6 +144,15 @@ bool parse(int argc, char** argv, Options& o) {
     }
     if (o.implicitNu > 0.0f && (o.ranks > 1 || o.floating)) {
         std::fprintf(stderr, "sph_headless: --implicit-viscosity runs on one GPU only (not with --ranks) and not together with --float\n");
+        return false;
+    }
+    if (!(o.tap >= 0.0f) || !std::isfinite(o.tap) || !(o.drain >= 0.0f) || !std::isfinite(o.drain) || o.capacity < 0 ||
+        o.capacity > 0x7fffffffLL) {
+        std::fprintf(stderr, "sph_headless: --tap SPEED and --drain SIDE need finite values > 0, --capacity N a count\n");
+        return false;
+    }
+    if ((o.tap > 0.0f || o.drain > 0.0f) && o.ranks > 1) {
+        std::fprintf(stderr, "sph_headless: --tap and --drain run on one GPU only (open boundaries are not supported with --ranks)\n");
         return false;
     }
     return o.frames >= 0 && o.vorticity >= 0.0f && o.block[0] > 0 && o.block[1] > 0 && o.block[2] > 0 &&
@@ -226,6 +247,22 @@ std::vector<float3> clear_of(const std::vector<float3>& fluid, const sphb200::Ki
     return out;
 }
 
+// --tap / --drain (DESIGN.md section 2.6)
+sphb200::OpenBoundaries open_boundaries(const Options& o, float spacing) {
+    sphb200::OpenBoundaries ob;
+    if (o.tap > 0.0f) {
+        sphb200::Emitter e;
+        e.origin = make_float3(o.origin[0] + 0.5f * spacing * (o.block[0] - 1), 0.85f * o.box[1], o.origin[2] + 0.5f * spacing * (o.block[2] - 1));
+        e.direction = make_float3(0.0f, -1.0f, 0.0f);
+        e.speed = o.tap;
+        e.spacing = spacing;
+        e.width = e.height = 8;
+        ob.emitters.push_back(e);
+    }
+    if (o.drain > 0.0f) ob.sinks.push_back({make_float3(0.0f, 0.0f, 0.0f), make_float3(o.drain, 0.05f * o.box[1], o.drain)});
+    return ob;
+}
+
 std::vector<float> flat(const std::vector<float3>& p) {
     std::vector<float> v;
     v.reserve(3 * p.size());
@@ -278,7 +315,8 @@ int main(int argc, char** argv) {
     Options o;
     if (!parse(argc, argv, o)) {
         std::fprintf(stderr, "usage: sph_headless [--solver sph|dfsph|pbd] [--frames N] [--box L | LX LY LZ] [--block NX NY NZ] "
-                             "[--origin X Y Z] [--dt DT] [--iters K] [--vorticity EPS] [--implicit-viscosity NU] [--stir OMEGA | --float REL] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] "
+                             "[--origin X Y Z] [--dt DT] [--iters K] [--vorticity EPS] [--implicit-viscosity NU] [--stir OMEGA | --float REL] "
+                             "[--tap SPEED] [--drain SIDE] [--capacity N] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] "
                              "[--ranks N [--rank R --rendezvous DIR]]\n");
         return 2;
     }
@@ -296,6 +334,8 @@ int main(int argc, char** argv) {
     if (o.stir) bodies.push_back(paddle(o, sphSpacing, boundarySpacing));
     if (o.floating) bodies.push_back(floating_cube(o, sphSpacing, boundarySpacing));
     if (!bodies.empty()) fluidPoints = clear_of(fluidPoints, bodies[0], boundarySpacing);
+    const sphb200::OpenBoundaries openB = open_boundaries(o, sphSpacing);
+    const bool open = !openB.emitters.empty() || !openB.sinks.empty();
     if (!o.emitScene.empty()) {
         const int3 cells = cellSize;
         bool ok = write_floats(o.emitScene + ".fluid.f32", flat(fluidPoints)) &&
@@ -310,6 +350,11 @@ int main(int argc, char** argv) {
             if (ok && o.floating)
                 ok = write_floats(o.emitScene + ".body_dyn.f32", {b.mass, b.inertia.x, b.inertia.y, b.inertia.z});
         }
+        for (const auto& e : openB.emitters)
+            ok = ok && write_floats(o.emitScene + ".emitter.f32", {e.origin.x, e.origin.y, e.origin.z, e.direction.x, e.direction.y, e.direction.z,
+                                                                    e.speed, e.spacing, float(e.width), float(e.height)});
+        for (const auto& b : openB.sinks)
+            ok = ok && write_floats(o.emitScene + ".sink.f32", {b.lo.x, b.lo.y, b.lo.z, b.hi.x, b.hi.y, b.hi.z});
         std::printf("{\"cells\": [%d, %d, %d]}\n", cells.x, cells.y, cells.z);
         return ok ? 0 : 5;
     }
@@ -369,16 +414,19 @@ int main(int argc, char** argv) {
     const float sphAirPressure = 0.0001f;
 
     // ---- the reference's call sites: particles (main.cpp:86,117), solver (:119-130), system (:131-134) ----
-    auto fluidParticles = std::make_shared<SPHParticles>(fluidPoints);
+    const unsigned int capacity = open ? static_cast<unsigned int>(o.capacity > 0 ? o.capacity : 2LL * static_cast<long long>(fluidPoints.size()))
+                                       : static_cast<unsigned int>(fluidPoints.size());
+    auto fluidParticles = open ? std::make_shared<SPHParticles>(fluidPoints, capacity) : std::make_shared<SPHParticles>(fluidPoints);
     auto boundaryParticles = std::make_shared<SPHParticles>(boundary_shell(cellSize, spaceSize));
     const int nFluid = static_cast<int>(fluidParticles->size()), nBoundary = static_cast<int>(boundaryParticles->size());
+    const int nSlots = static_cast<int>(fluidParticles->capacity());   // the solver's buffers hold every slot
     std::shared_ptr<BaseSolver> pSolver;
     if (o.solver == "pbd")
-        pSolver = o.iters > 0 ? std::make_shared<PBDSolver>(nFluid, o.iters) : std::make_shared<PBDSolver>(nFluid);
+        pSolver = o.iters > 0 ? std::make_shared<PBDSolver>(nSlots, o.iters) : std::make_shared<PBDSolver>(nSlots);
     else if (o.solver == "dfsph")
-        pSolver = o.iters > 0 ? std::make_shared<DFSPHSolver>(nFluid, -1.0f, -1.0f, o.iters) : std::make_shared<DFSPHSolver>(nFluid);
+        pSolver = o.iters > 0 ? std::make_shared<DFSPHSolver>(nSlots, -1.0f, -1.0f, o.iters) : std::make_shared<DFSPHSolver>(nSlots);
     else
-        pSolver = std::make_shared<BasicSPHSolver>(nFluid);
+        pSolver = std::make_shared<BasicSPHSolver>(nSlots);
     BasicSPHSolver* basicSolver = dynamic_cast<BasicSPHSolver*>(pSolver.get());   // (the systems take pSolver over)
     std::shared_ptr<SPHSystem> pSystem;
     std::shared_ptr<SlabSPHSystem> pSlab;
@@ -389,6 +437,11 @@ int main(int argc, char** argv) {
                                                 dt, sphM0, sphRho0, sphRhoBoundary, sphStiff, sphVisc, sphSurfaceTensionIntensity,
                                                 sphAirPressure, sphG, cellSize, boot);
         if (!pSlab->ok()) { std::fprintf(stderr, "sph_headless: rank %d: SlabSPHSystem did not come up\n", o.rank); return 4; }
+    } else if (open) {
+        pSystem = std::make_shared<SPHSystem>(fluidParticles, boundaryParticles, pSolver, spaceSize, sphCellLength, sphSmoothingRadius,
+                                              dt, sphM0, sphRho0, sphRhoBoundary, sphStiff, sphVisc, sphSurfaceTensionIntensity,
+                                              sphAirPressure, sphG, cellSize, bodies, openB);
+        if (!pSystem->openBoundariesActive()) { std::fprintf(stderr, "sph_headless: the open boundaries were refused\n"); return 4; }
     } else if (!bodies.empty()) {
         pSystem = std::make_shared<SPHSystem>(fluidParticles, boundaryParticles, pSolver, spaceSize, sphCellLength, sphSmoothingRadius,
                                               dt, sphM0, sphRho0, sphRhoBoundary, sphStiff, sphVisc, sphSurfaceTensionIntensity,
@@ -469,9 +522,16 @@ int main(int argc, char** argv) {
         std::fflush(stdout);
         return 0;
     }
+    std::string openJson;
+    if (open) {
+        const sphb200::OpenBoundaryStats st = pSystem->openBoundaryStats();
+        openJson = ", \"fluid_count\": " + std::to_string(pSystem->fluidSize()) + ", \"emitted\": " + std::to_string(st.emitted) +
+                   ", \"removed\": " + std::to_string(st.removed) + ", \"refused\": " + std::to_string(st.refused) +
+                   ", \"open_check\": " + std::to_string(pSystem->openBoundaryCheck());
+    }
     std::printf("{\"solver\": \"%s\", \"n_fluid\": %d, \"n_boundary\": %d, \"cells\": [%d, %d, %d], \"dt\": %g, \"frames\": %d, "
-                "\"avg_ms_per_frame\": %.4f, \"max_ms_per_frame\": %.4f, \"particle_steps_per_s\": %.1f}\n",
+                "\"avg_ms_per_frame\": %.4f, \"max_ms_per_frame\": %.4f, \"particle_steps_per_s\": %.1f%s}\n",
                 o.solver.c_str(), nFluid, nBoundary, cellSize.x, cellSize.y, cellSize.z, dt, frameId, avg, worst,
-                avg > 0.0f ? double(nFluid) / (double(avg) * 1e-3) : 0.0);
+                avg > 0.0f ? double(nFluid) / (double(avg) * 1e-3) : 0.0, openJson.c_str());
     return 0;
 }

@@ -35,6 +35,8 @@ SPHK_FUNCTIONS = [
     "sphk_bodies_get_motion", "sphk_bodies_get_impulse",
     "sphk_implicit_viscosity_work_floats", "sphk_implicit_viscosity", "sphk_implicit_viscosity_stats", "sphk_visc_implicit_setup",
     "sphk_visc_implicit_matvec",
+    "sphk_emitter_axes", "sphk_emitter_advance", "sphk_emit", "sphk_sinks_apply", "sphk_sinks_removed", "sphk_fluid_set_count",
+    "sphk_open_check",
 ]
 SPH_APP_FUNCTIONS = [
     "sph_app_create", "sph_app_destroy", "sph_app_step", "sph_app_fluid_size", "sph_app_boundary_size",
@@ -42,10 +44,11 @@ SPH_APP_FUNCTIONS = [
     "sph_app_submit", "sph_app_wait", "sph_app_dfsph_iterations", "sph_app_set_option", "sph_app_set_vorticity",
     "sph_app_create_with_bodies", "sph_app_set_body_motion", "sph_app_body_pose", "sph_app_step_graph_active",
     "sph_app_create_with_dynamic_bodies", "sph_app_body_motion", "sph_app_body_impulse", "sph_app_set_implicit_viscosity",
-    "sph_app_viscosity_stats",
+    "sph_app_viscosity_stats", "sph_app_create_open", "sph_app_open_boundary_stats",
 ]
 
 OPT_NEIGHBOR_LIST, OPT_LIST_CAPACITY, OPT_LIST_SKIN, OPT_SIMPLE_LIST_BUILD, OPT_TILE, OPT_STAGED_LIST_BUILD, OPT_PATCH = 1, 2, 5, 6, 9, 10, 11
+MAX_EMITTERS, MAX_SINKS = 16, 16   # SPHK_MAX_EMITTERS, SPHK_MAX_SINKS
 # tile-list geometry of csrc/sphk_internal.cuh (SPHK_BLOCK, SPHK_TILE_WINS, SPHK_TILE_CAP): sphk_get_tile_lists copies
 # TILE_WINDOWS windows per tile of TILE_PARTICLES particles; a tile whose windows exceed TILE_CAP records walks the cells
 TILE_PARTICLES, TILE_WINDOWS, TILE_CAP = 128, 18, 1535
@@ -55,6 +58,27 @@ def body_mass_inertia(bodies) -> np.ndarray:
     """{M, Ix, Iy, Iz} per body from the body dicts' optional "mass" (default 0: kinematic) and "inertia" (default 0)."""
     return np.ascontiguousarray([[float(b.get("mass", 0.0)), *[float(x) for x in b.get("inertia", (0.0, 0.0, 0.0))]]
                                  for b in bodies], np.float32).reshape(-1, 4)
+
+
+class SphkEmitter(C.Structure):
+    """sphk_emitter (include/sphk.h); sph_app_emitter has the same layout."""
+    _fields_ = [("origin", C.c_float * 3), ("direction", C.c_float * 3), ("speed", C.c_float), ("spacing", C.c_float),
+                ("width", C.c_int), ("height", C.c_int)]
+
+
+def emitter_struct(e: dict) -> SphkEmitter:
+    """An emitter dict {"origin", "direction", "speed", "spacing", "width", "height"} as the C struct."""
+    k = SphkEmitter()
+    k.origin[:] = [float(x) for x in e["origin"]]
+    k.direction[:] = [float(x) for x in e["direction"]]
+    k.speed, k.spacing = float(e["speed"]), float(e["spacing"])
+    k.width, k.height = int(e.get("width", 1)), int(e.get("height", 1))
+    return k
+
+
+def sink_boxes(sinks) -> np.ndarray:
+    """[(lo, hi), ...] as float32 {lo.xyz, hi.xyz} rows."""
+    return np.ascontiguousarray([[*lo, *hi] for lo, hi in sinks], np.float32).reshape(-1, 6)
 
 
 class SphkGrid(C.Structure):
@@ -117,6 +141,7 @@ def app_lib(path: str = LIBHOST):
         L.sph_app_create.restype = C.c_void_p
         L.sph_app_create_with_bodies.restype = C.c_void_p
         L.sph_app_create_with_dynamic_bodies.restype = C.c_void_p
+        L.sph_app_create_open.restype = C.c_void_p
         L.sph_app_step.restype = C.c_float
         L.sph_app_engine.restype = C.c_char_p
         L.sph_app_destroy.restype = None
@@ -150,8 +175,9 @@ class SphApp:
     `lib_path` selects the engine underneath: this repo's libsphhost.so (default) or the reference's own
     CUDA build oracle/_ref/libsphref.so -- the facade source is the same file for both."""
 
-    def __init__(self, scene, lib_path: str = LIBHOST, bodies=None):
-        """bodies: rigid bodies in engine.SphkSystem's format (sph_app_create_with_bodies; with a "mass" key on any body,
+    def __init__(self, scene, lib_path: str = LIBHOST, bodies=None, max_fluid=None, emitters=None, sinks=None):
+        """emitters / sinks / max_fluid: open boundaries (sph_app_create_open; engine.SphkSystem's format), no bodies.
+        bodies: rigid bodies in engine.SphkSystem's format (sph_app_create_with_bodies; with a "mass" key on any body,
         sph_app_create_with_dynamic_bodies: dynamics are declared when some mass is > 0, as in engine.SphkSystem); their
         particles follow the static boundary set, so nB counts them."""
         self.L = app_lib(lib_path)
@@ -160,7 +186,15 @@ class SphApp:
         bd = np.ascontiguousarray(scene.boundary, np.float32)
         self.nF, self.nB = fl.shape[0], bd.shape[0]
         prm = app_params(scene.params)
-        if bodies is not None:       # (an empty list: the bodies constructor without bodies)
+        if emitters is not None or sinks is not None:
+            em = list(emitters or [])
+            ems = (SphkEmitter * max(1, len(em)))(*[emitter_struct(e) for e in em])
+            boxes = sink_boxes(sinks or [])
+            cap = int(max_fluid) if max_fluid is not None else self.nF
+            self.h = self.L.sph_app_create_open(fl.ctypes.data_as(C.c_void_p), C.c_int(self.nF), C.c_int(cap),
+                                                bd.ctypes.data_as(C.c_void_p), C.c_int(self.nB), C.c_int(len(em)), ems,
+                                                C.c_int(boxes.shape[0]), boxes.ctypes.data_as(C.c_void_p), C.byref(prm))
+        elif bodies is not None:     # (an empty list: the bodies constructor without bodies)
             pts = [np.asarray(b["points"], np.float32).reshape(-1, 3) for b in bodies]
             xyz = np.ascontiguousarray(np.concatenate(pts, 0) if pts else np.zeros((0, 3), np.float32))
             begin = np.ascontiguousarray(np.concatenate([[0], np.cumsum([len(q) for q in pts])]).astype(np.int32))
@@ -187,9 +221,23 @@ class SphApp:
         return self.L.sph_app_engine().decode()
 
     def step(self) -> float:
-        return float(self.L.sph_app_step(self.h))
+        ms = float(self.L.sph_app_step(self.h))
+        self.nF = int(self.L.sph_app_fluid_size(self.h))    # open boundaries change the live count
+        return ms
+
+    @property
+    def fluid_count(self) -> int:
+        return int(self.L.sph_app_fluid_size(self.h))
+
+    def open_boundary_stats(self):
+        """({"emitted", "removed", "refused"} cumulative particle counts, sticky count-check bits); synchronises."""
+        st, bits = (C.c_longlong * 3)(), C.c_int(0)
+        if self.L.sph_app_open_boundary_stats(self.h, st, C.byref(bits)):
+            raise RuntimeError("sph_app_open_boundary_stats failed (reference engine)")
+        return {"emitted": int(st[0]), "removed": int(st[1]), "refused": int(st[2])}, int(bits.value)
 
     def download(self) -> dict:
+        self.nF = self.fluid_count
         out = {"pos": np.empty((self.nF, 3), np.float32), "vel": np.empty((self.nF, 3), np.float32),
                "density": np.empty(self.nF, np.float32), "pressure": np.empty(self.nF, np.float32),
                "mass": np.empty(self.nF, np.float32), "p2c": np.empty(self.nF, np.int32)}

@@ -129,6 +129,12 @@ struct sphk_ctx {
     long long launches = 0;
     BodyState* bodies = nullptr;     // non-null after sphk_bodies_init
     float* viscStats = nullptr;      // [2] device: {iterations (int bits), |r|_M / |b|_M} of the last sphk_implicit_viscosity
+    // open boundaries (sphk_sinks_apply / sphk_fluid_set_count; allocated on first use)
+    int* openDev = nullptr;          // device [2]: {particles the last sphk_sinks_apply removed, sticky check bits}
+    int* openPinned = nullptr;       // pinned [1]: the removed count, copied behind the sink kernel
+    cudaEvent_t sinkEvent = nullptr; // recorded after that copy
+    bool sinksApplied = false;
+    mutable bool countSettable = false;   // a fluid search ran and no sweep since (sphk_fluid_set_count is valid)
 };
 
 struct DevScene {

@@ -244,6 +244,9 @@ extern "C" void sphk_destroy(sphk_ctx* c) {
     cudaFree(c->snapA); cudaFree(c->snapB); cudaFree(c->rec.a); cudaFree(c->rec.b); cudaFree(c->massRange); cudaFree(c->dispMax); cudaFree(c->cellFlag);
     cudaFree(c->tmpF); cudaFree(c->partial); cudaFree(c->loops); cudaFree(c->viscStats); cudaFree(c->cnt); cudaFree(c->nbr); cudaFree(c->cubTemp); cudaFree(c->tileWin);
     if (c->pinned) cudaFreeHost(c->pinned);
+    cudaFree(c->openDev);
+    if (c->openPinned) cudaFreeHost(c->openPinned);
+    if (c->sinkEvent) cudaEventDestroy(c->sinkEvent);
     sphk_bodies_release(c->bodies);
     delete c;
 }
@@ -351,7 +354,7 @@ extern "C" int sphk_neighbor_search(sphk_ctx* c, int which, const sphk_particles
     k_cell_start<<<sphk_blocks(c->ncells + 1), SPHK_BLOCK, 0, st>>>(c->keysSorted, n, c->ncells, cell_start);
     c->launches += 3 + 4;   // 3 own kernels + CUB onesweep (histogram, scan, <=3 passes): counted as 4
     if (fluid) { c->nF = n; c->fluidSearched = true; c->permValid = true; c->searchEpoch++; c->posDirty = false; c->advected = false; c->sTag = nullptr;
-                 c->actBegin = 0; c->actCount = -1; }
+                 c->actBegin = 0; c->actCount = -1; c->countSettable = true; }
     else { c->nB = n; c->boundarySearched = true; c->listEpoch = ~0ull; c->permValid = false; }
     SPHK_CUDA_TRY(cudaGetLastError());
     return SPHK_OK;
@@ -1016,5 +1019,229 @@ extern "C" int sphk_bodies_get_local(sphk_ctx* c, float* local_out) {
     if (!c->bodies || !c->boundarySearched) return SPHK_ERR_STATE;
     SPHK_CUDA_TRY(cudaMemcpyAsync(local_out, c->bodies->local, sizeof(float4) * static_cast<size_t>(c->nB), cudaMemcpyDeviceToDevice,
                                   c->stream));
+    return SPHK_OK;
+}
+
+// ---- open boundaries: emitters and sinks (no reference counterpart; DESIGN.md section 2.6) ----------------------------------
+// A step of a system with emitters or sinks: k_open_sinks_mark over the n live slots, k_open_emit into [n, n + e), the
+// unchanged fluid search over n + e slots (marked particles get the out-of-grid key and sort behind the live ones), then
+// sphk_fluid_set_count(L = n + e - removed) with k_open_count_check.  The schedule of an emitter lives on the host
+// (sphk_emitter_advance); the kernels only write what it decided.
+
+#define SPHK_EMIT_LAYERS 32          // layer offsets per emission launch (kernel parameters: no host-to-device copy)
+struct EmitLayers { float delta[SPHK_EMIT_LAYERS]; };
+struct SinkBoxes { float b[6 * SPHK_MAX_SINKS]; };
+
+// One thread per emitted particle k W H + b W + a of the launch's layers; float operations in the order of sphk.h, no contraction.
+__global__ void __launch_bounds__(SPHK_BLOCK)
+k_open_emit(float* __restrict__ pos, float* __restrict__ vel, float* __restrict__ mass, float* __restrict__ density,
+            float* __restrict__ pressure, float* __restrict__ hist, int histKind, int dst, int W, int H, int nLayers, EmitLayers L,
+            float3 o, float3 d, float3 e1, float3 e2, float s, float u, float m0, float dt) {
+    const int t = blockIdx.x * SPHK_BLOCK + threadIdx.x;
+    const int per = W * H;
+    if (t >= nLayers * per) return;
+    const int k = t / per, r = t - k * per, b = r / W, a = r - b * W;
+    const float ta = __fmul_rn(__fsub_rn(static_cast<float>(a), __fmul_rn(0.5f, static_cast<float>(W - 1))), s);
+    const float tb = __fmul_rn(__fsub_rn(static_cast<float>(b), __fmul_rn(0.5f, static_cast<float>(H - 1))), s);
+    const float delta = L.delta[k];
+    const float3 x = f3(__fadd_rn(__fadd_rn(__fadd_rn(o.x, __fmul_rn(ta, e1.x)), __fmul_rn(tb, e2.x)), __fmul_rn(delta, d.x)),
+                        __fadd_rn(__fadd_rn(__fadd_rn(o.y, __fmul_rn(ta, e1.y)), __fmul_rn(tb, e2.y)), __fmul_rn(delta, d.y)),
+                        __fadd_rn(__fadd_rn(__fadd_rn(o.z, __fmul_rn(ta, e1.z)), __fmul_rn(tb, e2.z)), __fmul_rn(delta, d.z)));
+    const float3 v = f3(__fmul_rn(u, d.x), __fmul_rn(u, d.y), __fmul_rn(u, d.z));
+    const int i = dst + t;
+    store3(pos, i, x);
+    store3(vel, i, v);
+    mass[i] = m0;
+    density[i] = 0.f;
+    pressure[i] = 0.f;
+    if (histKind == 1) hist[i] = 0.f;
+    else if (histKind == 2)
+        store3(hist, i, f3(__fsub_rn(x.x, __fmul_rn(dt, v.x)), __fsub_rn(x.y, __fmul_rn(dt, v.y)), __fsub_rn(x.z, __fmul_rn(dt, v.z))));
+}
+
+// Marks the live particles inside a sink (lo <= x < hi on all axes) and counts them: one ballot per warp, one integer add per
+// warp with a hit (order-independent, so the count is deterministic).  Every lane reaches the ballot.
+__global__ void __launch_bounds__(SPHK_BLOCK)
+k_open_sinks_mark(float* __restrict__ pos, float* __restrict__ vel, int n, SinkBoxes B, int nBoxes, int* __restrict__ count) {
+    const int i = blockIdx.x * SPHK_BLOCK + threadIdx.x;
+    bool in = false;
+    if (i < n) {
+        const float3 p = load3(pos, i);
+        for (int k = 0; k < nBoxes; ++k) {
+            const float* q = B.b + 6 * k;
+            in = in || (p.x >= q[0] && p.x < q[3] && p.y >= q[1] && p.y < q[4] && p.z >= q[2] && p.z < q[5]);
+        }
+        if (in) {
+            store3(pos, i, f3(-1.0e6f, -1.0e6f, -1.0e6f));
+            store3(vel, i, f3(0.f, 0.f, 0.f));
+        }
+    }
+    const unsigned int hits = __ballot_sync(0xffffffffu, in);
+    if ((threadIdx.x & 31) == 0 && hits) atomicAdd(count, __popc(hits));
+}
+
+// After the search of n + e slots: the in-grid particles must be exactly the L live ones
+__global__ void k_open_count_check(const int* __restrict__ cellStart, int ncells, int L, int* __restrict__ bits) {
+    if (cellStart[ncells] != L) atomicOr(bits, 1);
+}
+
+static bool open_range_active(const sphk_ctx* c) { return c->actCount >= 0 || c->rangeDev != nullptr; }
+
+static int open_alloc(sphk_ctx* c) {
+    if (c->openDev) return SPHK_OK;
+    cudaError_t e = dalloc(&c->openDev, 2);
+    if (e == cudaSuccess) e = cudaMallocHost(reinterpret_cast<void**>(&c->openPinned), sizeof(int));
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->sinkEvent, cudaEventDisableTiming);
+    if (e != cudaSuccess) {
+        cudaFree(c->openDev); c->openDev = nullptr;
+        if (c->openPinned) cudaFreeHost(c->openPinned);
+        c->openPinned = nullptr;
+        if (c->sinkEvent) cudaEventDestroy(c->sinkEvent);
+        c->sinkEvent = nullptr;
+        cudaGetLastError();
+        return e == cudaErrorMemoryAllocation ? SPHK_ERR_ALLOC : static_cast<int>(e);
+    }
+    return SPHK_OK;
+}
+
+// {d, e1, e2} in double (sphk.h): d normalised; e1 = normalize(d x y^), or normalize(d x x^) when |d . y^| > 0.9; e2 = e1 x d
+static int emitter_axes(const sphk_emitter* e, double d[3], double e1[3], double e2[3]) {
+    if (!e) return SPHK_ERR_INVALID;
+    if (!all_finite(e->origin, 3) || !all_finite(e->direction, 3) || !all_finite(&e->speed, 1) || !all_finite(&e->spacing, 1))
+        return SPHK_ERR_INVALID;
+    if (!(e->speed > 0.f) || !(e->spacing > 0.f) || e->width < 1 || e->height < 1) return SPHK_ERR_INVALID;
+    const double l = std::sqrt(double(e->direction[0]) * e->direction[0] + double(e->direction[1]) * e->direction[1] +
+                               double(e->direction[2]) * e->direction[2]);
+    if (!(l > 0.0)) return SPHK_ERR_INVALID;
+    for (int a = 0; a < 3; ++a) d[a] = e->direction[a] / l;
+    double c[3];
+    if (std::fabs(d[1]) > 0.9) { c[0] = 0.0; c[1] = d[2]; c[2] = -d[1]; }   // d x x^
+    else { c[0] = -d[2]; c[1] = 0.0; c[2] = d[0]; }                           // d x y^
+    const double lc = std::sqrt(c[0] * c[0] + c[1] * c[1] + c[2] * c[2]);
+    for (int a = 0; a < 3; ++a) e1[a] = c[a] / lc;
+    e2[0] = e1[1] * d[2] - e1[2] * d[1];
+    e2[1] = e1[2] * d[0] - e1[0] * d[2];
+    e2[2] = e1[0] * d[1] - e1[1] * d[0];
+    return SPHK_OK;
+}
+
+extern "C" int sphk_emitter_axes(const sphk_emitter* e, float axes_out[9]) {
+    if (!axes_out) return SPHK_ERR_INVALID;
+    double d[3], e1[3], e2[3];
+    const int rc = emitter_axes(e, d, e1, e2);
+    if (rc != SPHK_OK) return rc;
+    for (int a = 0; a < 3; ++a) {
+        axes_out[a] = static_cast<float>(d[a]);
+        axes_out[3 + a] = static_cast<float>(e1[a]);
+        axes_out[6 + a] = static_cast<float>(e2[a]);
+    }
+    return SPHK_OK;
+}
+
+extern "C" int sphk_emitter_advance(const sphk_emitter* e, double* carry, float dt, int max_layers, float* offsets_out,
+                                    int* scheduled_out) {
+    double d[3], e1[3], e2[3];
+    if (emitter_axes(e, d, e1, e2) != SPHK_OK || !carry || !scheduled_out || max_layers < 0 || (max_layers > 0 && !offsets_out))
+        return SPHK_ERR_INVALID;
+    if (!(dt >= 0.f) || !all_finite(&dt, 1) || !(*carry >= 0.0) || !std::isfinite(*carry)) return SPHK_ERR_INVALID;
+    const double s = e->spacing;
+    double c = *carry + static_cast<double>(e->speed) * static_cast<double>(dt);
+    if (c / s > 65536.0) return SPHK_ERR_INVALID;
+    int k = 0;
+    while (c >= s && k <= 65536) {
+        const double delta = c - s;
+        if (k < max_layers) offsets_out[k] = static_cast<float>(delta);
+        c -= s;
+        ++k;
+    }
+    *carry = c;
+    *scheduled_out = k;
+    return SPHK_OK;
+}
+
+extern "C" int sphk_emit(sphk_ctx* c, const sphk_particles* fluid, int dst_begin, const sphk_emitter* e, int n_layers,
+                         const float* offsets_host, float m0, float dt, float* history, int history_kind) {
+    if (!c || !fluid || !fluid->pos || !fluid->vel || !fluid->mass || !fluid->density || !fluid->pressure) return SPHK_ERR_INVALID;
+    double d[3], e1[3], e2[3];
+    if (emitter_axes(e, d, e1, e2) != SPHK_OK || n_layers < 0 || dst_begin < 0 || (n_layers > 0 && !offsets_host)) return SPHK_ERR_INVALID;
+    if (!(m0 > 0.f) || !all_finite(&m0, 1) || !(dt >= 0.f) || !all_finite(&dt, 1)) return SPHK_ERR_INVALID;
+    if (history_kind < 0 || history_kind > 2 || (history_kind != 0 && !history)) return SPHK_ERR_INVALID;
+    if (n_layers > 0 && !all_finite(offsets_host, n_layers)) return SPHK_ERR_INVALID;
+    if (open_range_active(c)) return SPHK_ERR_STATE;
+    const long long per = static_cast<long long>(e->width) * e->height;
+    if (dst_begin + per * n_layers > c->capF) return SPHK_ERR_CAPACITY;
+    if (n_layers == 0) return SPHK_OK;
+    float ax[9];
+    sphk_emitter_axes(e, ax);
+    const float3 o = make_float3(e->origin[0], e->origin[1], e->origin[2]);
+    const float3 dv = make_float3(ax[0], ax[1], ax[2]), a1 = make_float3(ax[3], ax[4], ax[5]), a2 = make_float3(ax[6], ax[7], ax[8]);
+    for (int k0 = 0; k0 < n_layers; k0 += SPHK_EMIT_LAYERS) {
+        const int nl = std::min(SPHK_EMIT_LAYERS, n_layers - k0);
+        EmitLayers L{};
+        for (int k = 0; k < nl; ++k) L.delta[k] = offsets_host[k0 + k];
+        const int count = static_cast<int>(per * nl);
+        k_open_emit<<<sphk_blocks(count), SPHK_BLOCK, 0, c->stream>>>(fluid->pos, fluid->vel, fluid->mass, fluid->density, fluid->pressure,
+                                                                     history, history_kind, dst_begin + static_cast<int>(per * k0),
+                                                                     e->width, e->height, nl, L, o, dv, a1, a2, e->spacing, e->speed, m0, dt);
+        c->launches++;
+    }
+    c->fluidSearched = false; c->permValid = false;     // the new slots reach the records through the next fluid search
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+extern "C" int sphk_sinks_apply(sphk_ctx* c, const sphk_particles* fluid, const float* boxes_host, int n_boxes) {
+    if (!c || !fluid || !fluid->pos || !fluid->vel || fluid->n < 0 || n_boxes < 0 || n_boxes > SPHK_MAX_SINKS) return SPHK_ERR_INVALID;
+    if (n_boxes > 0 && (!boxes_host || !all_finite(boxes_host, 6 * n_boxes))) return SPHK_ERR_INVALID;
+    for (int k = 0; k < n_boxes; ++k)
+        for (int a = 0; a < 3; ++a)
+            if (!(boxes_host[6 * k + a] < boxes_host[6 * k + 3 + a])) return SPHK_ERR_INVALID;
+    if (open_range_active(c)) return SPHK_ERR_STATE;
+    if (fluid->n > c->capF) return SPHK_ERR_CAPACITY;
+    const int rc = open_alloc(c);
+    if (rc != SPHK_OK) return rc;
+    SinkBoxes B{};
+    for (int k = 0; k < 6 * n_boxes; ++k) B.b[k] = boxes_host[k];
+    SPHK_CUDA_TRY(cudaMemsetAsync(c->openDev, 0, sizeof(int), c->stream));
+    if (fluid->n > 0) {
+        k_open_sinks_mark<<<sphk_blocks(fluid->n), SPHK_BLOCK, 0, c->stream>>>(fluid->pos, fluid->vel, fluid->n, B, n_boxes, c->openDev);
+        c->launches++;
+    }
+    SPHK_CUDA_TRY(cudaMemcpyAsync(c->openPinned, c->openDev, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+    SPHK_CUDA_TRY(cudaEventRecord(c->sinkEvent, c->stream));
+    c->sinksApplied = true;
+    c->fluidSearched = false; c->permValid = false;     // marked positions reach the records through the next fluid search
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+extern "C" int sphk_sinks_removed(sphk_ctx* c, int* removed_host) {
+    if (!c || !removed_host) return SPHK_ERR_INVALID;
+    if (!c->sinksApplied) return SPHK_ERR_STATE;
+    SPHK_CUDA_TRY(cudaEventSynchronize(c->sinkEvent));
+    *removed_host = *c->openPinned;
+    return SPHK_OK;
+}
+
+extern "C" int sphk_fluid_set_count(sphk_ctx* c, const int* cell_start_fluid, int L) {
+    if (!c || !cell_start_fluid || L < 0) return SPHK_ERR_INVALID;
+    if (open_range_active(c) || !c->fluidSearched || !c->countSettable || L > c->nF) return SPHK_ERR_STATE;
+    const int rc = open_alloc(c);
+    if (rc != SPHK_OK) return rc;
+    k_open_count_check<<<1, 1, 0, c->stream>>>(cell_start_fluid, c->ncells, L, c->openDev + 1);
+    c->launches++;
+    c->nF = L;
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+extern "C" int sphk_open_check(sphk_ctx* c, int* error_bits_host) {
+    if (!c || !error_bits_host) return SPHK_ERR_INVALID;
+    int bits = 0;
+    if (c->openDev) {
+        SPHK_CUDA_TRY(cudaMemcpyAsync(&bits, c->openDev + 1, sizeof(int), cudaMemcpyDeviceToHost, c->stream));
+        SPHK_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    }
+    *error_bits_host = bits;
     return SPHK_OK;
 }

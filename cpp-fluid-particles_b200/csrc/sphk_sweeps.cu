@@ -1101,6 +1101,7 @@ static int check_scene(const sphk_ctx* c, const sphk_scene* s) {
     if (s->fluid.n != c->nF || s->boundary.n != c->nB) return SPHK_ERR_STATE;
     if (!s->cell_start_fluid || !s->cell_start_boundary || !s->fluid.pos || !s->fluid.vel) return SPHK_ERR_INVALID;
     if (!(s->radius > 0.f)) return SPHK_ERR_INVALID;
+    c->countSettable = false;           // the first sweep after a search closes sphk_fluid_set_count's window
     return SPHK_OK;
 }
 

@@ -50,14 +50,18 @@ def device_boundary_shell(L, params, device, stream) -> torch.Tensor:
 class ParticleSet:
     """Device arrays of one SPHParticles object (SPHParticles.h:56-59)."""
 
-    def __init__(self, pos_host, device):
-        """pos_host: (n, 3) host array, or a (n, 3) float32 tensor already on `device` (device-side scenes)."""
+    def __init__(self, pos_host, device, capacity: int | None = None):
+        """pos_host: (n, 3) host array, or a (n, 3) float32 tensor already on `device` (device-side scenes).  capacity (>= n):
+        the arrays' length, of which the first n slots are live (open boundaries change n)."""
         n = pos_host.shape[0]
         self.n = n
         if isinstance(pos_host, torch.Tensor):
             self.pos = pos_host
         else:
             self.pos = torch.from_numpy(np.ascontiguousarray(pos_host, np.float32)).to(device)
+        if capacity is not None and capacity > n:
+            self.pos = torch.cat([self.pos, torch.zeros((capacity - n, 3), dtype=torch.float32, device=device)], 0).contiguous()
+        n = self.pos.shape[0]
         self.vel = torch.zeros((n, 3), dtype=torch.float32, device=device)
         self.mass = torch.zeros(n, dtype=torch.float32, device=device)
         self.density = torch.zeros(n, dtype=torch.float32, device=device)
@@ -589,10 +593,85 @@ class SphkOps:
         self.advect()
         return True
 
+    # ---- open boundaries (DESIGN.md section 2.6) --------------------------------------------------------------------------
+    open = False
+
+    def _set_live(self, n: int):
+        self.fluid.n = n
+        self._scene = None           # the cached scene carries the count
+
+    def _history(self):
+        """(history tensor, kind) of the solver for sphk_emit: DFSPH warm start (1: zero), PBD last position (2: x - dt v)"""
+        if self.solver == "dfsph":
+            return self.warm, 1
+        if self.solver == "pbd":
+            return self.pos_last, 2
+        return None, 0
+
+    def open_emit(self) -> int:
+        """sinks over the live slots, then every emitter's scheduled layers into the slots after them (as SPHSystem::openEmit);
+        returns the emitted count"""
+        n, cap = self.fluid.n, self.fluid.pos.shape[0]
+        p = self.fluid.abi()
+        if self._sinks.shape[0]:
+            check(self.L.sphk_sinks_apply(self.ctx, C.byref(p), self._sinks.ctypes.data_as(C.POINTER(C.c_float)),
+                                          C.c_int(self._sinks.shape[0])), "sphk_sinks_apply")
+        hist, kind = self._history()
+        e = 0
+        for k, em in enumerate(self._emitters):
+            per = em.width * em.height
+            fit = min((cap - n - e) // per, 65536)
+            off = (C.c_float * max(fit, 1))()
+            carry, sched = C.c_double(self.emitter_carry[k]), C.c_int(0)
+            check(self.L.sphk_emitter_advance(C.byref(em), C.byref(carry), C.c_float(self.p.dt), C.c_int(fit), off, C.byref(sched)),
+                  "sphk_emitter_advance")
+            self.emitter_carry[k] = carry.value
+            layers = min(sched.value, fit)
+            self._open_stats["refused"] += (sched.value - layers) * per
+            if layers == 0:
+                continue
+            check(self.L.sphk_emit(self.ctx, C.byref(p), C.c_int(n + e), C.byref(em), C.c_int(layers), off, C.c_float(self.p.m0),
+                                   C.c_float(self.p.dt), _ptr(hist), C.c_int(kind)), "sphk_emit")
+            e += layers * per
+            self._open_stats["emitted"] += layers * per
+        return e
+
+    def open_set_count(self, searched: int) -> int:
+        """after the search of `searched` slots: L = searched - removed, sphk_fluid_set_count(L)"""
+        removed = C.c_int(0)
+        if self._sinks.shape[0]:
+            check(self.L.sphk_sinks_removed(self.ctx, C.byref(removed)), "sphk_sinks_removed")
+        live = searched - removed.value
+        check(self.L.sphk_fluid_set_count(self.ctx, _ptr(self.cs_fluid), C.c_int(live)), "sphk_fluid_set_count")
+        self._set_live(live)
+        self._open_stats["removed"] += removed.value
+        return live
+
+    @property
+    def fluid_count(self) -> int:
+        return self.fluid.n
+
+    def open_boundary_stats(self) -> dict:
+        """cumulative {"emitted", "removed", "refused"} particle counts"""
+        return dict(self._open_stats)
+
+    def open_check(self) -> int:
+        """sticky bits of the per-step count check (sphk_open_check; 0 = fine); synchronises"""
+        bits = C.c_int(0)
+        check(self.L.sphk_open_check(self.ctx, C.byref(bits)), "sphk_open_check")
+        return int(bits.value)
+
     def step(self):                  # SPHSystem.cu:129-158 (no host sync here; callers time with CUDA events)
+        e = self.open_emit() if self.open else 0
         if self.n_bodies:            # bodies move before the fluid search, as in SPHSystem::step
             self.bodies_step()
+        if self.open:
+            self._set_live(self.fluid.n + e)
+            if self.fluid.n == 0:
+                return
         self.search_fluid()
+        if self.open and self.open_set_count(self.fluid.n) == 0:
+            return
         if self.use_list:            # (the C++ layer builds the list lazily in the first sweep; same kernel)
             self.set_use_list(True, 150 if self.solver == "pbd" else 0)
             self.build_neighbor_list()
@@ -606,10 +685,12 @@ class SphkOps:
         self.bodies_integrate()
 
     def state(self) -> dict:
+        """the live fluid particles (and every boundary particle) on the host"""
         self.synchronize()
         g = lambda t: t.detach().cpu().numpy()  # noqa: E731
-        return {"pos": g(self.fluid.pos), "vel": g(self.fluid.vel), "density": g(self.fluid.density),
-                "pressure": g(self.fluid.pressure), "mass": g(self.fluid.mass), "p2c": g(self.fluid.p2c),
+        n = self.fluid.n
+        return {"pos": g(self.fluid.pos[:n]), "vel": g(self.fluid.vel[:n]), "density": g(self.fluid.density[:n]),
+                "pressure": g(self.fluid.pressure[:n]), "mass": g(self.fluid.mass[:n]), "p2c": g(self.fluid.p2c[:n]),
                 "cell_start": g(self.cs_fluid), "posB": g(self.boundary.pos), "massB": g(self.boundary.mass),
                 "p2cB": g(self.boundary.p2c), "cell_startB": g(self.cs_boundary)}
 
@@ -631,8 +712,11 @@ class SphkSystem(SphkOps):
     reference constructor including its implicit first step (Q3)."""
 
     def __init__(self, scene, device="cuda:0", use_list: bool | None = None, list_capacity: int | None = None,
-                 step0: bool = True, bodies=None):
-        """bodies: rigid bodies (DESIGN.md sections 2.3, 2.4), a list of dicts with "points" (k, 3) body coordinates,
+                 step0: bool = True, bodies=None, max_fluid: int | None = None, emitters=None, sinks=None):
+        """emitters / sinks: open boundaries (DESIGN.md section 2.6), the same C entries in the same order as SPHSystem::step.
+        emitters: dicts {"origin", "direction", "speed", "spacing", "width", "height"} (sphk_emitter); sinks: (lo, hi) boxes; max_fluid:
+        the capacity of the fluid set (default: the initial count).  fluid_count is the live count.
+        bodies: rigid bodies (DESIGN.md sections 2.3, 2.4), a list of dicts with "points" (k, 3) body coordinates,
         "position" (3,), "orientation" (x, y, z, w) unit quaternion, "linear_velocity" (3,), "angular_velocity" (3,) in the
         world frame, and optionally "mass" (> 0: dynamic, two-way coupled; default 0: kinematic, and held -- its reaction reported --
         when another body is dynamic) and "inertia" (3,) principal
@@ -647,8 +731,21 @@ class SphkSystem(SphkOps):
             self.fluid = ParticleSet(device_fluid_block(self.L, scene.lattice, self.device, self.stream), self.device)
             self.boundary = ParticleSet(device_boundary_shell(self.L, self.p, self.device, self.stream), self.device)
         else:
-            self.fluid = ParticleSet(scene.fluid, self.device)
+            self.fluid = ParticleSet(scene.fluid, self.device, max_fluid)
             self.boundary = ParticleSet(scene.boundary, self.device)
+        if scene.fluid is None and max_fluid is not None:
+            self.fluid = ParticleSet(self.fluid.pos, self.device, max_fluid)
+        self._emitters = [capi.emitter_struct(e) for e in (emitters or [])]
+        self._sinks = capi.sink_boxes(sinks or [])
+        if len(self._emitters) > capi.MAX_EMITTERS or self._sinks.shape[0] > capi.MAX_SINKS:
+            raise ValueError("at most 16 emitters and 16 sinks")
+        for em in self._emitters:          # the library's validation (sphk_emitter_axes)
+            check(self.L.sphk_emitter_axes(C.byref(em), (C.c_float * 9)()), "sphk_emitter_axes")
+        if (self._sinks.shape[0] and not (self._sinks[:, :3] < self._sinks[:, 3:]).all()) or not np.isfinite(self._sinks).all():
+            raise ValueError("a sink needs finite lo < hi on every axis")
+        self.open = bool(self._emitters) or self._sinks.shape[0] > 0
+        self.emitter_carry = [0.0] * len(self._emitters)
+        self._open_stats = {"emitted": 0, "removed": 0, "refused": 0}
         bodies = list(bodies or [])
         self.n_bodies = len(bodies)
         if bodies:                   # static set + the bodies' particles (placed by the first boundary search)
@@ -668,14 +765,14 @@ class SphkSystem(SphkOps):
         g.cell_size[:] = [int(c) for c in self.p.cell_size]
         g.cell_length = self.p.cell_length
         self.ctx = C.c_void_p()
-        check(self.L.sphk_create(C.byref(self.ctx), C.c_int(self.fluid.n), C.c_int(self.boundary.n), C.byref(g),
+        check(self.L.sphk_create(C.byref(self.ctx), C.c_int(self.fluid.pos.shape[0]), C.c_int(self.boundary.n), C.byref(g),
                                  C.c_void_p(self.stream.cuda_stream)), "sphk_create")
         if list_capacity is not None:
             self.set_option(capi.OPT_LIST_CAPACITY, list_capacity)
         self.solver = self.p.solver
         self.use_list = True if use_list is None else bool(use_list)
         n = self.fluid.n
-        self._alloc_solver_buffers(n)
+        self._alloc_solver_buffers(self.fluid.pos.shape[0])
         self._scene = None
         self._G = (C.c_float * 3)(*[float(x) for x in self.p.gravity])
         self._space = (C.c_float * 3)(*[float(x) for x in self.p.space])
@@ -696,3 +793,7 @@ class SphkSystem(SphkOps):
         self.search_fluid()
         if step0:
             self.step()
+
+    def owned(self, t):
+        """the live slots of a per-particle tensor (the reductions run over the live count, as in the class layer)"""
+        return t[: self.fluid.n]

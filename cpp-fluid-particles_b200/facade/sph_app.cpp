@@ -66,17 +66,26 @@ static std::vector<float3> to_float3(const float* xyz, int n) {
 
 #ifdef SPH_APP_REFERENCE_ENGINE
 struct body_list {};
+struct open_list {};
 #else
 using body_list = std::vector<sphb200::KinematicBody>;
+using open_list = sphb200::OpenBoundaries;
 #endif
 
+// open: emitters and sinks with a fluid capacity of max_fluid (nullptr: a closed system of n_fluid particles)
 static sph_app* create(const float* fluid_xyz, int n_fluid, const float* boundary_xyz, int n_boundary, const sph_app_params* p,
-                       const body_list* bodies) {
+                       const body_list* bodies, const open_list* open = nullptr, int max_fluid = 0) {
     if (!fluid_xyz || !boundary_xyz || !p || n_fluid <= 0 || n_boundary <= 0) return nullptr;
+#ifdef SPH_APP_REFERENCE_ENGINE
     auto fluidParticles = std::make_shared<SPHParticles>(to_float3(fluid_xyz, n_fluid));
+    const int num = static_cast<int>(fluidParticles->size());
+#else
+    auto fluidParticles = open ? std::make_shared<SPHParticles>(to_float3(fluid_xyz, n_fluid), static_cast<unsigned int>(max_fluid))
+                               : std::make_shared<SPHParticles>(to_float3(fluid_xyz, n_fluid));
+    const int num = static_cast<int>(fluidParticles->capacity());
+#endif
     auto boundaryParticles = std::make_shared<SPHParticles>(to_float3(boundary_xyz, n_boundary));
     std::shared_ptr<BaseSolver> pSolver;
-    const int num = static_cast<int>(fluidParticles->size());
     switch (p->solver) {
     case 2:
         if (p->max_iter > 0) pSolver = std::make_shared<PBDSolver>(num, p->max_iter);
@@ -97,7 +106,11 @@ static sph_app* create(const float* fluid_xyz, int n_fluid, const float* boundar
     const float3 space = make_float3(p->space[0], p->space[1], p->space[2]), G = make_float3(p->gravity[0], p->gravity[1], p->gravity[2]);
     const int3 cells = make_int3(p->cell_size[0], p->cell_size[1], p->cell_size[2]);
 #ifndef SPH_APP_REFERENCE_ENGINE
-    if (bodies)
+    if (open)
+        app->system = std::make_shared<SPHSystem>(fluidParticles, boundaryParticles, pSolver, space, p->cell_length, p->radius, p->dt,
+                                                  p->m0, p->rho0, p->rho_boundary, p->stiff, p->visc, p->surface_tension,
+                                                  p->air_pressure, G, cells, body_list{}, *open);
+    else if (bodies)
         app->system = std::make_shared<SPHSystem>(fluidParticles, boundaryParticles, pSolver, space, p->cell_length, p->radius, p->dt,
                                                   p->m0, p->rho0, p->rho_boundary, p->stiff, p->visc, p->surface_tension,
                                                   p->air_pressure, G, cells, *bodies);
@@ -106,7 +119,7 @@ static sph_app* create(const float* fluid_xyz, int n_fluid, const float* boundar
         app->system = std::make_shared<SPHSystem>(fluidParticles, boundaryParticles, pSolver, space, p->cell_length, p->radius, p->dt,
                                                   p->m0, p->rho0, p->rho_boundary, p->stiff, p->visc, p->surface_tension,
                                                   p->air_pressure, G, cells);
-    (void)bodies;
+    (void)bodies; (void)open; (void)max_fluid;
     if (cudaDeviceSynchronize() != cudaSuccess) {
         std::fprintf(stderr, "sph_app_create: %s\n", cudaGetErrorString(cudaGetLastError()));
         delete app;
@@ -177,6 +190,49 @@ extern "C" sph_app* sph_app_create_with_dynamic_bodies(const float* fluid_xyz, i
     if (!mass_inertia) return nullptr;
     return create_with_bodies(fluid_xyz, n_fluid, boundary_xyz, n_boundary, n_bodies, body_begin, body_xyz, pose, motion,
                               mass_inertia, p);
+#endif
+}
+
+extern "C" sph_app* sph_app_create_open(const float* fluid_xyz, int n_fluid, int max_fluid, const float* boundary_xyz, int n_boundary,
+                                        int n_emitters, const sph_app_emitter* emitters, int n_sinks, const float* sinks_lo_hi,
+                                        const sph_app_params* p) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)fluid_xyz; (void)n_fluid; (void)max_fluid; (void)boundary_xyz; (void)n_boundary; (void)n_emitters; (void)emitters;
+    (void)n_sinks; (void)sinks_lo_hi; (void)p;
+    return nullptr;
+#else
+    if (max_fluid < n_fluid || n_emitters < 0 || n_sinks < 0 || (n_emitters > 0 && !emitters) || (n_sinks > 0 && !sinks_lo_hi))
+        return nullptr;
+    open_list open;
+    for (int k = 0; k < n_emitters; ++k) {
+        const sph_app_emitter& e = emitters[k];
+        sphb200::Emitter m;
+        m.origin = make_float3(e.origin[0], e.origin[1], e.origin[2]);
+        m.direction = make_float3(e.direction[0], e.direction[1], e.direction[2]);
+        m.speed = e.speed; m.spacing = e.spacing; m.width = e.width; m.height = e.height;
+        open.emitters.push_back(m);
+    }
+    for (int k = 0; k < n_sinks; ++k) {
+        const float* b = sinks_lo_hi + 6 * k;
+        open.sinks.push_back({make_float3(b[0], b[1], b[2]), make_float3(b[3], b[4], b[5])});
+    }
+    sph_app* app = create(fluid_xyz, n_fluid, boundary_xyz, n_boundary, p, nullptr, &open, max_fluid);
+    // the class layer refused them (it then builds the closed system)
+    if (app && (n_emitters > 0 || n_sinks > 0) && !app->system->openBoundariesActive()) { delete app; return nullptr; }
+    return app;
+#endif
+}
+
+extern "C" int sph_app_open_boundary_stats(sph_app* app, long long* stats3, int* check_bits) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)stats3; (void)check_bits;
+    return 1;
+#else
+    if (!app) return 1;
+    const sphb200::OpenBoundaryStats s = app->system->openBoundaryStats();
+    if (stats3) { stats3[0] = s.emitted; stats3[1] = s.removed; stats3[2] = s.refused; }
+    if (check_bits) *check_bits = app->system->openBoundaryCheck();
+    return 0;
 #endif
 }
 
@@ -330,7 +386,11 @@ static int pipe_run(sph_app* app, int slot) {
 
 extern "C" int sph_app_submit(sph_app* app, const float* pos_in, const float* vel_in, float* pos_out, float* vel_out,
                               float* density_out) {
-    if (!app || !pos_in || !vel_in || !pipe_init(app)) return 1;
+    if (!app || !pos_in || !vel_in) return 1;
+#ifndef SPH_APP_REFERENCE_ENGINE
+    if (app->system->openBoundariesActive()) return 1;      // the pipelining assumes a fixed particle count
+#endif
+    if (!pipe_init(app)) return 1;
     const size_t n = app->system->getFluids()->size();
     const int slot = static_cast<int>(app->submitted & 1ull);
     sph_batch& b = app->batch[slot];

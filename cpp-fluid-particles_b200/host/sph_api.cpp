@@ -43,6 +43,11 @@ Particles::Particles(const std::vector<float3>& p) : pos(p.size()), vel(p.size()
     CUDA_CALL(cudaMemcpy(pos.addr(), p.data(), sizeof(float3) * p.size(), cudaMemcpyHostToDevice));
 }
 
+Particles::Particles(const std::vector<float3>& p, unsigned int capacity)
+    : pos(std::max<size_t>(capacity, p.size())), vel(std::max<size_t>(capacity, p.size())), activeCount_(static_cast<int>(p.size())) {
+    CUDA_CALL(cudaMemcpy(pos.addr(), p.data(), sizeof(float3) * p.size(), cudaMemcpyHostToDevice));
+}
+
 void Particles::advect(float dt) {
     // pos += dt * vel.  Not on the engine's hot path (BasicSPHSolver::advect uses the fused sphk_advect); kept for
     // API parity.  It moves particles behind the engine's back, so the packed records are re-packed before the
@@ -506,6 +511,15 @@ SPHSystem::SPHSystem(std::shared_ptr<SPHParticles>& fluidParticles, std::shared_
     : SPHSystem(fluidParticles, boundaryParticles, solver, spaceSize, sphCellLength, sphSmoothingRadius, dt, sphM0, sphRho0,
                 sphRhoBoundary, sphStiff, sphVisc, sphSurfaceTensionIntensity, sphAirPressure, sphG, cellSize, {}) {}
 
+SPHSystem::SPHSystem(std::shared_ptr<SPHParticles>& fluidParticles, std::shared_ptr<SPHParticles>& boundaryParticles,
+                     std::shared_ptr<BaseSolver>& solver, const float3 spaceSize, const float sphCellLength,
+                     const float sphSmoothingRadius, const float dt, const float sphM0, const float sphRho0,
+                     const float sphRhoBoundary, const float sphStiff, const float sphVisc,
+                     const float sphSurfaceTensionIntensity, const float sphAirPressure, const float3 sphG,
+                     const int3 cellSize, const std::vector<sphb200::KinematicBody>& bodies)
+    : SPHSystem(fluidParticles, boundaryParticles, solver, spaceSize, sphCellLength, sphSmoothingRadius, dt, sphM0, sphRho0,
+                sphRhoBoundary, sphStiff, sphVisc, sphSurfaceTensionIntensity, sphAirPressure, sphG, cellSize, bodies, {}) {}
+
 // the caller's static boundary set followed by the bodies' particles (placed on the host here only to give the arrays a
 // value: the first boundary search places them on the device)
 static std::shared_ptr<SPHParticles> withBodies(std::shared_ptr<SPHParticles>&& boundary,
@@ -524,20 +538,38 @@ SPHSystem::SPHSystem(std::shared_ptr<SPHParticles>& fluidParticles, std::shared_
                      const float sphSmoothingRadius, const float dt, const float sphM0, const float sphRho0,
                      const float sphRhoBoundary, const float sphStiff, const float sphVisc,
                      const float sphSurfaceTensionIntensity, const float sphAirPressure, const float3 sphG,
-                     const int3 cellSize, const std::vector<sphb200::KinematicBody>& bodies)
+                     const int3 cellSize, const std::vector<sphb200::KinematicBody>& bodies,
+                     const sphb200::OpenBoundaries& open)
     // the caller's three shared_ptrs are moved from, as in the reference (SPHSystem.cu:50-51)
     : _fluids(std::move(fluidParticles)), _boundaries(withBodies(std::move(boundaryParticles), bodies)), _solver(std::move(solver)),
       cellStartFluid(cellSize.x * cellSize.y * cellSize.z + 1), cellStartBoundary(cellSize.x * cellSize.y * cellSize.z + 1),
       _spaceSize(spaceSize), _sphSmoothingRadius(sphSmoothingRadius), _sphCellLength(sphCellLength), _dt(dt),
       _sphRho0(sphRho0), _sphRhoBoundary(sphRhoBoundary), _sphStiff(sphStiff), _sphG(sphG), _sphVisc(sphVisc),
       _sphSurfaceTensionIntensity(sphSurfaceTensionIntensity), _sphAirPressure(sphAirPressure), _cellSize(cellSize) {
-    _engine = std::make_shared<sphb200::Engine>(fluidSize(), boundarySize(), cellSize, sphCellLength);
+    _engine = std::make_shared<sphb200::Engine>(static_cast<int>(_fluids->capacity()), boundarySize(), cellSize, sphCellLength);
     _fluids->bindEngine(_engine);
     _boundaries->bindEngine(_engine);
     CUDA_CALL(cudaEventCreate(&_evStart));
     CUDA_CALL(cudaEventCreate(&_evStop));
     if (const char* g = std::getenv("SPHK_STEP_GRAPH")) _graphEnabled = g[0] != '0';
     if (!_engine->ok()) return;
+    _sphM0 = sphM0;
+    if (!open.emitters.empty() || !open.sinks.empty()) {
+        if (const char* why = openRefusal(open)) {
+            printf("SPHSystem: open boundaries refused (%s); the system is closed\n", why);
+        } else {
+            for (const auto& e : open.emitters) {
+                sphk_emitter k;
+                k.origin[0] = e.origin.x; k.origin[1] = e.origin.y; k.origin[2] = e.origin.z;
+                k.direction[0] = e.direction.x; k.direction[1] = e.direction.y; k.direction[2] = e.direction.z;
+                k.speed = e.speed; k.spacing = e.spacing; k.width = e.width; k.height = e.height;
+                _emitters.push_back(k);
+            }
+            _emitterCarry.assign(_emitters.size(), 0.0);
+            for (const auto& b : open.sinks) _sinkBoxes.insert(_sinkBoxes.end(), {b.lo.x, b.lo.y, b.lo.z, b.hi.x, b.hi.y, b.hi.z});
+            _open = true;
+        }
+    }
     if (!bodies.empty()) {
         const int nStatic = boundarySize() - static_cast<int>(std::accumulate(
             bodies.begin(), bodies.end(), size_t(0), [](size_t a, const sphb200::KinematicBody& b) { return a + b.points.size(); }));
@@ -598,12 +630,94 @@ void SPHSystem::neighborSearch(const std::shared_ptr<SPHParticles>& particles, D
     if (which == 0) _engine->shadowsStale = false;
 }
 
+// With open boundaries (DESIGN.md section 2.6): sinks and emitters, the bodies, the search over n + e slots, then the live count
+// L = n + e - removed (the wait for the sinks' count overlaps the search).
 void SPHSystem::searchForStep() {
+    const int n = fluidSize();
+    const int e = _open ? openEmit(n) : 0;
     if (!_bodyMotion.empty()) {
         const sphk_particles b = _boundaries->abi();
         check(sphk_bodies_step(_engine->ctx(), &b, cellStartBoundary.addr(), _dt), "sphk_bodies_step");
     }
+    if (!_open) { neighborSearch(_fluids, cellStartFluid); return; }
+    _fluids->setActiveCount(n + e);
+    if (n + e == 0) return;
     neighborSearch(_fluids, cellStartFluid);
+    int removed = 0;
+    if (!_sinkBoxes.empty()) check(sphk_sinks_removed(_engine->ctx(), &removed), "sphk_sinks_removed");
+    const int live = n + e - removed;
+    check(sphk_fluid_set_count(_engine->ctx(), cellStartFluid.addr(), live), "sphk_fluid_set_count");
+    _fluids->setActiveCount(live);
+    _openStats.removed += removed;
+}
+
+// the sinks over the n live slots, then every emitter's scheduled layers into the slots after them
+int SPHSystem::openEmit(int n) {
+    sphk_ctx* ctx = _engine->ctx();
+    const sphk_particles f = _fluids->abi();
+    if (!_sinkBoxes.empty())
+        check(sphk_sinks_apply(ctx, &f, _sinkBoxes.data(), static_cast<int>(_sinkBoxes.size() / 6)), "sphk_sinks_apply");
+    int width = 0;
+    float* history = dynamic_cast<BasicSPHSolver*>(_solver.get())->historyArray(width);
+    const int kind = width == 1 ? 1 : width == 3 ? 2 : 0;
+    const int cap = static_cast<int>(_fluids->capacity());
+    int e = 0;
+    for (size_t k = 0; k < _emitters.size(); ++k) {
+        const sphk_emitter& em = _emitters[k];
+        const int per = em.width * em.height;
+        const int fit = std::min((cap - n - e) / per, 65536);
+        if (static_cast<int>(_layerOffsets.size()) < fit) _layerOffsets.resize(static_cast<size_t>(fit));
+        int scheduled = 0;
+        const int rc = sphk_emitter_advance(&em, &_emitterCarry[k], _dt, fit, _layerOffsets.data(), &scheduled);
+        check(rc, "sphk_emitter_advance");
+        if (rc != 0) continue;
+        const int layers = std::min(scheduled, fit);
+        _openStats.refused += static_cast<long long>(scheduled - layers) * per;
+        if (layers == 0) continue;
+        check(sphk_emit(ctx, &f, n + e, &em, layers, _layerOffsets.data(), _sphM0, _dt, kind ? history : nullptr, kind), "sphk_emit");
+        e += layers * per;
+        _openStats.emitted += static_cast<long long>(layers) * per;
+    }
+    return e;
+}
+
+// why the constructor refuses the open boundaries (nullptr: accepted)
+const char* SPHSystem::openRefusal(const sphb200::OpenBoundaries& open) const {
+    const auto* basic = dynamic_cast<const BasicSPHSolver*>(_solver.get());
+    if (!basic) return "the solver is not a BasicSPHSolver, so its history array is unknown";
+    if (basic->capacity() < static_cast<int>(_fluids->capacity())) return "the solver's buffers are smaller than the fluid's capacity";
+    if (open.emitters.size() > SPHK_MAX_EMITTERS || open.sinks.size() > SPHK_MAX_SINKS) return "more than 16 emitters or sinks";
+    const float clamp[3] = {0.99f * _spaceSize.x, 0.99f * _spaceSize.y, 0.99f * _spaceSize.z};
+    for (const auto& s : open.sinks) {
+        const float b[6] = {s.lo.x, s.lo.y, s.lo.z, s.hi.x, s.hi.y, s.hi.z};
+        for (int a = 0; a < 3; ++a)
+            if (!std::isfinite(b[a]) || !std::isfinite(b[3 + a]) || !(b[a] < b[3 + a])) return "a sink needs finite lo < hi on every axis";
+    }
+    for (const auto& e : open.emitters) {
+        sphk_emitter k;
+        k.origin[0] = e.origin.x; k.origin[1] = e.origin.y; k.origin[2] = e.origin.z;
+        k.direction[0] = e.direction.x; k.direction[1] = e.direction.y; k.direction[2] = e.direction.z;
+        k.speed = e.speed; k.spacing = e.spacing; k.width = e.width; k.height = e.height;
+        float ax[9];
+        if (sphk_emitter_axes(&k, ax) != 0) return "an emitter needs finite values, |direction| > 0, speed > 0, spacing > 0, width and height >= 1";
+        // the corners of the layer, and of the layer advanced by speed * dt, in the kernel's float operations
+        for (int c = 0; c < 8; ++c) {
+            const float ta = ((c & 1) ? 0.5f : -0.5f) * static_cast<float>(e.width - 1) * e.spacing;
+            const float tb = ((c & 2) ? 0.5f : -0.5f) * static_cast<float>(e.height - 1) * e.spacing;
+            const float delta = (c & 4) ? e.speed * _dt : 0.0f;
+            for (int a = 0; a < 3; ++a) {
+                const float x = k.origin[a] + ta * ax[3 + a] + tb * ax[6 + a] + delta * ax[a];
+                if (!(x >= 0.0f && x <= clamp[a])) return "an emitter's layer reaches outside the clamp box [0, 0.99 spaceSize]";
+            }
+        }
+    }
+    return nullptr;
+}
+
+int SPHSystem::openBoundaryCheck() const {
+    int bits = 0;
+    if (_engine->ok()) check(sphk_open_check(_engine->ctx(), &bits), "sphk_open_check");
+    return bits;
 }
 
 // the end of a step with dynamic bodies (after the solver's last reaction, inside a captured step graph)
@@ -694,16 +808,17 @@ float SPHSystem::step() {
         sphk_add_launches(ctx, _graphLaunches);
         check(sphk_synchronize(ctx), "step");
     } else {
-        const bool capture = _graphEnabled && _plainSteps >= 2 && solverIsGraphSafe();
+        const bool capture = _graphEnabled && !_open && _plainSteps >= 2 && solverIsGraphSafe();
         const long long launches0 = sphk_launch_count(ctx);
         bool captured = false;
         if (capture) captured = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
         bool ok = false;
         try {
             searchForStep();
-            _solver->step(_fluids, _boundaries, cellStartFluid, cellStartBoundary, _spaceSize, _cellSize, _sphCellLength,
-                          _sphSmoothingRadius, _dt, _sphRho0, _sphRhoBoundary, _sphStiff, _sphVisc, _sphG,
-                          _sphSurfaceTensionIntensity, _sphAirPressure);
+            if (fluidSize() > 0)        // (an open system can run empty)
+                _solver->step(_fluids, _boundaries, cellStartFluid, cellStartBoundary, _spaceSize, _cellSize, _sphCellLength,
+                              _sphSmoothingRadius, _dt, _sphRho0, _sphRhoBoundary, _sphStiff, _sphVisc, _sphG,
+                              _sphSurfaceTensionIntensity, _sphAirPressure);
             integrateBodies();
             ok = true;
         } catch (const char* s) {

@@ -81,6 +81,28 @@ struct KinematicBody {
     float mass = 0;                 // M > 0: dynamic (two-way coupled); 0: kinematic
     float3 inertia = {0, 0, 0};     // principal moments about the centre, body axes (all > 0 when mass > 0)
 };
+
+// addition: open boundaries (DESIGN.md section 2.6).  An emitter is a rectangular nozzle that adds a W x H layer of fluid
+// particles, `spacing` apart, moving at speed * normalize(direction), every time the stream has advanced by one spacing; a sink
+// is an axis-aligned box lo <= x < hi whose fluid particles are removed.  The fluid set keeps its capacity (SPHParticles'
+// capacity constructor) and its live count changes between steps; a layer that does not fit is refused (counted, not emitted).
+struct Emitter {
+    float3 origin;                  // centre of the nozzle
+    float3 direction;               // any length > 0
+    float speed;                    // > 0
+    float spacing;                  // > 0: within a layer and between layers (normally the fluid's particle spacing)
+    int width = 1, height = 1;      // particles per layer along the nozzle's two in-plane axes (sphk_emitter_axes)
+};
+struct Sink {
+    float3 lo, hi;                  // lo < hi on every axis
+};
+struct OpenBoundaries {
+    std::vector<Emitter> emitters;  // at most SPHK_MAX_EMITTERS
+    std::vector<Sink> sinks;        // at most SPHK_MAX_SINKS
+};
+struct OpenBoundaryStats {
+    long long emitted = 0, removed = 0, refused = 0;   // cumulative particle counts
+};
 }  // namespace sphb200
 
 // ---- DArray.h:21-54 ---------------------------------------------------------------------------
@@ -113,6 +135,8 @@ private:
 class Particles {
 public:
     explicit Particles(const std::vector<float3>& p);
+    // addition: capacity slots (at least p.size()), of which the first p.size() are live (size())
+    Particles(const std::vector<float3>& p, unsigned int capacity);
     Particles(const Particles&) = delete;
     Particles& operator=(const Particles&) = delete;
     virtual ~Particles() noexcept {}
@@ -142,6 +166,10 @@ class SPHParticles final : public Particles {
 public:
     explicit SPHParticles(const std::vector<float3>& p)
         : Particles(p), pressure(p.size()), density(p.size()), mass(p.size()), particle2Cell(p.size()) {}
+    // addition: `capacity` slots with size() == p.size() (a fluid set whose count changes: open boundaries)
+    SPHParticles(const std::vector<float3>& p, unsigned int capacity)
+        : Particles(p, capacity), pressure(this->capacity()), density(this->capacity()), mass(this->capacity()),
+          particle2Cell(this->capacity()) {}
     SPHParticles(const SPHParticles&) = delete;
     SPHParticles& operator=(const SPHParticles&) = delete;
     virtual ~SPHParticles() noexcept {}
@@ -222,6 +250,8 @@ public:
     void setReduceHook(ReduceHook h, long long globalCount, RangeHook owned) { reduceHook_ = std::move(h); globalCount_ = globalCount; ownedRange_ = std::move(owned); }
     // the per-particle history array that must travel with a particle when it changes rank (nullptr: none)
     virtual float* historyArray(int& width) { width = 0; return nullptr; }
+    // addition: the particle count the solver's buffers hold (its constructor's num)
+    int capacity() const { return num_; }
     virtual ~BasicSPHSolver() noexcept {}
     virtual void step(std::shared_ptr<SPHParticles>& fluids, const std::shared_ptr<SPHParticles>& boundaries,
                       const DArray<int>& cellStartFluid, const DArray<int>& cellStartBoundary, float3 spaceSize,
@@ -392,6 +422,18 @@ public:
               float dt, float sphM0, float sphRho0, float sphRhoBoundary, float sphStiff, float sphVisc,
               float sphSurfaceTensionIntensity, float sphAirPressure, float3 sphG, int3 cellSize,
               const std::vector<sphb200::KinematicBody>& bodies);
+    // addition: the same system with open boundaries (DESIGN.md section 2.6): every step() removes the fluid particles inside a
+    // sink, emits the layers the emitters' schedules ask for into the free slots of the fluid set (fluidParticles' capacity),
+    // and runs the solver on the live particles.  Such a system never captures a step graph.  Refused with a printed message,
+    // building the closed system (openBoundariesActive() false): a solver that is not a BasicSPHSolver or whose buffers hold
+    // fewer particles than the fluid's capacity, an invalid emitter or sink, more than 16 of either, and an emitter whose layer
+    // (or the layer advanced by speed * dt) reaches outside the clamp box [0, 0.99 spaceSize].  Empty vectors are the
+    // constructors above.
+    SPHSystem(std::shared_ptr<SPHParticles>& fluidParticles, std::shared_ptr<SPHParticles>& boundaryParticles,
+              std::shared_ptr<BaseSolver>& solver, float3 spaceSize, float sphCellLength, float sphSmoothingRadius,
+              float dt, float sphM0, float sphRho0, float sphRhoBoundary, float sphStiff, float sphVisc,
+              float sphSurfaceTensionIntensity, float sphAirPressure, float3 sphG, int3 cellSize,
+              const std::vector<sphb200::KinematicBody>& bodies, const sphb200::OpenBoundaries& open);
     SPHSystem(const SPHSystem&) = delete;
     SPHSystem& operator=(const SPHSystem&) = delete;
     ~SPHSystem() noexcept;
@@ -422,6 +464,11 @@ public:
     void getBodyMotion(int body, float3& linearVelocity, float3& angularVelocity) const;
     void getBodyImpulse(int body, float3& linearImpulse, float3& angularImpulse) const;
     bool bodiesDynamic() const { return _bodiesDynamic; }   // the dynamics were declared (false if the engine refused them)
+    // open boundaries: cumulative {emitted, removed, refused} particle counts, and whether the system has emitters or sinks
+    sphb200::OpenBoundaryStats openBoundaryStats() const { return _openStats; }
+    bool openBoundariesActive() const { return _open; }
+    // the sticky bits of the per-step count check (sphk_open_check; 0 = every step's in-grid count matched; synchronises)
+    int openBoundaryCheck() const;
 
 private:
     std::shared_ptr<SPHParticles> _fluids;
@@ -458,6 +505,16 @@ private:
     void searchForStep();                 // bodies (if any), then the fluid search
     void integrateBodies();               // sphk_bodies_integrate at the end of a step with dynamic bodies
     void neighborSearch(const std::shared_ptr<SPHParticles>& particles, DArray<int>& cellStart);
+    // open boundaries
+    bool _open = false;
+    float _sphM0 = 0.0f;
+    std::vector<sphk_emitter> _emitters;
+    std::vector<double> _emitterCarry;    // the schedule's carry of each emitter (sphk_emitter_advance)
+    std::vector<float> _sinkBoxes;        // {lo.xyz, hi.xyz} per sink
+    std::vector<float> _layerOffsets;     // scratch of sphk_emitter_advance
+    sphb200::OpenBoundaryStats _openStats;
+    const char* openRefusal(const sphb200::OpenBoundaries& open) const;
+    int openEmit(int n);                  // sinks and emitters before the search; returns the emitted count
 };
 
 // ---- vbo.cu:46-51 --------------------------------------------------------------------------------

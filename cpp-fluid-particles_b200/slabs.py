@@ -283,11 +283,14 @@ class SlabSystem(SphkOps):
     HISTORY = {"dfsph": 1, "wcsph": 0, "pbd": 3}      # extra floats per particle that migrate with it
 
     def __init__(self, scene, rank: int, world: int, device, capacity_factor: float = 1.6, group=None, cut_skew: int = 0,
-                 bodies=None):
+                 bodies=None, emitters=None, sinks=None):
         """cut_skew: shifts the interior cuts by that many planes off the balanced position (tests of the re-balancing).
-        Kinematic bodies (engine.SphkSystem's `bodies`) are single-GPU only: every rank would have to hold every body."""
+        Kinematic bodies (engine.SphkSystem's `bodies`) are single-GPU only: every rank would have to hold every body.  So are
+        open boundaries (engine.SphkSystem's `emitters` / `sinks`): a rank's count is set by the decomposition."""
         if bodies:
             raise ValueError("kinematic bodies are not supported on slab ranks (single-GPU engine.SphkSystem only)")
+        if emitters or sinks:
+            raise ValueError("emitters and sinks are not supported on slab ranks (single-GPU engine.SphkSystem only)")
         self.L = capi.sphk()
         self.p = scene.params
         self.rank, self.world = rank, world

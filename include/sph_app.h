@@ -111,6 +111,28 @@ int   sph_app_body_motion(sph_app* app, int body, float* motion);
 /* {Jx, Jy, Jz, Hx, Hy, Hz}: the impulse and angular impulse about the centre the fluid gave one body over the last step
  * (zero without dynamic bodies); synchronises */
 int   sph_app_body_impulse(sph_app* app, int body, float* impulse);
+/* Open boundaries (SPHSystem's constructor with sphb200::OpenBoundaries; DESIGN.md section 2.6): emitters add fluid particles and
+ * sinks remove them, so the live count (sph_app_fluid_size, and the count the download / upload calls copy) changes between
+ * steps.  An emitter is a rectangular nozzle: `width` x `height` particles `spacing` apart in the plane normal to `direction`,
+ * centred on `origin`, moving at speed * normalize(direction); one layer enters every time the stream has advanced by one
+ * spacing.  A sink is the box lo <= x < hi, sinks_lo_hi[6 k ..] = {lo.xyz, hi.xyz}.  max_fluid (>= n_fluid) is the capacity of
+ * the fluid set: a layer that does not fit is refused.  No bodies.  NULL on failure, including emitters or sinks the class layer
+ * refuses (invalid values, more than 16 of either, a layer outside the clamp box [0, 0.99 space]), and on the reference build.
+ * sph_app_submit returns 1 for such a system (its pipelining assumes a fixed count). */
+typedef struct sph_app_emitter {
+    float origin[3];
+    float direction[3];
+    float speed;
+    float spacing;
+    int   width, height;
+} sph_app_emitter;
+sph_app* sph_app_create_open(const float* fluid_xyz, int n_fluid, int max_fluid, const float* boundary_xyz, int n_boundary,
+                             int n_emitters, const sph_app_emitter* emitters, int n_sinks, const float* sinks_lo_hi,
+                             const sph_app_params* params);
+/* cumulative particle counts {emitted, removed, refused} (zeros for a closed system) and, when check_bits is not NULL, the sticky
+ * bits of the per-step count check (0 = fine; 1 = after some step the in-grid particles were not exactly the live ones, e.g. a live
+ * particle uploaded outside the grid); synchronises for the bits; 1 on the reference build */
+int   sph_app_open_boundary_stats(sph_app* app, long long* stats3, int* check_bits);
 /* Name of the engine underneath: "reference-cuda" or "b200-native". */
 const char* sph_app_engine(void);
 

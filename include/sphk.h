@@ -359,6 +359,72 @@ int sphk_bodies_get_motion(sphk_ctx* ctx, float* motion_host);
 /* {Jx, Jy, Jz, Hx, Hy, Hz} per body of the last integrated step (host float[6 * n_bodies]; J / dt is the mean force); synchronises */
 int sphk_bodies_get_impulse(sphk_ctx* ctx, float* impulse_host);
 
+/* ---- open boundaries: emitters and sinks (no reference counterpart; DESIGN.md section 2.6) ----------------------------------
+ * The fluid set keeps capF slots (sphk_create's max_fluid) of which the first n are live; n changes between steps.
+ * An emitter is a rectangular nozzle {origin o, direction d, speed u > 0, spacing s > 0, width W >= 1, height H >= 1}.  Its axes
+ * (sphk_emitter_axes) are d normalised in double, e1 = normalize(d x y^) (normalize(d x x^) when |d . y^| > 0.9) and e2 = e1 x d,
+ * all in double, rounded to float once.  A layer at offset delta is the W x H lattice
+ *     x_ab = o + ((a - (W-1)/2) s) e1 + ((b - (H-1)/2) s) e2 + delta d      (float, in that order, no contraction)
+ * with slot dst + k W H + b W + a for layer k; its particles get v = u d, mass m0, density 0, pressure 0.
+ * A sink is an axis-aligned box {lo, hi}, lo < hi per axis: a live fluid particle with lo <= x < hi on all three axes is removed.
+ *
+ * The order of a step (the class layer's SPHSystem::step, engine.SphkSystem.step):
+ *   1. sphk_sinks_apply over the n live slots: marks the particles inside a sink (position -1e6, velocity 0) and counts them;
+ *   2. sphk_emit of the scheduled layers (sphk_emitter_advance) into slots [n, n + e), history slot included;
+ *   3. the bodies' step, if any;
+ *   4. sphk_neighbor_search over n + e slots: marked particles get the out-of-grid key and sort behind every live one (stable);
+ *   5. L = n + e - removed (sphk_sinks_removed waits for the sinks' count only, so it overlaps the search), then
+ *      sphk_fluid_set_count(L): permutes, lists and sweeps cover [0, L) from here on;
+ *   6. the solver's step on L particles.
+ * Removal happens before the search, so the L live particles are exactly the set a closed system built from the survivors plus
+ * the emitted particles (in the same pre-sort order) would hold after its search.
+ * All of these entries except the two host-only ones return SPHK_ERR_STATE under an active range (slab ranks). */
+#define SPHK_MAX_EMITTERS 16
+#define SPHK_MAX_SINKS 16
+typedef struct sphk_emitter {
+    float origin[3];
+    float direction[3];   /* any length > 0: the library normalises it */
+    float speed;          /* u > 0 */
+    float spacing;        /* s > 0: lattice spacing within a layer and distance between layers */
+    int   width, height;  /* W, H >= 1 */
+} sphk_emitter;
+/* Host only (no context, no device): {d, e1, e2} as float[9], the values sphk_emit uses.  SPHK_ERR_INVALID for a NULL pointer, a
+ * non-finite value, |d| = 0, u <= 0, s <= 0, W or H < 1. */
+int sphk_emitter_axes(const sphk_emitter* e, float axes_out[9]);
+/* Host only: the emission schedule of one step, in double.  carry += u dt; while carry >= s: a layer with delta = carry - s,
+ * carry -= s.  Layers are therefore exactly s apart along the stream, and several may come in one step.  *scheduled_out = the
+ * layers due this step; the first min(scheduled, max_layers) deltas go to offsets_out (float[max_layers]); the rest are refused
+ * (the caller counts them: a partial layer is never emitted, and their carry is spent all the same).  max_layers = the whole
+ * layers that fit in the remaining capacity.  SPHK_ERR_INVALID: an invalid emitter (as sphk_emitter_axes), a NULL carry or
+ * scheduled_out, offsets_out NULL with max_layers > 0, max_layers < 0, dt < 0 or not finite, a carry < 0 or not finite, or more than
+ * 65536 layers due in one step. */
+int sphk_emitter_advance(const sphk_emitter* e, double* carry, float dt, int max_layers, float* offsets_out, int* scheduled_out);
+/* Writes n_layers layers of emitter e (offsets_host: their deltas, host float[n_layers]) into fluid slots [dst_begin,
+ * dst_begin + n_layers W H): pos, vel, mass (= m0), density and pressure (= 0), and the solver's history slot of each:
+ * history_kind 0 = none (history NULL), 1 = zero (width 1: DFSPH's warm-start stiffness), 2 = x - dt v (width 3: PBD's last
+ * position, from which PBDSolver recovers v).  The slots must then be searched (sphk_neighbor_search over dst_begin + the new
+ * particles): until then sweeps return SPHK_ERR_STATE.  SPHK_ERR_INVALID: NULL pointers, an invalid emitter, non-finite offsets,
+ * m0 <= 0, dt < 0, n_layers < 0, dst_begin < 0, history_kind outside 0..2 or history NULL with kind != 0; SPHK_ERR_CAPACITY when
+ * dst_begin + n_layers W H > max_fluid. */
+int sphk_emit(sphk_ctx* ctx, const sphk_particles* fluid, int dst_begin, const sphk_emitter* e, int n_layers,
+              const float* offsets_host, float m0, float dt, float* history, int history_kind);
+/* Marks the live particles [0, fluid->n) inside any of the n_boxes sinks (boxes_host: float[6 n_boxes] = {lo.xyz, hi.xyz}): position
+ * (-1e6, -1e6, -1e6), velocity 0; counts them (warp-aggregated integer adds: deterministic) into memory the context owns, then an
+ * event.  Must be followed by a fluid search (sweeps return SPHK_ERR_STATE until then).  SPHK_ERR_INVALID: NULL pointers, n_boxes
+ * outside 0..SPHK_MAX_SINKS, a non-finite bound or lo >= hi on some axis. */
+int sphk_sinks_apply(sphk_ctx* ctx, const sphk_particles* fluid, const float* boxes_host, int n_boxes);
+/* The count of the last sphk_sinks_apply; waits for that kernel only (not for work enqueued after it).  SPHK_ERR_STATE before the
+ * first sphk_sinks_apply. */
+int sphk_sinks_removed(sphk_ctx* ctx, int* removed_host);
+/* Truncates the searched fluid set to its first L slots (the marked particles sorted behind them): nF = L for sphk_permute, the
+ * lists and the sweeps.  Valid between a fluid search and the first sweep (SPHK_ERR_STATE otherwise, and for L > the searched
+ * count; SPHK_ERR_INVALID for L < 0 or a NULL cell_start_fluid).  Enqueues a one-thread check that cell_start_fluid[ncells] == L:
+ * a mismatch (a live particle had left the grid, or a marked one had not) sets a sticky bit read by sphk_open_check. */
+int sphk_fluid_set_count(sphk_ctx* ctx, const int* cell_start_fluid, int L);
+/* the sticky error bits of sphk_fluid_set_count's check (0 = fine; bit 0 = a count mismatch since the context was created);
+ * synchronises */
+int sphk_open_check(sphk_ctx* ctx, int* error_bits_host);
+
 /* Builds the per-step neighbour list now (sweeps otherwise build it lazily on first use). */
 int sphk_build_neighbor_list(sphk_ctx* ctx, const sphk_scene* s);
 
