@@ -10,6 +10,10 @@
 //   sph_headless [--solver sph|dfsph|pbd] [--frames N] [--box L | --box LX LY LZ] [--block NX NY NZ] [--origin X Y Z]
 //                [--dt DT] [--iters K] [--vorticity EPS] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] [--ranks N [--rank R --rendezvous DIR]]
 //                [--bullets K] [--stir OMEGA] [--float REL] [--implicit-viscosity NU] [--tap SPEED] [--drain SIDE] [--capacity N]
+//                [--cfl C [--dt-min X]]
+// --cfl C turns on CFL-adaptive time stepping (SPHSystem::setAdaptiveTimeStep, DESIGN.md section 2.8) after the constructor's step 0:
+// every frame then advances --dt of simulated time in CFL substeps (SPHSystem::advance; dt_max = --dt, dt_min = X or dt / 64) and
+// prints their count and the smallest dt of the frame; the JSON summary adds the substeps of every frame.  Single GPU only.
 // --tap SPEED adds an emitter (SPHSystem's constructor with sphb200::OpenBoundaries, DESIGN.md section 2.6): an 8 x 8 nozzle at the
 // fluid spacing, centred above the block at 0.85 of the box height, pointing down, SPEED fast.  --drain SIDE adds a sink on the
 // floor: the box [0, SIDE] x [0, 0.05 L] x [0, SIDE] in the (0, 0, 0) corner of the clamp box.  --capacity N is the fluid set's
@@ -86,6 +90,8 @@ struct Options {
     float tap = 0.0f;                         // --tap SPEED: an emitter above the block (0: none)
     float drain = 0.0f;                       // --drain SIDE: a floor sink (0: none)
     long long capacity = 0;                   // --capacity N: fluid capacity of an open system (0: twice the initial count)
+    float cfl = 0.0f;                         // --cfl C: CFL-adaptive substeps, --dt of simulated time per frame (0: off)
+    float dtMin = 0.0f;                       // --dt-min X: their smallest dt (0: dt / 64)
     int bullets = 0;                          // test aid: this many top-layer particles start at ~3 cell planes per step
     int ranks = 1, rank = -1;                 // --ranks N: SlabSPHSystem on N GPUs; --rank R: this process is rank R
     std::string rendezvous;
@@ -110,6 +116,8 @@ bool parse(int argc, char** argv, Options& o) {
         else if (a == "--tap" && need(i, 1)) o.tap = static_cast<float>(std::atof(argv[++i]));
         else if (a == "--drain" && need(i, 1)) o.drain = static_cast<float>(std::atof(argv[++i]));
         else if (a == "--capacity" && need(i, 1)) o.capacity = std::atoll(argv[++i]);
+        else if (a == "--cfl" && need(i, 1)) o.cfl = static_cast<float>(std::atof(argv[++i]));
+        else if (a == "--dt-min" && need(i, 1)) o.dtMin = static_cast<float>(std::atof(argv[++i]));
         else if (a == "--ranks" && need(i, 1)) o.ranks = std::atoi(argv[++i]);
         else if (a == "--rank" && need(i, 1)) o.rank = std::atoi(argv[++i]);
         else if (a == "--rendezvous" && need(i, 1)) o.rendezvous = argv[++i];
@@ -153,6 +161,14 @@ bool parse(int argc, char** argv, Options& o) {
     }
     if ((o.tap > 0.0f || o.drain > 0.0f) && o.ranks > 1) {
         std::fprintf(stderr, "sph_headless: --tap and --drain run on one GPU only (open boundaries are not supported with --ranks)\n");
+        return false;
+    }
+    if (!(o.cfl >= 0.0f) || !std::isfinite(o.cfl) || !(o.dtMin >= 0.0f) || !std::isfinite(o.dtMin)) {
+        std::fprintf(stderr, "sph_headless: --cfl C and --dt-min X need finite values > 0\n");
+        return false;
+    }
+    if (o.cfl > 0.0f && o.ranks > 1) {
+        std::fprintf(stderr, "sph_headless: --cfl runs on one GPU only (adaptive time stepping is not supported with --ranks)\n");
         return false;
     }
     return o.frames >= 0 && o.vorticity >= 0.0f && o.block[0] > 0 && o.block[1] > 0 && o.block[2] > 0 &&
@@ -316,7 +332,7 @@ int main(int argc, char** argv) {
     if (!parse(argc, argv, o)) {
         std::fprintf(stderr, "usage: sph_headless [--solver sph|dfsph|pbd] [--frames N] [--box L | LX LY LZ] [--block NX NY NZ] "
                              "[--origin X Y Z] [--dt DT] [--iters K] [--vorticity EPS] [--implicit-viscosity NU] [--stir OMEGA | --float REL] "
-                             "[--tap SPEED] [--drain SIDE] [--capacity N] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] "
+                             "[--tap SPEED] [--drain SIDE] [--capacity N] [--cfl C [--dt-min X]] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] "
                              "[--ranks N [--rank R --rendezvous DIR]]\n");
         return 2;
     }
@@ -458,20 +474,38 @@ int main(int argc, char** argv) {
 
     if (o.vorticity > 0.0f) basicSolver->setVorticityConfinement(o.vorticity);
     if (o.implicitNu > 0.0f) basicSolver->setImplicitViscosity(o.implicitNu, o.implicitNu);
+    if (o.cfl > 0.0f && !pSystem->setAdaptiveTimeStep(o.cfl, o.dtMin)) {
+        std::fprintf(stderr, "sph_headless: --cfl %g --dt-min %g was refused\n", o.cfl, o.dtMin);
+        return 4;
+    }
 
     if (o.bullets > 0) {
         const int hit = slab ? shoot(o, sphSpacing, dt, pSlab->getFluids(), static_cast<size_t>(pSlab->ownedBegin()), static_cast<size_t>(pSlab->size()))
                              : shoot(o, sphSpacing, dt, pSystem->getFluids(), 0, pSystem->getFluids()->size());
         if (hit < 0 || (!slab && hit != o.bullets)) { std::fprintf(stderr, "sph_headless: --bullets found %d of %d particles\n", hit, o.bullets); return 5; }
+        if (!slab) pSystem->refreshSpeedBound();   // the shot particles set the first adaptive dt
     }
 
     // ---- oneStep(), main.cpp:300-306 ----
     int frameId = 0, straysRouted = 0;
     float totalTime = 0.0f, worst = 0.0f;
+    std::string substepsJson;
     for (; frameId < o.frames;) {
         ++frameId;
         float milliseconds = 0.0f;
-        try {
+        if (o.cfl > 0.0f) {                              // one frame = dt of simulated time in CFL substeps
+            cudaEvent_t e0, e1;
+            cudaEventCreate(&e0); cudaEventCreate(&e1);
+            cudaEventRecord(e0, pSystem->engine()->stream());
+            const int k = pSystem->advance(dt);
+            cudaEventRecord(e1, pSystem->engine()->stream());
+            cudaEventSynchronize(e1);
+            cudaEventElapsedTime(&milliseconds, e0, e1);
+            cudaEventDestroy(e0); cudaEventDestroy(e1);
+            substepsJson += (substepsJson.empty() ? "" : ", ") + std::to_string(k);
+            if (!o.quiet) std::printf("Frame %d - %d substeps, min dt %g s\n", frameId, k, pSystem->adaptiveStats().frameMinDt);
+            if (k == 0) return 4;
+        } else try {
             milliseconds = slab ? pSlab->step() : pSystem->step();
         } catch (const std::exception& e) {             // SlabSPHSystem::step: a broken decomposition contract ends the rank
             std::fprintf(stderr, "sph_headless: %s\n", e.what());
@@ -523,9 +557,16 @@ int main(int argc, char** argv) {
         return 0;
     }
     std::string openJson;
+    if (o.cfl > 0.0f) {
+        const sphb200::AdaptiveStats st = pSystem->adaptiveStats();
+        char buf[160];
+        std::snprintf(buf, sizeof buf, ", \"simulated_time\": %.17g, \"dt_min_clamps\": %lld, \"nonfinite_steps\": %lld, \"last_dt\": %.9g",
+                      pSystem->simulatedTime(), st.minClamps, st.nonFiniteSteps, pSystem->lastTimeStep());
+        openJson += ", \"frame_substeps\": [" + substepsJson + "]" + buf;
+    }
     if (open) {
         const sphb200::OpenBoundaryStats st = pSystem->openBoundaryStats();
-        openJson = ", \"fluid_count\": " + std::to_string(pSystem->fluidSize()) + ", \"emitted\": " + std::to_string(st.emitted) +
+        openJson += ", \"fluid_count\": " + std::to_string(pSystem->fluidSize()) + ", \"emitted\": " + std::to_string(st.emitted) +
                    ", \"removed\": " + std::to_string(st.removed) + ", \"refused\": " + std::to_string(st.refused) +
                    ", \"open_check\": " + std::to_string(pSystem->openBoundaryCheck());
     }

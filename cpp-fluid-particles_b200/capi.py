@@ -36,7 +36,7 @@ SPHK_FUNCTIONS = [
     "sphk_implicit_viscosity_work_floats", "sphk_implicit_viscosity", "sphk_implicit_viscosity_stats", "sphk_visc_implicit_setup",
     "sphk_visc_implicit_matvec",
     "sphk_emitter_axes", "sphk_emitter_advance", "sphk_emit", "sphk_sinks_apply", "sphk_sinks_removed", "sphk_fluid_set_count",
-    "sphk_open_check",
+    "sphk_open_check", "sphk_time_step", "sphk_step_speed", "sphk_step_speed_result",
 ]
 SPH_APP_FUNCTIONS = [
     "sph_app_create", "sph_app_destroy", "sph_app_step", "sph_app_fluid_size", "sph_app_boundary_size",
@@ -44,11 +44,13 @@ SPH_APP_FUNCTIONS = [
     "sph_app_submit", "sph_app_wait", "sph_app_dfsph_iterations", "sph_app_set_option", "sph_app_set_vorticity",
     "sph_app_create_with_bodies", "sph_app_set_body_motion", "sph_app_body_pose", "sph_app_step_graph_active",
     "sph_app_create_with_dynamic_bodies", "sph_app_body_motion", "sph_app_body_impulse", "sph_app_set_implicit_viscosity",
-    "sph_app_viscosity_stats", "sph_app_create_open", "sph_app_open_boundary_stats",
+    "sph_app_viscosity_stats", "sph_app_create_open", "sph_app_open_boundary_stats", "sph_app_set_adaptive_dt", "sph_app_advance",
+    "sph_app_adaptive_stats",
 ]
 
 OPT_NEIGHBOR_LIST, OPT_LIST_CAPACITY, OPT_LIST_SKIN, OPT_SIMPLE_LIST_BUILD, OPT_TILE, OPT_STAGED_LIST_BUILD, OPT_PATCH = 1, 2, 5, 6, 9, 10, 11
 MAX_EMITTERS, MAX_SINKS = 16, 16   # SPHK_MAX_EMITTERS, SPHK_MAX_SINKS
+DT_MIN_CLAMP, DT_NONFINITE, DT_FRAME_END = 1, 2, 4   # SPHK_DT_* flags of sphk_time_step
 # tile-list geometry of csrc/sphk_internal.cuh (SPHK_BLOCK, SPHK_TILE_WINS, SPHK_TILE_CAP): sphk_get_tile_lists copies
 # TILE_WINDOWS windows per tile of TILE_PARTICLES particles; a tile whose windows exceed TILE_CAP records walks the cells
 TILE_PARTICLES, TILE_WINDOWS, TILE_CAP = 128, 18, 1535
@@ -79,6 +81,11 @@ def emitter_struct(e: dict) -> SphkEmitter:
 def sink_boxes(sinks) -> np.ndarray:
     """[(lo, hi), ...] as float32 {lo.xyz, hi.xyz} rows."""
     return np.ascontiguousarray([[*lo, *hi] for lo, hi in sinks], np.float32).reshape(-1, 6)
+
+
+class SphkTimeStepRule(C.Structure):
+    """sphk_time_step_rule (include/sphk.h)."""
+    _fields_ = [("cfl", C.c_double), ("dt_min", C.c_double), ("dt_max", C.c_double), ("radius", C.c_double), ("gravity", C.c_double)]
 
 
 class SphkGrid(C.Structure):
@@ -315,6 +322,27 @@ class SphApp:
         w = np.ascontiguousarray(angular_velocity, np.float32)
         if self.L.sph_app_set_body_motion(self.h, C.c_int(body), v.ctypes.data_as(C.c_void_p), w.ctypes.data_as(C.c_void_p)):
             raise RuntimeError("sph_app_set_body_motion failed (reference engine, bad index or non-finite motion)")
+
+    def set_adaptive_dt(self, cfl: float, dt_min: float = 0.0, dt_max: float = 0.0):
+        """CFL-adaptive time stepping from the next step on (cfl = 0: off).  Not on the reference engine."""
+        if self.L.sph_app_set_adaptive_dt(self.h, C.c_float(cfl), C.c_float(dt_min), C.c_float(dt_max)):
+            raise RuntimeError("sph_app_set_adaptive_dt failed (reference engine or invalid values)")
+
+    def advance(self, frame_seconds: float):
+        """CFL substeps until frame_seconds of simulated time have passed: (substeps, smallest dt)."""
+        k, m = C.c_int(0), C.c_float(0.0)
+        if self.L.sph_app_advance(self.h, C.c_double(frame_seconds), C.byref(k), C.byref(m)):
+            raise RuntimeError("sph_app_advance failed (not adaptive, invalid frame or reference engine)")
+        self.nF = self.fluid_count
+        return int(k.value), float(m.value)
+
+    def adaptive_stats(self) -> dict:
+        """{"speed", "last_dt", "frame_min_dt", "source", "min_clamps", "nonfinite_steps", "simulated_time"}"""
+        f, src, cnt, t = (C.c_float * 3)(), C.c_int(0), (C.c_longlong * 2)(), C.c_double(0.0)
+        if self.L.sph_app_adaptive_stats(self.h, f, C.byref(src), cnt, C.byref(t)):
+            raise RuntimeError("sph_app_adaptive_stats failed (reference engine)")
+        return {"speed": float(f[0]), "last_dt": float(f[1]), "frame_min_dt": float(f[2]), "source": int(src.value),
+                "min_clamps": int(cnt[0]), "nonfinite_steps": int(cnt[1]), "simulated_time": float(t.value)}
 
     def step_graph_active(self) -> bool:
         """True when the next step replays a captured step graph (this repository's engine only)."""

@@ -68,6 +68,7 @@ struct BodyState {
     int* snapDecl = nullptr;         // device [capB]: pre-sort snapshot of decl
     int* begin = nullptr;            // device [nBodies + 1]: body_begin of sphk_bodies_init (declaration slots)
     float box[6 * SPHK_MAX_BODIES] = {};   // host: body-frame bounding box of each body's r_k, {lo.xyz, hi.xyz}
+    float rmax[SPHK_MAX_BODIES] = {};      // host: max_k |r_k| of each body (the speed bound of sphk_step_speed)
     bool stepped = false;            // sphk_bodies_step has run
     // two-way coupling (sphk_bodies_set_dynamics; DESIGN.md section 2.4)
     float* dyn = nullptr;            // device [SPHK_DYN * nBodies]: M, I.xyz, box lo.xyz, box hi.xyz, clamp box hi.xyz
@@ -135,6 +136,10 @@ struct sphk_ctx {
     cudaEvent_t sinkEvent = nullptr; // recorded after that copy
     bool sinksApplied = false;
     mutable bool countSettable = false;   // a fluid search ran and no sweep since (sphk_fluid_set_count is valid)
+    // speed bound of adaptive time stepping (sphk_step_speed; allocated on first use)
+    unsigned int* speedDev = nullptr;     // device [3]: {fluid max |v|^2, body max bound (float bits), non-finite count}
+    unsigned int* speedPinned = nullptr;  // pinned [3]: their copy
+    cudaEvent_t speedEvent = nullptr;     // recorded after that copy
 };
 
 struct DevScene {

@@ -14,6 +14,7 @@
 //                        fill + countingInCell_CUDA + exclusive_scan (SPHSystem.cu:123-125) exactly.
 // HBM-bound; algorithmic bytes per particle are listed in DESIGN.md.
 #include <cub/device/device_radix_sort.cuh>
+#include <algorithm>
 #include <cstdio>
 #include <cmath>
 #include <cstdlib>
@@ -247,6 +248,9 @@ extern "C" void sphk_destroy(sphk_ctx* c) {
     cudaFree(c->openDev);
     if (c->openPinned) cudaFreeHost(c->openPinned);
     if (c->sinkEvent) cudaEventDestroy(c->sinkEvent);
+    cudaFree(c->speedDev);
+    if (c->speedPinned) cudaFreeHost(c->speedPinned);
+    if (c->speedEvent) cudaEventDestroy(c->speedEvent);
     sphk_bodies_release(c->bodies);
     delete c;
 }
@@ -878,6 +882,12 @@ extern "C" int sphk_bodies_init(sphk_ctx* c, const sphk_particles* boundary, int
                 if (k == body_begin[b] || r < box[a]) box[a] = r;
                 if (k == body_begin[b] || r > box[3 + a]) box[3 + a] = r;
             }
+        double r2 = 0.0;
+        for (int k = body_begin[b]; k < body_begin[b + 1]; ++k) {
+            const float* r = local_xyz + 3 * static_cast<size_t>(k - n_static);
+            r2 = std::fmax(r2, double(r[0]) * r[0] + double(r[1]) * r[1] + double(r[2]) * r[2]);
+        }
+        B->rmax[b] = static_cast<float>(std::sqrt(r2));
     }
     std::vector<int> decl(static_cast<size_t>(n));
     for (int k = 0; k < n; ++k) decl[k] = k;
@@ -1243,5 +1253,137 @@ extern "C" int sphk_open_check(sphk_ctx* c, int* error_bits_host) {
         SPHK_CUDA_TRY(cudaStreamSynchronize(c->stream));
     }
     *error_bits_host = bits;
+    return SPHK_OK;
+}
+
+// ---- CFL-adaptive time stepping (no reference counterpart; DESIGN.md section 2.8) ---------------------------------------------
+// The rule lives on the host (sphk_time_step); the device only measures the speed bound the rule starts from.
+
+struct BodyRadii { float r[SPHK_MAX_BODIES]; };
+
+__device__ __forceinline__ bool finite_bits(float x) { return (__float_as_uint(x) & 0x7f800000u) != 0x7f800000u; }
+
+// out[0] = max |v|^2 over the finite fluid velocities, out[1] = max |V| + |Omega| r_max over the finite body motions (block 0),
+// out[2] += the particles and bodies left out.  The maxima are non-negative floats, so their bits order as unsigned integers: one
+// atomicMax per block gives the same bits whatever order the blocks run in.  Every lane of a block reaches every shuffle and ballot.
+__global__ void __launch_bounds__(SPHK_BLOCK)
+k_step_speed(const float* __restrict__ vel, int n, const float* __restrict__ motion, int nBodies, BodyRadii R,
+             unsigned int* __restrict__ out) {
+    __shared__ unsigned int warpMax[SPHK_BLOCK / 32];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    unsigned int m = 0u;
+    for (int i = blockIdx.x * SPHK_BLOCK + threadIdx.x; i - static_cast<int>(threadIdx.x) < n; i += gridDim.x * SPHK_BLOCK) {
+        bool bad = false;
+        if (i < n) {
+            const float3 v = load3(vel, i);
+            bad = !(finite_bits(v.x) && finite_bits(v.y) && finite_bits(v.z));
+            if (!bad) m = max(m, __float_as_uint(__fadd_rn(__fadd_rn(__fmul_rn(v.x, v.x), __fmul_rn(v.y, v.y)), __fmul_rn(v.z, v.z))));
+        }
+        const unsigned int hits = __ballot_sync(0xffffffffu, bad);
+        if (lane == 0 && hits) atomicAdd(out + 2, static_cast<unsigned int>(__popc(hits)));
+    }
+    for (int o = 16; o > 0; o >>= 1) m = max(m, __shfl_xor_sync(0xffffffffu, m, o));
+    if (lane == 0) warpMax[warp] = m;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int w = 1; w < SPHK_BLOCK / 32; ++w) m = max(m, warpMax[w]);
+        if (m) atomicMax(out, m);
+    }
+    if (blockIdx.x == 0 && threadIdx.x < nBodies) {
+        const float* M = motion + 6 * threadIdx.x;
+        bool ok = true;
+        for (int a = 0; a < 6; ++a) ok = ok && finite_bits(M[a]);
+        if (!ok) {
+            atomicAdd(out + 2, 1u);
+        } else {
+            const float v = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(M[0], M[0]), __fmul_rn(M[1], M[1])), __fmul_rn(M[2], M[2])));
+            const float w = __fsqrt_rn(__fadd_rn(__fadd_rn(__fmul_rn(M[3], M[3]), __fmul_rn(M[4], M[4])), __fmul_rn(M[5], M[5])));
+            const float b = __fadd_rn(v, __fmul_rn(w, R.r[threadIdx.x]));
+            if (finite_bits(b)) atomicMax(out + 1, __float_as_uint(b));
+            else atomicAdd(out + 2, 1u);
+        }
+    }
+}
+
+static bool rule_valid(const sphk_time_step_rule* r) {
+    const double f[5] = {r->cfl, r->dt_min, r->dt_max, r->radius, r->gravity};
+    for (double x : f)
+        if (!std::isfinite(x)) return false;
+    return r->cfl > 0.0 && r->dt_min > 0.0 && r->dt_min <= r->dt_max && r->radius > 0.0 && r->gravity >= 0.0;
+}
+
+extern "C" int sphk_time_step(const sphk_time_step_rule* r, double v_max, double dt_prev, double remaining, float* dt_out,
+                              int* flags_out) {
+    if (!r || !dt_out || !flags_out || !rule_valid(r)) return SPHK_ERR_INVALID;
+    if (v_max < 0.0 || !(dt_prev >= 0.0) || !std::isfinite(dt_prev) || !std::isfinite(remaining)) return SPHK_ERR_INVALID;
+    int flags = 0;
+    double dt;
+    if (!std::isfinite(v_max)) {                  // NaN or +inf
+        dt = r->dt_min;
+        flags |= SPHK_DT_NONFINITE;
+    } else {
+        const double vb = v_max + r->gravity * dt_prev;
+        dt = vb > 0.0 ? r->cfl * r->radius / vb : r->dt_max;
+        if (dt > r->dt_max) dt = r->dt_max;
+        if (dt < r->dt_min) { dt = r->dt_min; flags |= SPHK_DT_MIN_CLAMP; }
+    }
+    if (remaining > 0.0) {
+        if (remaining <= dt) { dt = remaining; flags |= SPHK_DT_FRAME_END; }
+        else if (remaining < 2.0 * dt) dt = 0.5 * remaining;
+    }
+    *dt_out = static_cast<float>(dt);
+    *flags_out = flags;
+    return SPHK_OK;
+}
+
+static int speed_alloc(sphk_ctx* c) {
+    if (c->speedDev) return SPHK_OK;
+    cudaError_t e = dalloc(&c->speedDev, 3);
+    if (e == cudaSuccess) e = cudaMallocHost(reinterpret_cast<void**>(&c->speedPinned), 3 * sizeof(unsigned int));
+    if (e == cudaSuccess) e = cudaEventCreateWithFlags(&c->speedEvent, cudaEventDisableTiming);
+    if (e != cudaSuccess) {
+        cudaFree(c->speedDev); c->speedDev = nullptr;
+        if (c->speedPinned) cudaFreeHost(c->speedPinned);
+        c->speedPinned = nullptr;
+        if (c->speedEvent) cudaEventDestroy(c->speedEvent);
+        c->speedEvent = nullptr;
+        cudaGetLastError();
+        return e == cudaErrorMemoryAllocation ? SPHK_ERR_ALLOC : static_cast<int>(e);
+    }
+    return SPHK_OK;
+}
+
+extern "C" int sphk_step_speed(sphk_ctx* c, const sphk_particles* fluid, int with_bodies) {
+    if (!c || !fluid || !fluid->vel || fluid->n < 0 || fluid->n > c->capF) return SPHK_ERR_INVALID;
+    if (c->actCount >= 0 || c->rangeDev) return SPHK_ERR_STATE;
+    if (with_bodies && !c->bodies) return SPHK_ERR_STATE;
+    const int rc = speed_alloc(c);
+    if (rc != SPHK_OK) return rc;
+    const int nBodies = with_bodies ? c->bodies->nBodies : 0;
+    BodyRadii R{};
+    for (int b = 0; b < nBodies; ++b) R.r[b] = c->bodies->rmax[b];
+    SPHK_CUDA_TRY(cudaMemsetAsync(c->speedDev, 0, 3 * sizeof(unsigned int), c->stream));
+    if (fluid->n > 0 || nBodies > 0) {
+        const int blocks = std::max(1, std::min(sphk_blocks(fluid->n), 8 * std::max(c->numSMs, 1)));
+        k_step_speed<<<blocks, SPHK_BLOCK, 0, c->stream>>>(fluid->vel, fluid->n, nBodies ? c->bodies->motion : nullptr, nBodies, R,
+                                                           c->speedDev);
+        c->launches++;
+    }
+    SPHK_CUDA_TRY(cudaMemcpyAsync(c->speedPinned, c->speedDev, 3 * sizeof(unsigned int), cudaMemcpyDeviceToHost, c->stream));
+    SPHK_CUDA_TRY(cudaEventRecord(c->speedEvent, c->stream));
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+extern "C" int sphk_step_speed_result(sphk_ctx* c, float* v_max_host, int* nonfinite_host) {
+    if (!c || !v_max_host || !nonfinite_host) return SPHK_ERR_INVALID;
+    if (!c->speedEvent) return SPHK_ERR_STATE;
+    SPHK_CUDA_TRY(cudaEventSynchronize(c->speedEvent));
+    float v2, b;
+    std::memcpy(&v2, c->speedPinned, sizeof(float));
+    std::memcpy(&b, c->speedPinned + 1, sizeof(float));
+    v_max_host[0] = std::sqrt(v2);
+    v_max_host[1] = b;
+    *nonfinite_host = static_cast<int>(c->speedPinned[2]);
     return SPHK_OK;
 }

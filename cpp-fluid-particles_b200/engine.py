@@ -87,6 +87,12 @@ class SphkOps:
     implicit_nu_boundary = 0.0
     implicit_tol = 1e-4
     implicit_max_iter = 20
+    _step_dt = None                  # the dt of the step in flight (None: the scene's dt); CFL-adaptive systems set it per step
+    pbd_last_dt = None               # PBD: the dt of the last predict (the interval the next projection acts on)
+
+    @property
+    def dt(self) -> float:
+        return self.p.dt if self._step_dt is None else self._step_dt
 
     # ---- multi-GPU hooks ---------------------------------------------------------------------------------
     def sync_vel(self):
@@ -158,7 +164,7 @@ class SphkOps:
 
     def bodies_step(self):
         p = self.boundary.abi()
-        check(self.L.sphk_bodies_step(self.ctx, C.byref(p), _ptr(self.cs_boundary), C.c_float(self.p.dt)), "sphk_bodies_step")
+        check(self.L.sphk_bodies_step(self.ctx, C.byref(p), _ptr(self.cs_boundary), C.c_float(self.dt)), "sphk_bodies_step")
 
     def set_body_motion(self, body: int, linear_velocity, angular_velocity):
         """New motion of one body from the next step on (an asynchronous copy, like SPHSystem::setBodyMotion); the other
@@ -167,6 +173,8 @@ class SphkOps:
         check(self.L.sphk_bodies_set_body_motion(self.ctx, C.c_int(body), m.ctypes.data_as(C.POINTER(C.c_float))),
               "sphk_bodies_set_body_motion")
         self.body_motion[body] = m
+        if self.adaptive:            # the next step's dt must see the new motion, as SPHSystem::setBodyMotion
+            self.measure_speed()
 
     # ---- two-way coupled bodies (DESIGN.md section 2.4) -----------------------------------------------------------------
     bodies_dynamic = False
@@ -178,7 +186,7 @@ class SphkOps:
 
     def bodies_integrate(self):
         if self.bodies_dynamic:
-            check(self.L.sphk_bodies_integrate(self.ctx, C.c_float(self.p.dt), self._G), "sphk_bodies_integrate")
+            check(self.L.sphk_bodies_integrate(self.ctx, C.c_float(self.dt), self._G), "sphk_bodies_integrate")
 
     def current_body_motion(self) -> np.ndarray:
         """(n_bodies, 6) motions {V, Omega} on the device (the integrated ones for dynamic bodies; the attribute body_motion
@@ -276,18 +284,18 @@ class SphkOps:
 
     # ---- one entry per reference launch site --------------------------------------------------------
     def gravity(self):
-        check(self.L.sphk_gravity(self.ctx, self._s(), C.c_float(self.p.dt), self._G), "sphk_gravity")
+        check(self.L.sphk_gravity(self.ctx, self._s(), C.c_float(self.dt), self._G), "sphk_gravity")
 
     def viscosity(self):
         check(self.L.sphk_viscosity(self.ctx, self._s(), _ptr(self.buffer3), C.c_float(self.p.rho0),
-                                    C.c_float(self.p.visc), C.c_float(self.p.dt)), "sphk_viscosity")
+                                    C.c_float(self.p.visc), C.c_float(self.dt)), "sphk_viscosity")
 
     def color_grad(self):
         check(self.L.sphk_color_grad(self.ctx, self._s(), _ptr(self.buffer3), C.c_float(self.p.rho0),
                                      C.c_float(self.p.rho_boundary)), "sphk_color_grad")
 
     def surface(self):
-        check(self.L.sphk_surface(self.ctx, self._s(), _ptr(self.buffer3), C.c_float(self.p.dt), C.c_float(self.p.rho0),
+        check(self.L.sphk_surface(self.ctx, self._s(), _ptr(self.buffer3), C.c_float(self.dt), C.c_float(self.p.rho0),
                                   C.c_float(self.p.surface_tension), C.c_float(self.p.air_pressure)), "sphk_surface")
 
     def density(self):
@@ -306,12 +314,12 @@ class SphkOps:
         check(self.L.sphk_fused_dfsph_density_alpha_div_error(self.ctx, self._s(), _ptr(self.alpha),
                                                               _ptr(self.color_grad_buf) if with_color_grad else None,
                                                               C.c_float(self.p.rho0), C.c_float(self.p.rho_boundary), _ptr(self.error),
-                                                              _ptr(self.kappa), C.c_float(self.p.dt)),
+                                                              _ptr(self.kappa), C.c_float(self.dt)),
               "sphk_fused_dfsph_density_alpha_div_error")
 
     def fused_viscosity_surface(self):
         check(self.L.sphk_fused_viscosity_surface(self.ctx, self._s(), _ptr(self.buffer3), _ptr(self.color_grad_buf),
-                                                  C.c_float(self.p.rho0), C.c_float(self.p.visc), C.c_float(self.p.dt),
+                                                  C.c_float(self.p.rho0), C.c_float(self.p.visc), C.c_float(self.dt),
                                                   C.c_float(self.p.surface_tension), C.c_float(self.p.air_pressure)),
               "sphk_fused_viscosity_surface")
 
@@ -328,12 +336,12 @@ class SphkOps:
 
     def vorticity_confinement(self, eps=None):
         check(self.L.sphk_vorticity_confinement(self.ctx, self._s(), *self._vort_buffers(),
-                                                C.c_float(self.vorticity_eps if eps is None else eps), C.c_float(self.p.dt),
+                                                C.c_float(self.vorticity_eps if eps is None else eps), C.c_float(self.dt),
                                                 C.c_float(self.p.rho0)), "sphk_vorticity_confinement")
 
     def fused_viscosity_surface_vorticity(self):
         check(self.L.sphk_fused_viscosity_surface_vorticity(self.ctx, self._s(), _ptr(self.buffer3), _ptr(self.color_grad_buf),
-                                                            C.c_float(self.p.rho0), C.c_float(self.p.visc), C.c_float(self.p.dt),
+                                                            C.c_float(self.p.rho0), C.c_float(self.p.visc), C.c_float(self.dt),
                                                             C.c_float(self.p.surface_tension), C.c_float(self.p.air_pressure),
                                                             *self._vort_buffers()), "sphk_fused_viscosity_surface_vorticity")
 
@@ -354,7 +362,7 @@ class SphkOps:
         """The implicit viscosity solve with the attributes' settings (or the arguments)."""
         a = lambda x, d: d if x is None else x  # noqa: E731
         check(self.L.sphk_implicit_viscosity(self.ctx, self._s(), self._visc_work(), C.c_float(a(nu, self.implicit_nu)),
-                                             C.c_float(a(nu_boundary, self.implicit_nu_boundary)), C.c_float(self.p.dt),
+                                             C.c_float(a(nu_boundary, self.implicit_nu_boundary)), C.c_float(self.dt),
                                              C.c_float(self.p.rho0), C.c_float(self.p.rho_boundary),
                                              C.c_float(a(tol, self.implicit_tol)), C.c_int(int(a(max_iter, self.implicit_max_iter)))),
               "sphk_implicit_viscosity")
@@ -368,29 +376,29 @@ class SphkOps:
     def visc_implicit_setup(self, d_out, b_out, nu, nu_boundary):
         """D_i (n, 6) and b_i (n, 3) of the solve into the given tensors (one sweep)."""
         check(self.L.sphk_visc_implicit_setup(self.ctx, self._s(), _ptr(d_out), _ptr(b_out), C.c_float(nu), C.c_float(nu_boundary),
-                                              C.c_float(self.p.dt), C.c_float(self.p.rho0), C.c_float(self.p.rho_boundary)),
+                                              C.c_float(self.dt), C.c_float(self.p.rho0), C.c_float(self.p.rho_boundary)),
               "sphk_visc_implicit_setup")
 
     def visc_implicit_matvec(self, d_in, p_in, ap_out, nu):
         """(A p)_i (n, 3) from D (n, 6) and p (n, 3) (one sweep)."""
         check(self.L.sphk_visc_implicit_matvec(self.ctx, self._s(), _ptr(d_in), _ptr(p_in), _ptr(ap_out), C.c_float(nu),
-                                               C.c_float(self.p.dt), C.c_float(self.p.rho0)), "sphk_visc_implicit_matvec")
+                                               C.c_float(self.dt), C.c_float(self.p.rho0)), "sphk_visc_implicit_matvec")
 
     def pressure(self):
         check(self.L.sphk_pressure(self.ctx, self._s(), C.c_float(self.p.rho0), C.c_float(self.p.stiff)), "sphk_pressure")
 
     def pressure_force(self):
-        check(self.L.sphk_pressure_force(self.ctx, self._s(), C.c_float(self.p.dt)), "sphk_pressure_force")
+        check(self.L.sphk_pressure_force(self.ctx, self._s(), C.c_float(self.dt)), "sphk_pressure_force")
 
     def advect(self):
-        check(self.L.sphk_advect(self.ctx, self._s(), C.c_float(self.p.dt), self._space), "sphk_advect")
+        check(self.L.sphk_advect(self.ctx, self._s(), C.c_float(self.dt), self._space), "sphk_advect")
 
     def dfsph_density_alpha(self):
         check(self.L.sphk_dfsph_density_alpha(self.ctx, self._s(), _ptr(self.alpha)), "sphk_dfsph_density_alpha")
 
     def dfsph_div_error(self):
         check(self.L.sphk_dfsph_div_error(self.ctx, self._s(), _ptr(self.alpha), _ptr(self.error), _ptr(self.kappa),
-                                          C.c_float(self.p.dt), C.c_float(self.p.rho0)), "sphk_dfsph_div_error")
+                                          C.c_float(self.dt), C.c_float(self.p.rho0)), "sphk_dfsph_div_error")
 
     def dfsph_div_correct(self, stiff=None):
         check(self.L.sphk_dfsph_div_correct(self.ctx, self._s(), _ptr(self.kappa if stiff is None else stiff)),
@@ -398,12 +406,12 @@ class SphkOps:
 
     def dfsph_den_error(self, accumulate_warm: bool):
         check(self.L.sphk_dfsph_den_error(self.ctx, self._s(), _ptr(self.alpha), _ptr(self.error), _ptr(self.kappa),
-                                          C.c_float(self.p.dt), C.c_float(self.p.rho0),
+                                          C.c_float(self.dt), C.c_float(self.p.rho0),
                                           _ptr(self.warm) if accumulate_warm else None), "sphk_dfsph_den_error")
 
     def dfsph_den_correct(self, stiff=None):
         check(self.L.sphk_dfsph_den_correct(self.ctx, self._s(), _ptr(self.kappa if stiff is None else stiff),
-                                            C.c_float(self.p.dt)), "sphk_dfsph_den_correct")
+                                            C.c_float(self.dt)), "sphk_dfsph_den_correct")
 
     def reduce_abs_sum(self, x: torch.Tensor) -> float:
         out = C.c_float()
@@ -424,8 +432,12 @@ class SphkOps:
         check(self.L.sphk_pbd_delta_pos_apply(self.ctx, self._s(), _ptr(self.lam), _ptr(self.dpos),
                                               C.c_float(self.p.rho0), self._space), "sphk_pbd_delta_pos_apply")
 
+    def pbd_dt_prev(self) -> float:
+        """the dt of the last predict (the step's own dt before the first), as PBDSolver::historyTimeStep"""
+        return self.dt if self.pbd_last_dt is None else self.pbd_last_dt
+
     def pbd_velocity_from_positions(self):
-        check(self.L.sphk_pbd_velocity_from_positions(self.ctx, self._s(), _ptr(self.pos_last), C.c_float(self.p.dt)),
+        check(self.L.sphk_pbd_velocity_from_positions(self.ctx, self._s(), _ptr(self.pos_last), C.c_float(self.pbd_dt_prev())),
               "sphk_pbd_velocity_from_positions")
 
     def fused_pbd_xsph_color_grad(self):
@@ -488,7 +500,7 @@ class SphkOps:
         self.pressure()
         self.sync_array(self.fluid.density); self.sync_array(self.fluid.pressure)
         self.pressure_force()
-        self.bodies_react(-np.float32(self.p.dt))
+        self.bodies_react(-np.float32(self.dt))
         self.advect()
 
     def step_dfsph(self):            # DFSPHSolver.cu:33-72
@@ -536,7 +548,7 @@ class SphkOps:
         total, it = 3.4e38, 0        # project :160-210
         self.permute(self.warm, 1)
         self._run(lambda: self.dfsph_den_correct(self.warm), "vel")
-        inv_dt = np.float32(1.0) / np.float32(self.p.dt)
+        inv_dt = np.float32(1.0) / np.float32(self.dt)
         self.bodies_react(inv_dt)
         self._run(lambda: self.dfsph_den_error(False), "scalar", self.kappa)
         self.copy(self.warm, self.kappa)
@@ -557,7 +569,7 @@ class SphkOps:
             return False
         self.set_use_list(self.use_list, 150 if self.use_list else 0)   # skin list: positions move inside the step
         self.permute(self.pos_last, 3)
-        c = np.float32(1.0) / (np.float32(self.p.rho0) * np.float32(self.p.dt))
+        c = np.float32(1.0) / (np.float32(self.p.rho0) * np.float32(self.pbd_dt_prev()))
         for _ in range(self.max_iter):
             self._run(self.pbd_density_lambda, "scalar", self.lam)
             self.bodies_react(c)     # before the positions move: the pairs of this correction
@@ -591,6 +603,7 @@ class SphkOps:
         self.gravity()
         self.copy(self.pos_last, self.fluid.pos)
         self.advect()
+        self.pbd_last_dt = self.dt
         return True
 
     # ---- open boundaries (DESIGN.md section 2.6) --------------------------------------------------------------------------
@@ -617,13 +630,14 @@ class SphkOps:
             check(self.L.sphk_sinks_apply(self.ctx, C.byref(p), self._sinks.ctypes.data_as(C.POINTER(C.c_float)),
                                           C.c_int(self._sinks.shape[0])), "sphk_sinks_apply")
         hist, kind = self._history()
+        hist_dt = self.pbd_dt_prev() if self.solver == "pbd" else self.dt
         e = 0
         for k, em in enumerate(self._emitters):
             per = em.width * em.height
             fit = min((cap - n - e) // per, 65536)
             off = (C.c_float * max(fit, 1))()
             carry, sched = C.c_double(self.emitter_carry[k]), C.c_int(0)
-            check(self.L.sphk_emitter_advance(C.byref(em), C.byref(carry), C.c_float(self.p.dt), C.c_int(fit), off, C.byref(sched)),
+            check(self.L.sphk_emitter_advance(C.byref(em), C.byref(carry), C.c_float(self.dt), C.c_int(fit), off, C.byref(sched)),
                   "sphk_emitter_advance")
             self.emitter_carry[k] = carry.value
             layers = min(sched.value, fit)
@@ -631,7 +645,7 @@ class SphkOps:
             if layers == 0:
                 continue
             check(self.L.sphk_emit(self.ctx, C.byref(p), C.c_int(n + e), C.byref(em), C.c_int(layers), off, C.c_float(self.p.m0),
-                                   C.c_float(self.p.dt), _ptr(hist), C.c_int(kind)), "sphk_emit")
+                                   C.c_float(hist_dt), _ptr(hist), C.c_int(kind)), "sphk_emit")
             e += layers * per
             self._open_stats["emitted"] += layers * per
         return e
@@ -661,7 +675,97 @@ class SphkOps:
         check(self.L.sphk_open_check(self.ctx, C.byref(bits)), "sphk_open_check")
         return int(bits.value)
 
-    def step(self):                  # SPHSystem.cu:129-158 (no host sync here; callers time with CUDA events)
+    # ---- CFL-adaptive time stepping (DESIGN.md section 2.8): the same C rule and order as SPHSystem ------------------------------
+    adaptive = False
+    last_dt = None                   # the dt of the last step (float32 value)
+    simulated_time = 0.0             # the double sum of the float dt of every step
+
+    def set_adaptive(self, C_: float, dt_min: float = 0.0, dt_max: float = 0.0):
+        """SPHSystem::setAdaptiveTimeStep: from the next step on, every step runs at the rule's dt (0 = the defaults: dt_max = the
+        scene's dt, dt_min = dt_max / 64).  Raises ValueError for values the rule refuses (the setting is kept)."""
+        f = lambda x: float(np.float32(x))  # noqa: E731
+        r = capi.SphkTimeStepRule()
+        r.cfl = f(C_)
+        r.dt_max = f(dt_max) if dt_max > 0 else f(self.p.dt)
+        r.dt_min = f(dt_min) if dt_min > 0 else float(np.float32(r.dt_max) / np.float32(64.0))
+        r.radius = f(self.p.radius)
+        g = [f(x) for x in self.p.gravity]
+        r.gravity = float(np.sqrt(g[0] * g[0] + g[1] * g[1] + g[2] * g[2]))
+        dt, flags = C.c_float(0.0), C.c_int(0)
+        if not (dt_min >= 0 and dt_max >= 0) or self.L.sphk_time_step(C.byref(r), C.c_double(0.0), C.c_double(0.0), C.c_double(0.0),
+                                                                      C.byref(dt), C.byref(flags)) != 0:
+            raise ValueError(f"adaptive time stepping needs C > 0, dt_min >= 0 and dt_max >= 0 (finite) with dt_min <= dt_max "
+                             f"(got {C_}, {dt_min}, {dt_max})")
+        if self._emitters and r.dt_max > f(self.p.dt):
+            raise ValueError(f"dt_max {dt_max} is above the scene's dt {self.p.dt}, for which the emitters' layers were placed")
+        self._rule = r
+        self.adaptive = True
+        self.adaptive_stats = {"speed": 0.0, "source": 0, "min_clamps": 0, "nonfinite_steps": 0, "frame_min_dt": 0.0}
+        self.measure_speed()
+
+    def disable_adaptive(self):
+        self.adaptive = False
+        self._step_dt = None
+
+    def measure_speed(self):
+        """enqueues the speed bound of the current state (sphk_step_speed)"""
+        p = self.fluid.abi()
+        check(self.L.sphk_step_speed(self.ctx, C.byref(p), C.c_int(1 if self.n_bodies else 0)), "sphk_step_speed")
+
+    def refresh_speed_bound(self):
+        """SPHSystem::refreshSpeedBound: measure the bound again after writing velocities or positions between steps"""
+        if self.adaptive:
+            self.measure_speed()
+
+    def speed_result(self):
+        """((fluid max |v|, body max |V| + |Omega| r_max), non-finite count) of the last measure_speed"""
+        v, bad = (C.c_float * 2)(), C.c_int(0)
+        check(self.L.sphk_step_speed_result(self.ctx, v, C.byref(bad)), "sphk_step_speed_result")
+        return (float(v[0]), float(v[1])), int(bad.value)
+
+    def choose_time_step(self, remaining: float):
+        """(dt, frame_end) of the next step, as SPHSystem::chooseTimeStep"""
+        (vf, vb), bad = self.speed_result()
+        vmax, source = vf, 0
+        if vb > vmax:
+            vmax, source = vb, 1
+        for em in self._emitters:
+            if em.speed > vmax:
+                vmax, source = float(em.speed), 2
+        dt, flags = C.c_float(0.0), C.c_int(0)
+        check(self.L.sphk_time_step(C.byref(self._rule), C.c_double(vmax), C.c_double(self.last_dt), C.c_double(remaining),
+                                    C.byref(dt), C.byref(flags)), "sphk_time_step")
+        st = self.adaptive_stats
+        st["speed"], st["source"] = vmax, source
+        st["min_clamps"] += bool(flags.value & capi.DT_MIN_CLAMP)
+        st["nonfinite_steps"] += bool(flags.value & capi.DT_NONFINITE) or bad > 0
+        return float(dt.value), bool(flags.value & capi.DT_FRAME_END)
+
+    def advance(self, frame_seconds: float) -> int:
+        """SPHSystem::advance: CFL substeps until frame_seconds of simulated time have passed; returns their count"""
+        if not self.adaptive or not (frame_seconds > 0) or not np.isfinite(frame_seconds):
+            raise ValueError("advance needs an adaptive system and a finite frame > 0")
+        elapsed, k, end, min_dt = 0.0, 0, False, np.inf
+        while not end:
+            dt, end = self.choose_time_step(frame_seconds - elapsed)
+            self._run_step(dt)
+            elapsed += dt
+            min_dt = min(min_dt, dt)
+            k += 1
+        self.adaptive_stats["frame_min_dt"] = min_dt
+        return k
+
+    def step(self):                  # SPHSystem.cu:129-158 (no host sync here, except for the speed bound of an adaptive system)
+        self._run_step(self.choose_time_step(0.0)[0] if self.adaptive else float(np.float32(self.p.dt)))
+
+    def _run_step(self, dt: float):
+        self._step_dt = dt if self.adaptive else None
+        if self._step_body() is not False and self.adaptive:
+            self.measure_speed()     # after the step's last velocity write
+        self.last_dt = dt
+        self.simulated_time += dt
+
+    def _step_body(self):
         e = self.open_emit() if self.open else 0
         if self.n_bodies:            # bodies move before the fluid search, as in SPHSystem::step
             self.bodies_step()
@@ -679,7 +783,7 @@ class SphkOps:
             self.step_dfsph()
         elif self.solver == "pbd":
             if not self.step_pbd():
-                return           # the "throwing" first call: no sweep ran, nothing to integrate (as in SPHSystem::step)
+                return False     # the "throwing" first call: no sweep ran, nothing to integrate (as in SPHSystem::step)
         else:
             self.step_wcsph()
         self.bodies_integrate()
@@ -712,7 +816,7 @@ class SphkSystem(SphkOps):
     reference constructor including its implicit first step (Q3)."""
 
     def __init__(self, scene, device="cuda:0", use_list: bool | None = None, list_capacity: int | None = None,
-                 step0: bool = True, bodies=None, max_fluid: int | None = None, emitters=None, sinks=None):
+                 step0: bool = True, bodies=None, max_fluid: int | None = None, emitters=None, sinks=None, adaptive=None):
         """emitters / sinks: open boundaries (DESIGN.md section 2.6), the same C entries in the same order as SPHSystem::step.
         emitters: dicts {"origin", "direction", "speed", "spacing", "width", "height"} (sphk_emitter); sinks: (lo, hi) boxes; max_fluid:
         the capacity of the fluid set (default: the initial count).  fluid_count is the live count.
@@ -721,7 +825,8 @@ class SphkSystem(SphkOps):
         world frame, and optionally "mass" (> 0: dynamic, two-way coupled; default 0: kinematic, and held -- its reaction reported --
         when another body is dynamic) and "inertia" (3,) principal
         moments about the centre in the axes of "points".  Masses are in the fluid's units, m0 / spacing^3 per unit volume
-        (not rho0).  Their particles follow the static boundary set; every step() moves them before the fluid search."""
+        (not rho0).  Their particles follow the static boundary set; every step() moves them before the fluid search.
+        adaptive: dict(C=, dt_min=0, dt_max=0): CFL-adaptive time stepping (set_adaptive) from the step after the constructor's on."""
         self.L = capi.sphk()
         self.p = scene.params
         self.device = torch.device(device)
@@ -770,6 +875,7 @@ class SphkSystem(SphkOps):
         if list_capacity is not None:
             self.set_option(capi.OPT_LIST_CAPACITY, list_capacity)
         self.solver = self.p.solver
+        self.last_dt = float(np.float32(self.p.dt))   # as SPHSystem's _lastDt: the dt_prev of a first adaptive step
         self.use_list = True if use_list is None else bool(use_list)
         n = self.fluid.n
         self._alloc_solver_buffers(self.fluid.pos.shape[0])
@@ -793,6 +899,8 @@ class SphkSystem(SphkOps):
         self.search_fluid()
         if step0:
             self.step()
+        if adaptive is not None:
+            self.set_adaptive(adaptive["C"], adaptive.get("dt_min", 0.0), adaptive.get("dt_max", 0.0))
 
     def owned(self, t):
         """the live slots of a per-particle tensor (the reductions run over the live count, as in the class layer)"""

@@ -326,6 +326,9 @@ extern "C" int sph_app_upload_fluid(sph_app* app, const float* pos, const float*
     int bad = 0;
     if (pos) bad |= cudaMemcpy(f->getPosPtr(), pos, n * sizeof(float3), cudaMemcpyHostToDevice) != cudaSuccess;
     if (vel) bad |= cudaMemcpy(f->getVelPtr(), vel, n * sizeof(float3), cudaMemcpyHostToDevice) != cudaSuccess;
+#ifndef SPH_APP_REFERENCE_ENGINE
+    app->system->refreshSpeedBound();       // an adaptive system's next dt sees the uploaded state
+#endif
     return bad;
 }
 
@@ -389,6 +392,7 @@ extern "C" int sph_app_submit(sph_app* app, const float* pos_in, const float* ve
     if (!app || !pos_in || !vel_in) return 1;
 #ifndef SPH_APP_REFERENCE_ENGINE
     if (app->system->openBoundariesActive()) return 1;      // the pipelining assumes a fixed particle count
+    if (app->system->adaptiveTimeStep()) return 1;          // ... and a fixed step
 #endif
     if (!pipe_init(app)) return 1;
     const size_t n = app->system->getFluids()->size();
@@ -492,6 +496,45 @@ extern "C" int sph_app_viscosity_stats(sph_app* app, int* iterations, float* rel
     if (!b) return 1;
     if (iterations) *iterations = b->lastViscosityIterations();
     if (rel_residual) *rel_residual = b->lastViscosityResidual();
+    return 0;
+#endif
+}
+
+extern "C" int sph_app_set_adaptive_dt(sph_app* app, float C, float dt_min, float dt_max) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)C; (void)dt_min; (void)dt_max;
+    return 1;
+#else
+    if (!app) return 1;
+    if (C == 0.0f) { app->system->disableAdaptiveTimeStep(); return 0; }
+    return app->system->setAdaptiveTimeStep(C, dt_min, dt_max) ? 0 : 1;
+#endif
+}
+
+extern "C" int sph_app_advance(sph_app* app, double frame_seconds, int* substeps, float* min_dt) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)frame_seconds; (void)substeps; (void)min_dt;
+    return 1;
+#else
+    if (!app || !app->system->adaptiveTimeStep() || !(frame_seconds > 0.0) || !std::isfinite(frame_seconds)) return 1;
+    const int k = app->system->advance(frame_seconds);
+    if (substeps) *substeps = k;
+    if (min_dt) *min_dt = app->system->adaptiveStats().frameMinDt;
+    return k > 0 ? 0 : 1;
+#endif
+}
+
+extern "C" int sph_app_adaptive_stats(sph_app* app, float* speed_dt3, int* source, long long* counts2, double* simulated_time) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)speed_dt3; (void)source; (void)counts2; (void)simulated_time;
+    return 1;
+#else
+    if (!app) return 1;
+    const sphb200::AdaptiveStats s = app->system->adaptiveStats();
+    if (speed_dt3) { speed_dt3[0] = s.speed; speed_dt3[1] = app->system->lastTimeStep(); speed_dt3[2] = s.frameMinDt; }
+    if (source) *source = s.source;
+    if (counts2) { counts2[0] = s.minClamps; counts2[1] = s.nonFiniteSteps; }
+    if (simulated_time) *simulated_time = app->system->simulatedTime();
     return 0;
 #endif
 }

@@ -424,9 +424,11 @@ void PBDSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shared_pt
     // displacement on the device and falls back to the cell walk if the corrections ever exceed skin/2
     if (!beginStep(fluids, boundaries, cellStartFluid, cellStartBoundary, radius, true, 150)) return;
     updateNeighborhood(fluids);
-    reactCoef_ = 1.0f / (rho0 * dt);
+    // the positions were advanced by the last predict: its dt is the interval of the projection and the velocity derivation
+    const float dtPrev = historyTimeStep(dt);
+    reactCoef_ = 1.0f / (rho0 * dtPrev);
     project(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, cellSize, spaceSize, cellLength, radius, maxIter);
-    check(sphk_pbd_velocity_from_positions(current_.ctx, &current_.abi, reinterpret_cast<float*>(fluidPosLast.addr()), dt),
+    check(sphk_pbd_velocity_from_positions(current_.ctx, &current_.abi, reinterpret_cast<float*>(fluidPosLast.addr()), dtPrev),
           "sphk_pbd_velocity_from_positions");
     const bool surface = surfaceTensionIntensity > EPSILON || airPressure > EPSILON;
     if (fusedSweeps_ && vorticityOn()) {
@@ -467,6 +469,7 @@ void PBDSolver::predict(std::shared_ptr<SPHParticles>& fluids, float dt, float3 
                     reinterpret_cast<const float*>(fluids->getPosPtr()), 3 * static_cast<int>(fluids->size())),
           "sphk_copy");
     advect(fluids, dt, spaceSize);
+    lastPredictDt_ = dt;
 }
 
 // :81-87
@@ -552,6 +555,7 @@ SPHSystem::SPHSystem(std::shared_ptr<SPHParticles>& fluidParticles, std::shared_
     CUDA_CALL(cudaEventCreate(&_evStart));
     CUDA_CALL(cudaEventCreate(&_evStop));
     if (const char* g = std::getenv("SPHK_STEP_GRAPH")) _graphEnabled = g[0] != '0';
+    _stepDt = _lastDt = dt;
     if (!_engine->ok()) return;
     _sphM0 = sphM0;
     if (!open.emitters.empty() || !open.sinks.empty()) {
@@ -637,7 +641,7 @@ void SPHSystem::searchForStep() {
     const int e = _open ? openEmit(n) : 0;
     if (!_bodyMotion.empty()) {
         const sphk_particles b = _boundaries->abi();
-        check(sphk_bodies_step(_engine->ctx(), &b, cellStartBoundary.addr(), _dt), "sphk_bodies_step");
+        check(sphk_bodies_step(_engine->ctx(), &b, cellStartBoundary.addr(), _stepDt), "sphk_bodies_step");
     }
     if (!_open) { neighborSearch(_fluids, cellStartFluid); return; }
     _fluids->setActiveCount(n + e);
@@ -658,7 +662,9 @@ int SPHSystem::openEmit(int n) {
     if (!_sinkBoxes.empty())
         check(sphk_sinks_apply(ctx, &f, _sinkBoxes.data(), static_cast<int>(_sinkBoxes.size() / 6)), "sphk_sinks_apply");
     int width = 0;
-    float* history = dynamic_cast<BasicSPHSolver*>(_solver.get())->historyArray(width);
+    auto* solver = dynamic_cast<BasicSPHSolver*>(_solver.get());
+    float* history = solver->historyArray(width);
+    const float historyDt = solver->historyTimeStep(_stepDt);
     const int kind = width == 1 ? 1 : width == 3 ? 2 : 0;
     const int cap = static_cast<int>(_fluids->capacity());
     int e = 0;
@@ -668,13 +674,13 @@ int SPHSystem::openEmit(int n) {
         const int fit = std::min((cap - n - e) / per, 65536);
         if (static_cast<int>(_layerOffsets.size()) < fit) _layerOffsets.resize(static_cast<size_t>(fit));
         int scheduled = 0;
-        const int rc = sphk_emitter_advance(&em, &_emitterCarry[k], _dt, fit, _layerOffsets.data(), &scheduled);
+        const int rc = sphk_emitter_advance(&em, &_emitterCarry[k], _stepDt, fit, _layerOffsets.data(), &scheduled);
         check(rc, "sphk_emitter_advance");
         if (rc != 0) continue;
         const int layers = std::min(scheduled, fit);
         _openStats.refused += static_cast<long long>(scheduled - layers) * per;
         if (layers == 0) continue;
-        check(sphk_emit(ctx, &f, n + e, &em, layers, _layerOffsets.data(), _sphM0, _dt, kind ? history : nullptr, kind), "sphk_emit");
+        check(sphk_emit(ctx, &f, n + e, &em, layers, _layerOffsets.data(), _sphM0, historyDt, kind ? history : nullptr, kind), "sphk_emit");
         e += layers * per;
         _openStats.emitted += static_cast<long long>(layers) * per;
     }
@@ -724,7 +730,7 @@ int SPHSystem::openBoundaryCheck() const {
 void SPHSystem::integrateBodies() {
     if (!_bodiesDynamic) return;
     const float g[3] = {_sphG.x, _sphG.y, _sphG.z};
-    check(sphk_bodies_integrate(_engine->ctx(), _dt, g), "sphk_bodies_integrate");
+    check(sphk_bodies_integrate(_engine->ctx(), _stepDt, g), "sphk_bodies_integrate");
 }
 
 void SPHSystem::setBodyMotion(int body, float3 linearVelocity, float3 angularVelocity) {
@@ -735,6 +741,7 @@ void SPHSystem::setBodyMotion(int body, float3 linearVelocity, float3 angularVel
     const int rc = sphk_bodies_set_body_motion(_engine->ctx(), body, m);   // refuses non-finite values: the motion is kept
     check(rc, "sphk_bodies_set_body_motion");
     if (rc == 0) std::copy(m, m + 6, _bodyMotion.begin() + 6 * body);
+    refreshSpeedBound();                    // the next step's dt must see the new motion (enqueued after its copy)
 }
 
 void SPHSystem::getBodyMotion(int body, float3& linearVelocity, float3& angularVelocity) const {
@@ -795,6 +802,99 @@ void SPHSystem::setStepGraph(bool on) {
 // replayed -- same kernels, same order, same arguments (all scene parameters are const members).
 float SPHSystem::step() {
     if (!_engine->ok()) return 0.0f;
+    bool frameEnd = false;
+    _stepDt = _adaptive ? chooseTimeStep(0.0, frameEnd) : _dt;
+    return runStep();
+}
+
+// ---- CFL-adaptive time stepping (DESIGN.md section 2.8) ----
+bool SPHSystem::setAdaptiveTimeStep(float C, float dtMin, float dtMax) {
+    sphk_time_step_rule r;
+    r.cfl = C;
+    r.dt_max = dtMax > 0.0f ? dtMax : _dt;
+    r.dt_min = dtMin > 0.0f ? dtMin : static_cast<float>(r.dt_max) / 64.0f;
+    r.radius = _sphSmoothingRadius;
+    r.gravity = std::sqrt(double(_sphG.x) * _sphG.x + double(_sphG.y) * _sphG.y + double(_sphG.z) * _sphG.z);
+    float dt = 0.0f;
+    int flags = 0;
+    // the library's rule validates its own parameters
+    if (dtMin < 0.0f || dtMax < 0.0f || sphk_time_step(&r, 0.0, 0.0, 0.0, &dt, &flags) != 0) {
+        printf("setAdaptiveTimeStep: need C > 0, dtMin >= 0 and dtMax >= 0 (finite; 0 = the default) with dtMin <= dtMax (got %g, %g, "
+               "%g); the setting is kept\n", C, dtMin, dtMax);
+        return false;
+    }
+    // the constructor checked that every emitted layer, advanced by speed * dt, stays inside the clamp box: a longer step could
+    // emit past it
+    if (!_emitters.empty() && r.dt_max > _dt) {
+        printf("setAdaptiveTimeStep: dtMax %g is above the constructor's dt %g, for which the emitters were checked; the setting is "
+               "kept\n", dtMax, _dt);
+        return false;
+    }
+    dropStepGraph();
+    _rule = r;
+    _adaptive = true;
+    if (_engine->ok()) measureSpeed();       // the bound of the current state, for the first adaptive step
+    return true;
+}
+
+void SPHSystem::refreshSpeedBound() {
+    if (_adaptive && _engine->ok()) measureSpeed();
+}
+
+void SPHSystem::disableAdaptiveTimeStep() {
+    if (!_adaptive) return;
+    _adaptive = false;
+    _plainSteps = 0;       // a PBD step still derives its velocities over the last adaptive dt: capture after two fixed steps
+}
+
+int SPHSystem::advance(double frameSeconds) {
+    if (!_adaptive || !(frameSeconds > 0.0) || !std::isfinite(frameSeconds)) {
+        printf("SPHSystem::advance: needs an adaptive system (setAdaptiveTimeStep) and a finite frame > 0 (got %g)\n", frameSeconds);
+        return 0;
+    }
+    if (!_engine->ok()) return 0;
+    double elapsed = 0.0;
+    int steps = 0;
+    bool frameEnd = false;
+    float minDt = std::numeric_limits<float>::max();
+    while (!frameEnd) {
+        _stepDt = chooseTimeStep(frameSeconds - elapsed, frameEnd);
+        runStep();
+        elapsed += _stepDt;
+        minDt = std::min(minDt, _stepDt);
+        ++steps;
+    }
+    _adaptiveStats.frameMinDt = minDt;
+    return steps;
+}
+
+void SPHSystem::measureSpeed() {
+    const sphk_particles f = _fluids->abi();
+    check(sphk_step_speed(_engine->ctx(), &f, _bodyMotion.empty() ? 0 : 1), "sphk_step_speed");
+}
+
+float SPHSystem::chooseTimeStep(double remaining, bool& frameEnd) {
+    float v[2] = {0.0f, 0.0f};
+    int nonFinite = 0;
+    check(sphk_step_speed_result(_engine->ctx(), v, &nonFinite), "sphk_step_speed_result");
+    float vmax = v[0];
+    int source = 0;
+    if (v[1] > vmax) { vmax = v[1]; source = 1; }
+    for (const auto& e : _emitters)
+        if (e.speed > vmax) { vmax = e.speed; source = 2; }
+    float dt = _rule.dt_min;
+    int flags = SPHK_DT_NONFINITE;
+    const int rc = sphk_time_step(&_rule, vmax, _lastDt, remaining, &dt, &flags);
+    check(rc, "sphk_time_step");
+    _adaptiveStats.speed = vmax;
+    _adaptiveStats.source = source;
+    if (flags & SPHK_DT_MIN_CLAMP) ++_adaptiveStats.minClamps;
+    if ((flags & SPHK_DT_NONFINITE) || nonFinite > 0) ++_adaptiveStats.nonFiniteSteps;
+    frameEnd = rc != 0 || (flags & SPHK_DT_FRAME_END) != 0;
+    return dt;
+}
+
+float SPHSystem::runStep() {
     cudaStream_t st = _engine->stream();
     sphk_ctx* ctx = _engine->ctx();
     CUDA_CALL(cudaEventRecord(_evStart, st));
@@ -808,7 +908,7 @@ float SPHSystem::step() {
         sphk_add_launches(ctx, _graphLaunches);
         check(sphk_synchronize(ctx), "step");
     } else {
-        const bool capture = _graphEnabled && !_open && _plainSteps >= 2 && solverIsGraphSafe();
+        const bool capture = _graphEnabled && !_open && !_adaptive && _plainSteps >= 2 && solverIsGraphSafe();
         const long long launches0 = sphk_launch_count(ctx);
         bool captured = false;
         if (capture) captured = cudaStreamBeginCapture(st, cudaStreamCaptureModeThreadLocal) == cudaSuccess;
@@ -817,9 +917,10 @@ float SPHSystem::step() {
             searchForStep();
             if (fluidSize() > 0)        // (an open system can run empty)
                 _solver->step(_fluids, _boundaries, cellStartFluid, cellStartBoundary, _spaceSize, _cellSize, _sphCellLength,
-                              _sphSmoothingRadius, _dt, _sphRho0, _sphRhoBoundary, _sphStiff, _sphVisc, _sphG,
+                              _sphSmoothingRadius, _stepDt, _sphRho0, _sphRhoBoundary, _sphStiff, _sphVisc, _sphG,
                               _sphSurfaceTensionIntensity, _sphAirPressure);
             integrateBodies();
+            if (_adaptive) measureSpeed();      // after the step's last velocity write; read before the next step
             ok = true;
         } catch (const char* s) {
             std::cout << s << "\n";
@@ -841,7 +942,7 @@ float SPHSystem::step() {
                 searchForStep();
                 try {
                     _solver->step(_fluids, _boundaries, cellStartFluid, cellStartBoundary, _spaceSize, _cellSize,
-                                  _sphCellLength, _sphSmoothingRadius, _dt, _sphRho0, _sphRhoBoundary, _sphStiff, _sphVisc,
+                                  _sphCellLength, _sphSmoothingRadius, _stepDt, _sphRho0, _sphRhoBoundary, _sphStiff, _sphVisc,
                                   _sphG, _sphSurfaceTensionIntensity, _sphAirPressure);
                     integrateBodies();
                 } catch (const char* s) {
@@ -855,6 +956,8 @@ float SPHSystem::step() {
         if (ok) ++_plainSteps;
         check(sphk_synchronize(ctx), "step");
     }
+    _lastDt = _stepDt;
+    _simTime += _stepDt;
     float milliseconds = 0.0f;
     CUDA_CALL(cudaEventRecord(_evStop, st));
     CUDA_CALL(cudaEventSynchronize(_evStop));

@@ -103,6 +103,14 @@ struct OpenBoundaries {
 struct OpenBoundaryStats {
     long long emitted = 0, removed = 0, refused = 0;   // cumulative particle counts
 };
+// addition: CFL-adaptive time stepping (DESIGN.md section 2.8)
+struct AdaptiveStats {
+    float speed = 0.0f;              // the speed bound v_max the last step's dt was chosen from
+    int source = 0;                  // what set it: 0 = the fluid, 1 = a body, 2 = an emitter
+    long long minClamps = 0;         // steps held at dt_min because C R / v_b was smaller
+    long long nonFiniteSteps = 0;    // steps whose bound left out non-finite velocities, or was not finite
+    float frameMinDt = 0.0f;         // the smallest dt of the last advance()
+};
 }  // namespace sphb200
 
 // ---- DArray.h:21-54 ---------------------------------------------------------------------------
@@ -252,6 +260,8 @@ public:
     virtual float* historyArray(int& width) { width = 0; return nullptr; }
     // addition: the particle count the solver's buffers hold (its constructor's num)
     int capacity() const { return num_; }
+    // addition: the dt an emitted particle's history slot is written with when the coming step runs at dt (PBD: its last predict's)
+    virtual float historyTimeStep(float dt) const { return dt; }
     virtual ~BasicSPHSolver() noexcept {}
     virtual void step(std::shared_ptr<SPHParticles>& fluids, const std::shared_ptr<SPHParticles>& boundaries,
                       const DArray<int>& cellStartFluid, const DArray<int>& cellStartBoundary, float3 spaceSize,
@@ -381,6 +391,7 @@ public:
                       float visc, float3 G, float surfaceTensionIntensity, float airPressure) override;
     bool stepIsGraphSafe() const override { return posLastInitialized && !fieldHook_; }
     float* historyArray(int& width) override { width = 3; return reinterpret_cast<float*>(fluidPosLast.addr()); }
+    float historyTimeStep(float dt) const override { return lastPredictDt_ > 0.0f ? lastPredictDt_ : dt; }
     void initializePosLast(const DArray<float3>& posFluid) {
         CUDA_CALL(cudaMemcpy(fluidPosLast.addr(), posFluid.addr(), sizeof(float3) * std::min(fluidPosLast.length(), posFluid.length()),
                              cudaMemcpyDeviceToDevice));
@@ -396,6 +407,9 @@ protected:
 private:
     void updateNeighborhood(const std::shared_ptr<SPHParticles>& particles);
     float reactCoef_ = 0.0f;       // 1 / (rho0 dt) of the step in flight: c of the position-correction reaction
+    // the dt of the last predict: the projection and the velocity derivation of the next step act on the interval it advanced
+    // (0: none yet, the step's own dt is used)
+    float lastPredictDt_ = 0.0f;
     bool posLastInitialized = false;
     const int maxIter;
     const float xSPH_c;
@@ -469,6 +483,27 @@ public:
     bool openBoundariesActive() const { return _open; }
     // the sticky bits of the per-step count check (sphk_open_check; 0 = every step's in-grid count matched; synchronises)
     int openBoundaryCheck() const;
+    // CFL-adaptive time stepping (DESIGN.md section 2.8): from the next step on, every step() runs at the dt of the rule
+    // sphk_time_step {C, dtMin, dtMax, R = sphSmoothingRadius, |G|} applied to the speed bound the previous step left on the
+    // device (fluid, bodies and the emitters' speeds).  0 = the default: dtMax = the constructor's dt, dtMin = dtMax / 64.
+    // C <= 0, a non-finite value, a negative one, dtMin > dtMax, and for a system with emitters a dtMax above the constructor's dt
+    // (the emitters were checked against the clamp box for that dt) are refused (printed, setting kept, false returned).  An adaptive
+    // system runs plain launches and never captures a step graph; disableAdaptiveTimeStep() returns to the constructor's dt and
+    // allows it again.
+    bool setAdaptiveTimeStep(float C, float dtMin = 0.0f, float dtMax = 0.0f);
+    void disableAdaptiveTimeStep();
+    bool adaptiveTimeStep() const { return _adaptive; }
+    // the next step's dt is chosen from the speed bound measured at the end of the previous step (or by setAdaptiveTimeStep).
+    // setBodyMotion measures it again; a caller that writes velocities or positions through the raw accessors between steps
+    // calls refreshSpeedBound() so that the next dt sees them (no effect on a system that is not adaptive)
+    void refreshSpeedBound();
+    // CFL substeps until frameSeconds (> 0) of simulated time have passed (the last one is shortened to end the frame exactly, the
+    // one before it halved when the frame would otherwise end with a sliver); returns their count (0 and a printed message for a
+    // system that is not adaptive or a frame that is not finite and > 0)
+    int advance(double frameSeconds);
+    float lastTimeStep() const { return _lastDt; }            // the dt of the last step
+    double simulatedTime() const { return _simTime; }         // the double sum of the float dt of every step
+    sphb200::AdaptiveStats adaptiveStats() const { return _adaptiveStats; }
 
 private:
     std::shared_ptr<SPHParticles> _fluids;
@@ -515,6 +550,15 @@ private:
     sphb200::OpenBoundaryStats _openStats;
     const char* openRefusal(const sphb200::OpenBoundaries& open) const;
     int openEmit(int n);                  // sinks and emitters before the search; returns the emitted count
+    // time steps: every kernel of a step receives _stepDt (the constructor's dt unless adaptive)
+    float _stepDt = 0.0f, _lastDt = 0.0f;
+    double _simTime = 0.0;
+    bool _adaptive = false;
+    sphk_time_step_rule _rule{};
+    sphb200::AdaptiveStats _adaptiveStats;
+    float runStep();                      // one step at _stepDt
+    float chooseTimeStep(double remaining, bool& frameEnd);   // waits for the last speed bound, applies the rule
+    void measureSpeed();                  // enqueues the speed bound of the current state (sphk_step_speed)
 };
 
 // ---- vbo.cu:46-51 --------------------------------------------------------------------------------

@@ -395,6 +395,8 @@ float SlabSPHSystem::step() {
     const auto* known = dynamic_cast<const BasicSPHSolver*>(solver_.get());
     if (known && known->implicitViscosity() > 0.0f)
         throw std::runtime_error("SlabSPHSystem: implicit viscosity is not supported on slab ranks (single-GPU SPHSystem only)");
+    if (adaptive_)
+        throw std::runtime_error("SlabSPHSystem: adaptive time stepping is not supported on slab ranks (single-GPU SPHSystem only)");
     cudaStream_t st = engine_->stream();
     CUDA_CALL(cudaEventRecord(evStart_, st));
     if (strayCap_ > 0 && haveRanges_ && comm_) collectStrays();

@@ -52,8 +52,12 @@ public:
     auto getBoundaries() const { return static_cast<const std::shared_ptr<SPHParticles>>(boundaries_); }
     int straysRouted();                                 // strays all ranks collected for the last step (synchronises; introspection)
     const char* haloTransport() const { return transport_ == 1 ? "peer-memory mailboxes" : "NCCL send/recv"; }
+    // the same setter as SPHSystem's; not supported on slab ranks (the speed bound would need a global maximum): step() throws
+    void setAdaptiveTimeStep(float, float = 0.0f, float = 0.0f) { adaptive_ = true; }
+    void disableAdaptiveTimeStep() { adaptive_ = false; }
 
 private:
+    bool adaptive_ = false;
     struct Ranges { int own[2], toLeft[2], toRight[2], first[2], last[2], ghostL[2], ghostR[2]; };
     void beginStep();
     void searchAll(int n);

@@ -283,14 +283,18 @@ class SlabSystem(SphkOps):
     HISTORY = {"dfsph": 1, "wcsph": 0, "pbd": 3}      # extra floats per particle that migrate with it
 
     def __init__(self, scene, rank: int, world: int, device, capacity_factor: float = 1.6, group=None, cut_skew: int = 0,
-                 bodies=None, emitters=None, sinks=None):
+                 bodies=None, emitters=None, sinks=None, adaptive=None):
         """cut_skew: shifts the interior cuts by that many planes off the balanced position (tests of the re-balancing).
         Kinematic bodies (engine.SphkSystem's `bodies`) are single-GPU only: every rank would have to hold every body.  So are
-        open boundaries (engine.SphkSystem's `emitters` / `sinks`): a rank's count is set by the decomposition."""
+        open boundaries (engine.SphkSystem's `emitters` / `sinks`): a rank's count is set by the decomposition.  So is CFL-adaptive time
+        stepping (engine.SphkSystem's `adaptive`)."""
         if bodies:
             raise ValueError("kinematic bodies are not supported on slab ranks (single-GPU engine.SphkSystem only)")
         if emitters or sinks:
             raise ValueError("emitters and sinks are not supported on slab ranks (single-GPU engine.SphkSystem only)")
+        if adaptive:
+            raise ValueError("adaptive time stepping is not supported on slab ranks (the speed bound would need a global maximum; "
+                             "single-GPU engine.SphkSystem only)")
         self.L = capi.sphk()
         self.p = scene.params
         self.rank, self.world = rank, world

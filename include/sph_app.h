@@ -53,7 +53,8 @@ int   sph_app_boundary_size(const sph_app* app);
 int   sph_app_download_fluid(sph_app* app, float* pos_xyz, float* vel_xyz, float* density,
                              float* pressure, float* mass, int* particle2cell);
 int   sph_app_download_boundary(sph_app* app, float* pos_xyz, float* mass, int* particle2cell);
-/* Host->device overwrite of fluid pos / vel through getPosPtr / getVelPtr (either may be NULL). */
+/* Host->device overwrite of fluid pos / vel through getPosPtr / getVelPtr (either may be NULL).  An adaptive system measures its
+ * speed bound again, so the next step's dt sees the uploaded state. */
 int   sph_app_upload_fluid(sph_app* app, const float* pos_xyz, const float* vel_xyz);
 /* Pipelined host-buffer stepping: one call = "advance the particle state held in HOST memory (pos_in, vel_in) by one
  * SPHSystem::step() and deliver pos / vel / density of the result to HOST memory".  The upload of this batch and the
@@ -133,6 +134,20 @@ sph_app* sph_app_create_open(const float* fluid_xyz, int n_fluid, int max_fluid,
  * bits of the per-step count check (0 = fine; 1 = after some step the in-grid particles were not exactly the live ones, e.g. a live
  * particle uploaded outside the grid); synchronises for the bits; 1 on the reference build */
 int   sph_app_open_boundary_stats(sph_app* app, long long* stats3, int* check_bits);
+/* CFL-adaptive time stepping (SPHSystem::setAdaptiveTimeStep; DESIGN.md section 2.8): from the next step on, every step runs at
+ * dt = C R / (v_max + |G| dt_prev) clamped to [dt_min, dt_max] (0 = the defaults: dt_max = params.dt, dt_min = dt_max / 64), v_max
+ * the speed bound of fluid, bodies and emitters the previous step left on the device.  C = 0 turns it off again (back to params.dt).
+ * Returns 1 on the reference build and for values the class layer refuses (C < 0, non-finite or negative values, dt_min > dt_max,
+ * dt_max above params.dt in a system with emitters;
+ * the setting is then kept).  An adaptive system never captures a step graph, and sph_app_submit returns 1 for it. */
+int   sph_app_set_adaptive_dt(sph_app* app, float C, float dt_min, float dt_max);
+/* CFL substeps until frame_seconds (> 0) of simulated time have passed (SPHSystem::advance): their count and smallest dt (either
+ * pointer may be NULL).  1 for a system that is not adaptive, a frame that is not finite and > 0, and on the reference build. */
+int   sph_app_advance(sph_app* app, double frame_seconds, int* substeps, float* min_dt);
+/* speed_dt3 = {the speed bound the last dt was chosen from, the last dt, the smallest dt of the last sph_app_advance}, *source = what
+ * set the bound (0 fluid, 1 body, 2 emitter), counts2 = {steps held at dt_min, steps with non-finite velocities or bound},
+ * *simulated_time = the double sum of the float dt of every step.  Any pointer may be NULL; 1 on the reference build. */
+int   sph_app_adaptive_stats(sph_app* app, float* speed_dt3, int* source, long long* counts2, double* simulated_time);
 /* Name of the engine underneath: "reference-cuda" or "b200-native". */
 const char* sph_app_engine(void);
 

@@ -425,6 +425,39 @@ int sphk_fluid_set_count(sphk_ctx* ctx, const int* cell_start_fluid, int L);
  * synchronises */
 int sphk_open_check(sphk_ctx* ctx, int* error_bits_host);
 
+/* ---- CFL-adaptive time stepping (no reference counterpart; DESIGN.md section 2.8) ---------------------------------------------
+ * The step-size rule {C, dt_min, dt_max, R, |G|}, host only, in double (sphk_time_step):
+ *   v_b = v_max + |G| dt_prev;  dt_cfl = C R / v_b (dt_max when v_b = 0), clamped to [dt_min, dt_max] (SPHK_DT_MIN_CLAMP when
+ *   dt_min binds); a v_max that is not finite gives dt_min (SPHK_DT_NONFINITE).  With remaining > 0 (the rest of a frame):
+ *   remaining <= dt_cfl gives dt = remaining (SPHK_DT_FRAME_END: the frame ends with this step, which may be shorter than
+ *   dt_min), remaining < 2 dt_cfl gives dt = remaining / 2 (no sliver step at the end of the frame).  remaining <= 0: no frame.
+ *   The result is rounded to float once; that float is the dt every kernel of the step receives.
+ * The speed bound of a step (sphk_step_speed) is computed on the device after the step's last velocity write. */
+typedef struct sphk_time_step_rule {
+    double cfl;        /* C > 0 (relative to the support radius R) */
+    double dt_min;     /* 0 < dt_min <= dt_max */
+    double dt_max;
+    double radius;     /* R > 0 */
+    double gravity;    /* |G| >= 0 */
+} sphk_time_step_rule;
+#define SPHK_DT_MIN_CLAMP 1
+#define SPHK_DT_NONFINITE 2
+#define SPHK_DT_FRAME_END 4
+/* Host only (no context, no device).  SPHK_ERR_INVALID: NULL pointers, a rule field that is not finite or out of range,
+ * v_max < 0 (NaN and +inf are accepted and flagged), dt_prev < 0 or not finite, remaining not finite. */
+int sphk_time_step(const sphk_time_step_rule* r, double v_max, double dt_prev, double remaining, float* dt_out, int* flags_out);
+/* Enqueues the speed bound of the current state: max |v| over the live fluid particles [0, fluid->n) (|v|^2 = (vx vx + vy vy) +
+ * vz vz in float, no contraction; warp and block maxima, one atomicMax on the float bits per block: order-independent), particles
+ * with a non-finite velocity component counted (warp-aggregated adds) and left out of the max; with with_bodies != 0 also
+ * |V| + |Omega| r_max per body from the device-resident motions (r_max = max_k |r_k|, from sphk_bodies_init; a non-finite motion
+ * is counted and left out).  The result goes to memory the context owns, then by an asynchronous copy to pinned memory, then an
+ * event.  SPHK_ERR_INVALID: NULL pointers, fluid->n < 0 or > max_fluid; SPHK_ERR_STATE: with_bodies without sphk_bodies_init, or
+ * an active range is set (slab ranks: the bound would need a global maximum). */
+int sphk_step_speed(sphk_ctx* ctx, const sphk_particles* fluid, int with_bodies);
+/* Waits for the copy of the last sphk_step_speed only; v_max_host = float[2] {fluid max |v|, body max |V| + |Omega| r_max} (0 for
+ * an empty set), *nonfinite_host = the particles and bodies left out.  SPHK_ERR_STATE before the first sphk_step_speed. */
+int sphk_step_speed_result(sphk_ctx* ctx, float* v_max_host, int* nonfinite_host);
+
 /* Builds the per-step neighbour list now (sweeps otherwise build it lazily on first use). */
 int sphk_build_neighbor_list(sphk_ctx* ctx, const sphk_scene* s);
 
