@@ -451,11 +451,6 @@ class SphkOps:
     def _surface_enabled(self) -> bool:
         return self.p.surface_tension > EPSILON or self.p.air_pressure > EPSILON
 
-    def _handle_surface(self):       # BasicSPHSolver.cu:262-275
-        if self._surface_enabled():
-            self.color_grad()
-            self.surface()
-
     def _run(self, op, sync=None, tensor=None, split=True):
         """One sweep followed by the halo refresh of what it produced (`sync`: None | "vel" | "scalar" | "array").
         On one GPU the refresh is a no-op; the slab driver overrides this to overlap the exchange with the sweep
@@ -468,34 +463,52 @@ class SphkOps:
         elif sync == "array":
             self.sync_array(tensor)
 
-    def step_wcsph(self):            # BasicSPHSolver.cu:237-260
-        self.set_use_list(self.use_list)
-        self.gravity()
-        vort = self.vorticity_eps > 0
+    def _velocity_stage(self, xsph: bool = False):
+        """The velocity terms of every solver's step, in the class layer's order (BasicSPHSolver::velocityStage): vorticity omega,
+        viscosity (xsph: PBD's XSPH), surface tension, implicit viscosity, vorticity confinement.  With fused sweeps and not xsph
+        the colour gradient must be in color_grad_buf already (the density sweep computes it)."""
+        surface, vort = self._surface_enabled(), self.vorticity_eps > 0
         if vort:
             self._vort_buffers()
-        if self.fused and self._surface_enabled():
-            self._run(lambda: self.fused_density_color_grad(False), "array", self.color_grad_buf)
-            if vort:                 # + omega from the velocities the viscosity term reads
-                self._run(self.fused_viscosity_surface_vorticity, "vel", split=False)
+        if self.fused and xsph and (surface or vort):
+            # XSPH + colour gradient (positions are final after the projection) + omega from the velocities XSPH reads
+            if vort:
+                self._run(lambda: self.fused_pbd_xsph_vorticity(surface), "vel", split=False)
                 self.sync_scalar(self.omega_norm)
             else:
-                self._run(self.fused_viscosity_surface, "vel", split=False)
-            if self.implicit_nu > 0:
-                self._run(self.implicit_viscosity, "vel")
+                self._run(self.fused_pbd_xsph_color_grad, "vel", split=False)
+            if surface:
+                self.sync_array(self.buffer3)
+                self._run(self.surface, "vel")
+        elif self.fused and not xsph and surface:
+            # viscosity + surface (+ omega from the velocities the viscosity term reads)
             if vort:
-                self._run(self.vorticity_confinement, "vel")
+                self._run(self.fused_viscosity_surface_vorticity, "scalar", self.omega_norm, split=False)
+                self.sync_vel()
+            else:
+                self._run(self.fused_viscosity_surface, "vel", split=False)
         else:
             if vort:
                 self._run(self.vorticity, "scalar", self.omega_norm)
-            self._run(self.viscosity, "vel", split=False)
-            if self._surface_enabled():  # handleSurface, :262-275
+            self._run(self.pbd_xsph if xsph else self.viscosity, "vel", split=False)
+            if surface:              # handleSurface, BasicSPHSolver.cu:262-275
                 self._run(self.color_grad, "array", self.buffer3)
                 self._run(self.surface, "vel")
-            if self.implicit_nu > 0:
-                self._run(self.implicit_viscosity, "vel")
-            if vort:
-                self._run(self.vorticity_confinement, "vel")
+        if self.implicit_nu > 0:
+            self._run(self.implicit_viscosity, "vel")
+        if vort:
+            self._run(self.vorticity_confinement, "vel")
+
+    def step_wcsph(self):            # BasicSPHSolver.cu:237-260
+        self.set_use_list(self.use_list)
+        self.gravity()
+        if self.fused:               # density (+ colour gradient) before the velocity terms: it reads positions and masses only
+            if self._surface_enabled():
+                self._run(lambda: self.fused_density_color_grad(False), "array", self.color_grad_buf)
+            else:
+                self.density()
+        self._velocity_stage()
+        if not self.fused:
             self.density()
         self.pressure()
         self.sync_array(self.fluid.density); self.sync_array(self.fluid.pressure)
@@ -506,10 +519,10 @@ class SphkOps:
     def step_dfsph(self):            # DFSPHSolver.cu:33-72
         self.set_use_list(self.use_list)
         n, rho0 = self.n_total(), self.p.rho0
-        fused = self.fused and self._surface_enabled()
         if self.fused:               # density/alpha (+ colour gradient) + the first divergence error (:341) in one sweep
-            self._run(lambda: self.fused_density_alpha_div_error(fused), "scalar", self.kappa)
-            if fused:
+            surface = self._surface_enabled()
+            self._run(lambda: self.fused_density_alpha_div_error(surface), "scalar", self.kappa)
+            if surface:
                 self.sync_array(self.color_grad_buf)
         else:
             self.dfsph_density_alpha()
@@ -526,25 +539,7 @@ class SphkOps:
                 total = self.reduce_sum(self.reduce_abs_sum(self.owned(self.error)))
         self.it_div = it
         self.gravity()
-        vort = self.vorticity_eps > 0
-        if vort:
-            self._vort_buffers()
-        if fused and vort:           # + omega from the velocities the viscosity term reads
-            self._run(self.fused_viscosity_surface_vorticity, "vel", split=False)
-            self.sync_scalar(self.omega_norm)
-        elif fused:
-            self._run(self.fused_viscosity_surface, "vel", split=False)
-        else:
-            if vort:
-                self._run(self.vorticity, "scalar", self.omega_norm)
-            self._run(self.viscosity, "vel", split=False)
-            if self._surface_enabled():
-                self._run(self.color_grad, "array", self.buffer3)
-                self._run(self.surface, "vel")
-        if self.implicit_nu > 0:     # after surface, before the density solve
-            self._run(self.implicit_viscosity, "vel")
-        if vort:                     # after surface, before the density solve
-            self._run(self.vorticity_confinement, "vel")
+        self._velocity_stage()
         total, it = 3.4e38, 0        # project :160-210
         self.permute(self.warm, 1)
         self._run(lambda: self.dfsph_den_correct(self.warm), "vel")
@@ -575,31 +570,7 @@ class SphkOps:
             self.bodies_react(c)     # before the positions move: the pairs of this correction
             self.pbd_delta_pos_apply(); self.sync_positions()
         self.pbd_velocity_from_positions()
-        vort = self.vorticity_eps > 0
-        if vort:
-            self._vort_buffers()
-        if self.fused and vort:      # XSPH (+ colour gradient) + omega from the velocities XSPH reads
-            surf = self._surface_enabled()
-            self._run(lambda: self.fused_pbd_xsph_vorticity(surf), "vel", split=False)
-            self.sync_scalar(self.omega_norm)
-            if surf:
-                self.sync_array(self.buffer3)
-                self._run(self.surface, "vel")
-        elif self.fused and self._surface_enabled():   # XSPH + colour gradient in one sweep, then the surface sweep
-            self._run(self.fused_pbd_xsph_color_grad, "vel", split=False)
-            self.sync_array(self.buffer3)
-            self._run(self.surface, "vel")
-        else:
-            if vort:
-                self._run(self.vorticity, "scalar", self.omega_norm)
-            self._run(self.pbd_xsph, "vel", split=False)
-            if self._surface_enabled():
-                self._run(self.color_grad, "array", self.buffer3)
-                self._run(self.surface, "vel")
-        if self.implicit_nu > 0:     # after XSPH and surface, before gravity
-            self._run(self.implicit_viscosity, "vel")
-        if vort:                     # after XSPH and surface, before gravity
-            self._run(self.vorticity_confinement, "vel")
+        self._velocity_stage(xsph=True)
         self.gravity()
         self.copy(self.pos_last, self.fluid.pos)
         self.advect()
@@ -779,14 +750,19 @@ class SphkOps:
         if self.use_list:            # (the C++ layer builds the list lazily in the first sweep; same kernel)
             self.set_use_list(True, 150 if self.solver == "pbd" else 0)
             self.build_neighbor_list()
+        if not self._step_solver():
+            return False             # the "throwing" first call: no sweep ran, nothing to integrate (as in SPHSystem::step)
+        self.bodies_integrate()
+
+    def _step_solver(self) -> bool:
+        """the solver's part of a step; False for PBD's "throwing" first call"""
         if self.solver == "dfsph":
             self.step_dfsph()
         elif self.solver == "pbd":
-            if not self.step_pbd():
-                return False     # the "throwing" first call: no sweep ran, nothing to integrate (as in SPHSystem::step)
+            return self.step_pbd()
         else:
             self.step_wcsph()
-        self.bodies_integrate()
+        return True
 
     def state(self) -> dict:
         """the live fluid particles (and every boundary particle) on the host"""

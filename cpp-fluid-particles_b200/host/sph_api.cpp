@@ -89,21 +89,68 @@ void BasicSPHSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shar
                           int3 cellSize, float cellLength, float radius, float dt, float rho0, float rhoB, float stiff,
                           float visc, float3 G, float surfaceTensionIntensity, float airPressure) {
     if (!beginStep(fluids, boundaries, cellStartFluid, cellStartBoundary, radius, true, 0)) return;
-    const bool surface = surfaceTensionIntensity > EPSILON || airPressure > EPSILON;
     force(fluids, dt, G);
     if (fusedSweeps_) {
-        // density and the colour gradient depend on positions and masses only: one sweep computes both (the
-        // reference computes them in two sweeps, :277-330 and :32-83, with nothing in between that they read)
-        densityAndColorGrad(nullptr, rho0, rhoB, surface);
-        if (surface) produced(0, colorGradBuffer(), 3);
-        diffuseAndSurface(rho0, rhoB, visc, dt, surfaceTensionIntensity, airPressure, surface, true);
-        producedVel(fluids);
-        if (implicitViscosityOn()) implicitViscosity(fluids, rho0, rhoB, dt);
-        if (vorticityOn()) confine(fluids, rho0, dt);
+        // density and the colour gradient depend on positions and masses only: one sweep computes both, before the velocity
+        // terms (the reference computes them in two sweeps, :277-330 and :32-83, with nothing in between that they read)
+        if (surfaceTensionIntensity > EPSILON || airPressure > EPSILON) {
+            check(sphk_fused_density_color_grad(current_.ctx, &current_.abi, colorGradBuffer(), rho0, rhoB), "sphk_fused_density_color_grad");
+            produced(0, colorGradBuffer(), 3);
+        } else {
+            check(sphk_density(current_.ctx, &current_.abi), "sphk_density");
+        }
+    }
+    velocityStage(fluids, boundaries, cellStartFluid, cellStartBoundary, cellSize, cellLength, radius, rho0, rhoB, visc, dt,
+                  surfaceTensionIntensity, airPressure, false);
+    if (fusedSweeps_) {
         check(sphk_pressure(current_.ctx, &current_.abi, rho0, stiff), "sphk_pressure");
         produced(0, fluids->getDensityPtr(), 1); produced(0, fluids->getPressurePtr(), 1);
         check(sphk_pressure_force(current_.ctx, &current_.abi, dt), "sphk_pressure_force");
         react(-dt);
+    } else {
+        project(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, stiff, cellSize, cellLength, radius, dt);
+    }
+    advect(fluids, dt, spaceSize);
+}
+
+// The velocity terms every solver applies between its density and its pressure (PBD: after its position) solve.  Fused sweeps
+// where the library has them; one sweep per reference launch site through the virtual hooks otherwise, and where there is nothing
+// to fuse (PBD's XSPH through its diffuse override).
+void BasicSPHSolver::velocityStage(std::shared_ptr<SPHParticles>& fluids, const std::shared_ptr<SPHParticles>& boundaries,
+                                   const DArray<int>& cellStartFluid, const DArray<int>& cellStartBoundary, int3 cellSize,
+                                   float cellLength, float radius, float rho0, float rhoB, float visc, float dt,
+                                   float surfaceTensionIntensity, float airPressure, bool xsph) {
+    const bool surface = surfaceTensionIntensity > EPSILON || airPressure > EPSILON;
+    float* dv = reinterpret_cast<float*>(bufferFloat3.addr());
+    float* cg = colorGradBuffer();
+    if (fusedSweeps_ && xsph && (surface || vorticityOn())) {
+        // XSPH + colour gradient (positions are final after the projection) + omega from the velocities XSPH reads, in one sweep
+        if (vorticityOn()) {
+            check(sphk_fused_pbd_xsph_vorticity(current_.ctx, &current_.abi, visc, rho0, surface ? cg : nullptr, rhoB, omegaBuffer(),
+                                                omegaNormBuffer()),
+                  "sphk_fused_pbd_xsph_vorticity");
+            producedVel(fluids); produced(2, omegaNormBuffer(), 1);
+        } else {
+            check(sphk_fused_pbd_xsph_color_grad(current_.ctx, &current_.abi, visc, rho0, cg, rhoB), "sphk_fused_pbd_xsph_color_grad");
+            producedVel(fluids);
+        }
+        if (surface) {
+            produced(0, cg, 3);
+            check(sphk_surface(current_.ctx, &current_.abi, cg, dt, rho0, surfaceTensionIntensity, airPressure), "sphk_surface");
+            producedVel(fluids);
+        }
+    } else if (fusedSweeps_ && !xsph && surface) {
+        // viscosity + surface from the colour gradient of the density sweep (+ omega from the velocities the viscosity term reads)
+        if (vorticityOn()) {
+            check(sphk_fused_viscosity_surface_vorticity(current_.ctx, &current_.abi, dv, cg, rho0, visc, dt, surfaceTensionIntensity,
+                                                         airPressure, omegaBuffer(), omegaNormBuffer()),
+                  "sphk_fused_viscosity_surface_vorticity");
+            produced(2, omegaNormBuffer(), 1);
+        } else {
+            check(sphk_fused_viscosity_surface(current_.ctx, &current_.abi, dv, cg, rho0, visc, dt, surfaceTensionIntensity, airPressure),
+                  "sphk_fused_viscosity_surface");
+        }
+        producedVel(fluids);
     } else {
         if (vorticityOn()) vorticity(rho0);
         diffuse(fluids, cellStartFluid, cellSize, cellLength, rho0, radius, visc, dt);
@@ -111,45 +158,9 @@ void BasicSPHSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shar
         if (surface)
             handleSurface(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, rhoB, cellSize, cellLength, radius,
                           dt, surfaceTensionIntensity, airPressure);
-        if (implicitViscosityOn()) implicitViscosity(fluids, rho0, rhoB, dt);
-        if (vorticityOn()) confine(fluids, rho0, dt);
-        project(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, stiff, cellSize, cellLength, radius, dt);
     }
-    advect(fluids, dt, spaceSize);
-}
-
-void BasicSPHSolver::densityAndColorGrad(float* alphaOrNull, float rho0, float rhoB, bool surface) {
-    float* cg = reinterpret_cast<float*>(bufferColorGrad.addr());
-    if (alphaOrNull) {
-        if (surface) check(sphk_fused_dfsph_density_alpha_color_grad(current_.ctx, &current_.abi, alphaOrNull, cg, rho0, rhoB),
-                           "sphk_fused_dfsph_density_alpha_color_grad");
-        else check(sphk_dfsph_density_alpha(current_.ctx, &current_.abi, alphaOrNull), "sphk_dfsph_density_alpha");
-    } else {
-        if (surface) check(sphk_fused_density_color_grad(current_.ctx, &current_.abi, cg, rho0, rhoB), "sphk_fused_density_color_grad");
-        else check(sphk_density(current_.ctx, &current_.abi), "sphk_density");
-    }
-}
-
-void BasicSPHSolver::diffuseAndSurface(float rho0, float rhoB, float visc, float dt, float surfaceTensionIntensity,
-                                       float airPressure, bool surface, bool colorGradReady) {
-    float* dv = reinterpret_cast<float*>(bufferFloat3.addr());
-    float* cg = reinterpret_cast<float*>(bufferColorGrad.addr());
-    if (!surface) {
-        if (vorticityOn()) vorticity(rho0);
-        check(sphk_viscosity(current_.ctx, &current_.abi, dv, rho0, visc, dt), "sphk_viscosity");
-        return;
-    }
-    if (!colorGradReady) check(sphk_color_grad(current_.ctx, &current_.abi, cg, rho0, rhoB), "sphk_color_grad");
-    if (vorticityOn()) {
-        // omega from the velocities the viscosity term reads, in the same sweep
-        check(sphk_fused_viscosity_surface_vorticity(current_.ctx, &current_.abi, dv, cg, rho0, visc, dt, surfaceTensionIntensity,
-                                                     airPressure, omegaBuffer(), omegaNormBuffer()),
-              "sphk_fused_viscosity_surface_vorticity");
-        produced(2, omegaNormBuffer(), 1);
-        return;
-    }
-    check(sphk_fused_viscosity_surface(current_.ctx, &current_.abi, dv, cg, rho0, visc, dt, surfaceTensionIntensity, airPressure),
-          "sphk_fused_viscosity_surface");
+    if (implicitViscosityOn()) implicitViscosity(fluids, rho0, rhoB, dt);
+    if (vorticityOn()) confine(fluids, rho0, dt);
 }
 
 // addition (no reference counterpart): vorticity confinement, sphk.h
@@ -266,9 +277,9 @@ void DFSPHSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shared_
                        float visc, float3 G, float surfaceTensionIntensity, float airPressure) {
     if (!beginStep(fluids, boundaries, cellStartFluid, cellStartBoundary, radius, true, 0)) return;
     const int num = static_cast<int>(fluids->size());
-    const bool surface = surfaceTensionIntensity > EPSILON || airPressure > EPSILON;
     if (fusedSweeps_) {
         // density/alpha + colour gradient (positions only) + the first divergence error of :341 in one sweep
+        const bool surface = surfaceTensionIntensity > EPSILON || airPressure > EPSILON;
         check(sphk_fused_dfsph_density_alpha_div_error(current_.ctx, &current_.abi, alpha.addr(), surface ? colorGradBuffer() : nullptr,
                                                        rho0, rhoB, error.addr(), bufferFloat.addr(), dt),
               "sphk_fused_dfsph_density_alpha_div_error");
@@ -279,19 +290,8 @@ void DFSPHSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shared_
     }
     itDiv_ = correctDivergenceError(rho0, dt, divergenceErrorThreshold, maxIter, num, fusedSweeps_);
     force(fluids, dt, G);
-    if (fusedSweeps_) {
-        diffuseAndSurface(rho0, rhoB, visc, dt, surfaceTensionIntensity, airPressure, surface, true);
-        producedVel(fluids);
-    } else {
-        if (vorticityOn()) vorticity(rho0);
-        BasicSPHSolver::diffuse(fluids, cellStartFluid, cellSize, cellLength, rho0, radius, visc, dt);
-        producedVel(fluids);
-        if (surface)
-            handleSurface(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, rhoB, cellSize, cellLength, radius,
-                          dt, surfaceTensionIntensity, airPressure);
-    }
-    if (implicitViscosityOn()) implicitViscosity(fluids, rho0, rhoB, dt);   // after surface, before the density solve
-    if (vorticityOn()) confine(fluids, rho0, dt);      // after surface, before the density solve
+    velocityStage(fluids, boundaries, cellStartFluid, cellStartBoundary, cellSize, cellLength, radius, rho0, rhoB, visc, dt,
+                  surfaceTensionIntensity, airPressure, false);
     itDen_ = project(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, cellSize, cellLength, radius, dt,
                      densityErrorThreshold, maxIter);
     advect(fluids, dt, spaceSize);
@@ -430,35 +430,8 @@ void PBDSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shared_pt
     project(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, cellSize, spaceSize, cellLength, radius, maxIter);
     check(sphk_pbd_velocity_from_positions(current_.ctx, &current_.abi, reinterpret_cast<float*>(fluidPosLast.addr()), dtPrev),
           "sphk_pbd_velocity_from_positions");
-    const bool surface = surfaceTensionIntensity > EPSILON || airPressure > EPSILON;
-    if (fusedSweeps_ && vorticityOn()) {
-        // XSPH (+ colour gradient) + vorticity in one sweep, omega from the velocities XSPH reads
-        float* cg = surface ? colorGradBuffer() : nullptr;
-        check(sphk_fused_pbd_xsph_vorticity(current_.ctx, &current_.abi, xSPH_c, rho0, cg, rhoB, omegaBuffer(), omegaNormBuffer()),
-              "sphk_fused_pbd_xsph_vorticity");
-        producedVel(fluids); produced(2, omegaNormBuffer(), 1);
-        if (surface) {
-            produced(0, cg, 3);
-            check(sphk_surface(current_.ctx, &current_.abi, cg, dt, rho0, surfaceTensionIntensity, airPressure), "sphk_surface");
-            producedVel(fluids);
-        }
-    } else if (fusedSweeps_ && surface) {
-        // XSPH + colour gradient in one sweep (positions are final after the projection), then the surface sweep
-        float* cg = colorGradBuffer();
-        check(sphk_fused_pbd_xsph_color_grad(current_.ctx, &current_.abi, xSPH_c, rho0, cg, rhoB), "sphk_fused_pbd_xsph_color_grad");
-        producedVel(fluids); produced(0, cg, 3);
-        check(sphk_surface(current_.ctx, &current_.abi, cg, dt, rho0, surfaceTensionIntensity, airPressure), "sphk_surface");
-        producedVel(fluids);
-    } else {
-        if (vorticityOn()) vorticity(rho0);
-        diffuse(fluids, cellStartFluid, cellSize, cellLength, rho0, radius, xSPH_c);
-        producedVel(fluids);
-        if (surface)
-            handleSurface(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, rhoB, cellSize, cellLength, radius,
-                          dt, surfaceTensionIntensity, airPressure);
-    }
-    if (implicitViscosityOn()) implicitViscosity(fluids, rho0, rhoB, dt);   // after XSPH and surface, before gravity
-    if (vorticityOn()) confine(fluids, rho0, dt);      // after XSPH and surface, before gravity
+    velocityStage(fluids, boundaries, cellStartFluid, cellStartBoundary, cellSize, cellLength, radius, rho0, rhoB, xSPH_c, dt,
+                  surfaceTensionIntensity, airPressure, true);
     force(fluids, dt, G);
     predict(fluids, dt, spaceSize);
 }
@@ -481,6 +454,10 @@ void PBDSolver::updateNeighborhood(const std::shared_ptr<SPHParticles>& particle
 // :117-125
 void PBDSolver::diffuse(std::shared_ptr<SPHParticles>&, const DArray<int>&, int3, float, float rho0, float, float visc) {
     check(sphk_pbd_xsph(current_.ctx, &current_.abi, visc, rho0), "sphk_pbd_xsph");
+}
+void PBDSolver::diffuse(std::shared_ptr<SPHParticles>& fluids, const DArray<int>& cellStartFluid, int3 cellSize, float cellLength,
+                        float rho0, float radius, float visc, float) {
+    diffuse(fluids, cellStartFluid, cellSize, cellLength, rho0, radius, visc);
 }
 
 // :225-258

@@ -285,10 +285,13 @@ protected:
         sphk_scene abi{};
     };
     StepScene current_;
-    // fused replacements of {computeDensity | computeDensityAlpha} + colour gradient, and viscosity + surface
-    void densityAndColorGrad(float* alphaOrNull, float rho0, float rhoB, bool surface);
-    void diffuseAndSurface(float rho0, float rhoB, float visc, float dt, float surfaceTensionIntensity, float airPressure,
-                           bool surface, bool colorGradReady);
+    // the velocity terms of every solver's step, in this order: vorticity omega, viscosity (xsph: PBD's XSPH with coefficient
+    // visc), surface tension, implicit viscosity, vorticity confinement.  With fused sweeps and xsph false the colour gradient
+    // must be in colorGradBuffer() already (the density sweep computes it).
+    void velocityStage(std::shared_ptr<SPHParticles>& fluids, const std::shared_ptr<SPHParticles>& boundaries,
+                       const DArray<int>& cellStartFluid, const DArray<int>& cellStartBoundary, int3 cellSize, float cellLength,
+                       float radius, float rho0, float rhoB, float visc, float dt, float surfaceTensionIntensity, float airPressure,
+                       bool xsph);
     bool fusedSweeps_ = true;
     unsigned int configEpoch_ = 0;
     FieldHook fieldHook_;
@@ -404,6 +407,9 @@ protected:
                         int3 cellSize, float3 spaceSize, float cellLength, float radius, int maxIter);
     virtual void diffuse(std::shared_ptr<SPHParticles>& fluids, const DArray<int>& cellStartFluid, int3 cellSize,
                          float cellLength, float rho0, float radius, float visc);
+    // XSPH is PBD's viscosity term: the base class's velocity stage reaches the hook above through this one (visc = xSPH_c)
+    void diffuse(std::shared_ptr<SPHParticles>& fluids, const DArray<int>& cellStartFluid, int3 cellSize, float cellLength,
+                 float rho0, float radius, float visc, float dt) override;
 private:
     void updateNeighborhood(const std::shared_ptr<SPHParticles>& particles);
     float reactCoef_ = 0.0f;       // 1 / (rho0 dt) of the step in flight: c of the position-correction reaction

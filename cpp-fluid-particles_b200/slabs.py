@@ -997,12 +997,7 @@ class SlabSystem(SphkOps):
         if self.rebalance_every > 0 and self._step_no % self.rebalance_every == 0:
             self.rebalance()
         self.begin_step()
-        if self.solver == "dfsph":
-            self.step_dfsph()
-        elif self.solver == "pbd":
-            self.step_pbd()
-        else:
-            self.step_wcsph()
+        self._step_solver()
 
     def n_global(self):
         self._refresh_ranges()
