@@ -754,33 +754,52 @@ k_build_tile(const DevScene s, unsigned short* __restrict__ nbr16, int* __restri
 // list it writes is the int32 per-particle list of k_build_list (global record indices, int4 batches, padded with the
 // particle itself) -- entry for entry, so the list sweeps and the list tests do not care which builder ran.
 // A tile whose windows exceed the staging capacity, and particles outside the grid, take the global-memory path.
+// Each lane collects its hits four at a time in registers and writes one int4 per completed batch (not one 4-byte store
+// per entry); the candidate tests of a chunk are built into the hit mask four at a time, with constant shifts.
 #define SPHK_BUILD_CAP 2047
-__device__ __forceinline__ void build_range_staged(const float4* smA, int slot0, int j0g, int count, float3 xi, float r2list, int self,
-                                                   int kmax, int& n, int*& wp, long long jump) {
-    for (int k0 = 0; k0 < count; k0 += 32) {
-        const int len = min(32, count - k0);
-        const float4* base = smA + slot0 + k0;
-        unsigned int mask = 0u;
-#pragma unroll 4
-        for (int k = 0; k < len; ++k) {
-            const float3 d = xi - xyz(base[k]);
-            mask |= (dot3(d, d) <= r2list ? 1u : 0u) << k;
+#define SPHK_BUILD_OVERREAD 3                       // records the 4-candidate groups may read past a range (masked out)
+struct ListBatch {
+    int4 e;                                         // the open batch; its newest entry in .w
+    int n;                                          // entries appended so far (the true count, may exceed kmax)
+    int4* wp;                                       // where the open batch goes: nbr4[(n / 4) * stride + i]
+    __device__ __forceinline__ void push(int v, int stride, int kmax) {
+        e = make_int4(e.y, e.z, e.w, v);
+        if ((n & 3) == 3) {
+            if (n < kmax) *wp = e;
+            wp += stride;
         }
-        const int sf = self - (j0g + k0);
+        ++n;
+    }
+};
+
+// candidates [a, b) (record indices; slot = index + slotOff) against xi, hits except `self` appended in ascending order
+__device__ __forceinline__ void build_range_staged(const float4* smA, int slotOff, int a, int b, float3 xi, float r2list, int self,
+                                                   ListBatch& lb, int stride, int kmax) {
+    for (int g0 = a; g0 < b; g0 += 32) {
+        const int len = min(32, b - g0);
+        const float4* base = smA + slotOff + g0;
+        unsigned int mask = 0u;
+        for (int k = 0; k < len; k += 4) {         // a group may run past len: those bits are cleared below
+            const float3 d0 = xi - xyz(base[k]), d1 = xi - xyz(base[k + 1]);
+            const float3 d2 = xi - xyz(base[k + 2]), d3 = xi - xyz(base[k + 3]);
+            const unsigned int m4 = (dot3(d0, d0) <= r2list ? 1u : 0u) | (dot3(d1, d1) <= r2list ? 2u : 0u) |
+                                    (dot3(d2, d2) <= r2list ? 4u : 0u) | (dot3(d3, d3) <= r2list ? 8u : 0u);
+            mask |= m4 << k;
+        }
+        mask &= 0xffffffffu >> (32 - len);
+        const int sf = self - g0;
         if (sf >= 0 && sf < 32) mask &= ~(1u << sf);
         while (mask) {
             const int k = __ffs(mask) - 1;
             mask &= mask - 1;
-            if (n < kmax) *wp = j0g + k0 + k;
-            wp += ((n & 3) == 3) ? jump : 1;
-            ++n;
+            lb.push(g0 + k, stride, kmax);
         }
     }
 }
 
 __global__ void __launch_bounds__(SPHK_BLOCK)
 k_build_list_staged(const DevScene s, int* __restrict__ nbr, int* __restrict__ cnt, float4* __restrict__ posBuild) {
-    extern __shared__ float4 smA[];                 // [SPHK_BUILD_CAP + 1]
+    extern __shared__ float4 smA[];                 // [SPHK_BUILD_CAP + 1 + SPHK_BUILD_OVERREAD]
     __shared__ unsigned long long bar;
     __shared__ int sMin, sMax;
     __shared__ int2 sWin[SPHK_TILE_WINS];
@@ -811,25 +830,19 @@ k_build_list_staged(const DevScene s, int* __restrict__ nbr, int* __restrict__ c
     if (!staged || c >= ncells) { build_particle_global(s, i, lo, nbr, cnt, posBuild); return; }
     const float3 xi = xyz(lo);
     const int zlo = max(cz - 1, 0), zhi = min(cz + 1, s.cs.z - 1);
-    int n = 0;
-    int* wp = nbr + static_cast<size_t>(i) * 4;
-    const long long jump = static_cast<long long>(s.nbrStride) * 4 - 3;
+    ListBatch lb{make_int4(i, i, i, i), 0, reinterpret_cast<int4*>(nbr) + i};
 #pragma unroll 1
     for (int r = 0; r < 9; ++r) {
         const int x = cx + r / 3 - 1, y = cy + r % 3 - 1;
         if (x < 0 || x >= s.cs.x || y < 0 || y >= s.cs.y) continue;
         const int c0 = (x * s.cs.y + y) * s.cs.z;
-        {
-            const int a = s.csF[c0 + zlo], b = s.csF[c0 + zhi + 1];
-            build_range_staged(smA, sPre[r] + (a - sWin[r].x), a, b - a, xi, s.r2list, i, s.kmax, n, wp, jump);
-        }
-        {
-            const int a = s.csB[c0 + zlo], b = s.csB[c0 + zhi + 1];
-            if (b > a) build_range_staged(smA, sPre[r + 9] + (a + s.bOff - sWin[r + 9].x), a + s.bOff, b - a, xi, s.r2list, -1, s.kmax, n, wp, jump);
-        }
+        build_range_staged(smA, sPre[r] - sWin[r].x, s.csF[c0 + zlo], s.csF[c0 + zhi + 1], xi, s.r2list, i, lb, s.nbrStride, s.kmax);
+        const int a = s.csB[c0 + zlo], b = s.csB[c0 + zhi + 1];
+        if (b > a) build_range_staged(smA, sPre[r + 9] - sWin[r + 9].x, a + s.bOff, b + s.bOff, xi, s.r2list, -1, lb, s.nbrStride, s.kmax);
     }
-    cnt[i] = n;
-    for (int m = n; (m & 3) && m < s.kmax; ++m) { *wp = i; ++wp; }            // pad the open batch with the particle itself
+    cnt[i] = lb.n;
+    if (lb.n < s.kmax)                              // pad the open batch with the particle itself
+        while (lb.n & 3) lb.push(i, s.nbrStride, s.kmax);
 }
 
 // ---- sweep ----------------------------------------------------------------------------------------------------------------
@@ -1186,7 +1199,7 @@ static int ensure_list(sphk_ctx* c, const DevScene& d) {
         k_sweep_cells<OpBuildList><<<sphk_blocks(b.iEnd - b.iBegin), SPHK_BLOCK, 0, c->stream>>>(b, op);
     } else if (c->stagedBuild) {
         static bool attr = false;
-        const int smem = (SPHK_BUILD_CAP + 1) * 16;
+        const int smem = (SPHK_BUILD_CAP + 1 + SPHK_BUILD_OVERREAD) * 16;
         if (!attr) { cudaFuncSetAttribute(k_build_list_staged, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); attr = true; }
         const int tiles = (b.iEnd + SPHK_BLOCK - 1) / SPHK_BLOCK - b.iBegin / SPHK_BLOCK;
         k_build_list_staged<<<tiles, SPHK_BLOCK, smem, c->stream>>>(b, c->nbr, c->cnt, nullptr);
