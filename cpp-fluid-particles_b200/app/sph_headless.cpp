@@ -10,7 +10,13 @@
 //   sph_headless [--solver sph|dfsph|pbd] [--frames N] [--box L | --box LX LY LZ] [--block NX NY NZ] [--origin X Y Z]
 //                [--dt DT] [--iters K] [--vorticity EPS] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] [--ranks N [--rank R --rendezvous DIR]]
 //                [--bullets K] [--stir OMEGA] [--float REL] [--implicit-viscosity NU] [--tap SPEED] [--drain SIDE] [--capacity N]
-//                [--cfl C [--dt-min X]]
+//                [--cfl C [--dt-min X]] [--rheology cross:NU0,NUINF,LAMBDA,M | hb:K,N,TAU[,MREG] [--rheology-max NU_MAX] [--no-slip]]
+// --rheology turns on non-Newtonian viscosity (BasicSPHSolver::setRheology, DESIGN.md section 2.9) after the constructor's step 0,
+// for every solver, instead of --implicit-viscosity: a Cross fluid (shear-thinning; Newtonian with NU0 = NUINF) or a
+// Herschel-Bulkley fluid with yield stress TAU (kinematic; Bingham with N = 1), regularisation MREG (default 1000 s).  nu is
+// clamped to [0, NU_MAX]; NU_MAX defaults to max(NU0, NUINF) for Cross and to 1 for Herschel-Bulkley.  --no-slip: walls and a
+// --stir paddle act with the fluid's own nu (boundary factor 1; default 0, free slip; not together with --float).  Every frame
+// prints the solve's iterations, the largest shear rate and the particles at the NU_MAX clamp.  Single GPU only.
 // --cfl C turns on CFL-adaptive time stepping (SPHSystem::setAdaptiveTimeStep, DESIGN.md section 2.8) after the constructor's step 0:
 // every frame then advances --dt of simulated time in CFL substeps (SPHSystem::advance; dt_max = --dt, dt_min = X or dt / 64) and
 // prints their count and the smallest dt of the frame; the JSON summary adds the substeps of every frame.  Single GPU only.
@@ -90,12 +96,43 @@ struct Options {
     float tap = 0.0f;                         // --tap SPEED: an emitter above the block (0: none)
     float drain = 0.0f;                       // --drain SIDE: a floor sink (0: none)
     long long capacity = 0;                   // --capacity N: fluid capacity of an open system (0: twice the initial count)
+    std::string rheology;                     // --rheology MODEL:PARAMS (empty: off)
+    float rheologyMax = -1.0f;                // --rheology-max NU_MAX (< 0: the model's default)
+    bool noSlip = false;                      // --no-slip: boundary factor 1 for --rheology
     float cfl = 0.0f;                         // --cfl C: CFL-adaptive substeps, --dt of simulated time per frame (0: off)
     float dtMin = 0.0f;                       // --dt-min X: their smallest dt (0: dt / 64)
     int bullets = 0;                          // test aid: this many top-layer particles start at ~3 cell planes per step
     int ranks = 1, rank = -1;                 // --ranks N: SlabSPHSystem on N GPUs; --rank R: this process is rank R
     std::string rendezvous;
 };
+
+// --rheology MODEL:a,b,c[,d] -> the model (not yet checked against its ranges: setRheology does that)
+bool rheology_of(const Options& o, sphb200::Rheology& r) {
+    const std::string& spec = o.rheology;
+    const size_t colon = spec.find(':');
+    if (colon == std::string::npos) return false;
+    const std::string model = spec.substr(0, colon);
+    std::vector<float> v;
+    size_t at = colon + 1;
+    while (at <= spec.size()) {
+        const size_t comma = std::min(spec.find(',', at), spec.size());
+        const std::string item = spec.substr(at, comma - at);
+        char* end = nullptr;
+        const float x = std::strtof(item.c_str(), &end);
+        if (item.empty() || *end != '\0' || !std::isfinite(x)) return false;
+        v.push_back(x);
+        at = comma + 1;
+    }
+    const float nuMax = o.rheologyMax;
+    if (model == "cross" && v.size() == 4) {
+        r = sphb200::Rheology::cross(v[0], v[1], v[2], v[3], nuMax >= 0.0f ? nuMax : std::max(v[0], v[1]));
+    } else if (model == "hb" && (v.size() == 3 || v.size() == 4)) {
+        r = sphb200::Rheology::herschelBulkley(v[0], v[1], v[2], v.size() == 4 ? v[3] : 1000.0f, nuMax >= 0.0f ? nuMax : 1.0f);
+    } else {
+        return false;
+    }
+    return std::isfinite(o.rheologyMax);
+}
 
 bool parse(int argc, char** argv, Options& o) {
     auto need = [&](int i, int k) { return i + k < argc; };
@@ -116,6 +153,9 @@ bool parse(int argc, char** argv, Options& o) {
         else if (a == "--tap" && need(i, 1)) o.tap = static_cast<float>(std::atof(argv[++i]));
         else if (a == "--drain" && need(i, 1)) o.drain = static_cast<float>(std::atof(argv[++i]));
         else if (a == "--capacity" && need(i, 1)) o.capacity = std::atoll(argv[++i]);
+        else if (a == "--rheology" && need(i, 1)) o.rheology = argv[++i];
+        else if (a == "--rheology-max" && need(i, 1)) o.rheologyMax = static_cast<float>(std::atof(argv[++i]));
+        else if (a == "--no-slip") o.noSlip = true;
         else if (a == "--cfl" && need(i, 1)) o.cfl = static_cast<float>(std::atof(argv[++i]));
         else if (a == "--dt-min" && need(i, 1)) o.dtMin = static_cast<float>(std::atof(argv[++i]));
         else if (a == "--ranks" && need(i, 1)) o.ranks = std::atoi(argv[++i]);
@@ -161,6 +201,21 @@ bool parse(int argc, char** argv, Options& o) {
     }
     if ((o.tap > 0.0f || o.drain > 0.0f) && o.ranks > 1) {
         std::fprintf(stderr, "sph_headless: --tap and --drain run on one GPU only (open boundaries are not supported with --ranks)\n");
+        return false;
+    }
+    if (!o.rheology.empty()) {
+        sphb200::Rheology r;
+        if (!rheology_of(o, r)) {
+            std::fprintf(stderr, "sph_headless: --rheology needs cross:NU0,NUINF,LAMBDA,M or hb:K,N,TAU[,MREG] with finite values\n");
+            return false;
+        }
+        if (o.ranks > 1 || o.implicitNu > 0.0f || (o.noSlip && o.floating)) {
+            std::fprintf(stderr, "sph_headless: --rheology runs on one GPU only (not with --ranks), not together with --implicit-viscosity, "
+                                 "and --no-slip not together with --float\n");
+            return false;
+        }
+    } else if (o.noSlip || o.rheologyMax >= 0.0f) {
+        std::fprintf(stderr, "sph_headless: --no-slip and --rheology-max go with --rheology\n");
         return false;
     }
     if (!(o.cfl >= 0.0f) || !std::isfinite(o.cfl) || !(o.dtMin >= 0.0f) || !std::isfinite(o.dtMin)) {
@@ -332,7 +387,8 @@ int main(int argc, char** argv) {
     if (!parse(argc, argv, o)) {
         std::fprintf(stderr, "usage: sph_headless [--solver sph|dfsph|pbd] [--frames N] [--box L | LX LY LZ] [--block NX NY NZ] "
                              "[--origin X Y Z] [--dt DT] [--iters K] [--vorticity EPS] [--implicit-viscosity NU] [--stir OMEGA | --float REL] "
-                             "[--tap SPEED] [--drain SIDE] [--capacity N] [--cfl C [--dt-min X]] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] "
+                             "[--tap SPEED] [--drain SIDE] [--capacity N] [--cfl C [--dt-min X]] [--rheology cross:NU0,NUINF,LAMBDA,M | hb:K,N,TAU[,MREG] "
+                             "[--rheology-max NU_MAX] [--no-slip]] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] "
                              "[--ranks N [--rank R --rendezvous DIR]]\n");
         return 2;
     }
@@ -474,6 +530,14 @@ int main(int argc, char** argv) {
 
     if (o.vorticity > 0.0f) basicSolver->setVorticityConfinement(o.vorticity);
     if (o.implicitNu > 0.0f) basicSolver->setImplicitViscosity(o.implicitNu, o.implicitNu);
+    if (!o.rheology.empty()) {
+        sphb200::Rheology r;
+        rheology_of(o, r);
+        if (!basicSolver->setRheology(r, o.noSlip ? 1.0f : 0.0f)) {
+            std::fprintf(stderr, "sph_headless: --rheology %s was refused\n", o.rheology.c_str());
+            return 4;
+        }
+    }
     if (o.cfl > 0.0f && !pSystem->setAdaptiveTimeStep(o.cfl, o.dtMin)) {
         std::fprintf(stderr, "sph_headless: --cfl %g --dt-min %g was refused\n", o.cfl, o.dtMin);
         return 4;
@@ -515,6 +579,11 @@ int main(int argc, char** argv) {
         if (slab && o.bullets > 0) straysRouted += pSlab->straysRouted();
         totalTime += milliseconds;
         worst = milliseconds > worst ? milliseconds : worst;
+        if (!o.quiet && !o.rheology.empty()) {
+            const sphb200::RheologyStats rs = basicSolver->lastRheologyStats();
+            std::printf("Frame %d rheology - %d iterations, residual %.3g, max shear rate %g 1/s, %d particles at nu_max\n", frameId,
+                        rs.iterations, rs.residual, rs.gammaMax, rs.atNuMax);
+        }
         if (!o.quiet)
             std::printf("Frame %d - %2.2f ms, avg time - %2.2f ms/frame (%3.2f FPS)\r", frameId % 10000, milliseconds,
                         totalTime / float(frameId), float(frameId) * 1000.0f / totalTime);

@@ -37,6 +37,8 @@ SPHK_FUNCTIONS = [
     "sphk_visc_implicit_matvec",
     "sphk_emitter_axes", "sphk_emitter_advance", "sphk_emit", "sphk_sinks_apply", "sphk_sinks_removed", "sphk_fluid_set_count",
     "sphk_open_check", "sphk_time_step", "sphk_step_speed", "sphk_step_speed_result",
+    "sphk_rheology_work_floats", "sphk_non_newtonian_viscosity", "sphk_non_newtonian_stats", "sphk_shear_rate", "sphk_rheology_eval",
+    "sphk_visc_field_setup", "sphk_visc_field_matvec",
 ]
 SPH_APP_FUNCTIONS = [
     "sph_app_create", "sph_app_destroy", "sph_app_step", "sph_app_fluid_size", "sph_app_boundary_size",
@@ -45,8 +47,44 @@ SPH_APP_FUNCTIONS = [
     "sph_app_create_with_bodies", "sph_app_set_body_motion", "sph_app_body_pose", "sph_app_step_graph_active",
     "sph_app_create_with_dynamic_bodies", "sph_app_body_motion", "sph_app_body_impulse", "sph_app_set_implicit_viscosity",
     "sph_app_viscosity_stats", "sph_app_create_open", "sph_app_open_boundary_stats", "sph_app_set_adaptive_dt", "sph_app_advance",
-    "sph_app_adaptive_stats",
+    "sph_app_adaptive_stats", "sph_app_set_rheology", "sph_app_rheology_stats", "sph_app_download_viscosity",
 ]
+
+RHEOLOGY_CROSS, RHEOLOGY_HERSCHEL_BULKLEY = 1, 2   # SPHK_RHEOLOGY_* of sphk.h
+
+
+class Rheology(C.Structure):
+    """sphk_rheology of sphk.h"""
+    _fields_ = [("model", C.c_int), ("params", C.c_float * 6), ("nu_min", C.c_float), ("nu_max", C.c_float)]
+
+
+# the solve's settings of a rheology dict, beside the model's own keys
+RHEOLOGY_SOLVE_DEFAULTS = {"beta": 0.0, "tol": 1e-4, "max_iter": 20}
+
+
+def rheology(spec: dict) -> Rheology:
+    """sphk_rheology from dict(model="cross", nu0, nu_inf, lam, m, nu_max[, nu_min]) or dict(model="hb", k, n, tau_y[, m_reg = 1000],
+    nu_max[, nu_min]) (the solve's keys beta, tol and max_iter are ignored here).  Unknown models and keys raise ValueError; the
+    ranges are checked by the library."""
+    keys = {"cross": ("nu0", "nu_inf", "lam", "m"), "hb": ("k", "n", "tau_y", "m_reg")}
+    model = spec.get("model")
+    if model not in keys:
+        raise ValueError(f"rheology model must be 'cross' or 'hb' (got {model!r})")
+    extra = set(spec) - set(keys[model]) - {"model", "nu_min", "nu_max"} - set(RHEOLOGY_SOLVE_DEFAULTS)
+    if extra:
+        raise ValueError(f"unknown rheology keys {sorted(extra)}")
+    r = Rheology()
+    r.model = RHEOLOGY_CROSS if model == "cross" else RHEOLOGY_HERSCHEL_BULKLEY
+    defaults = {"m_reg": 1000.0}
+    for k, name in enumerate(keys[model]):
+        if name not in spec and name not in defaults:
+            raise ValueError(f"rheology {model!r} needs {name!r}")
+        r.params[k] = float(spec.get(name, defaults.get(name, 0.0)))
+    if "nu_max" not in spec:
+        raise ValueError("rheology needs a finite nu_max")
+    r.nu_min, r.nu_max = float(spec.get("nu_min", 0.0)), float(spec["nu_max"])
+    return r
+
 
 OPT_NEIGHBOR_LIST, OPT_LIST_CAPACITY, OPT_LIST_SKIN, OPT_SIMPLE_LIST_BUILD, OPT_TILE, OPT_STAGED_LIST_BUILD, OPT_PATCH = 1, 2, 5, 6, 9, 10, 11
 MAX_EMITTERS, MAX_SINKS = 16, 16   # SPHK_MAX_EMITTERS, SPHK_MAX_SINKS
@@ -133,6 +171,7 @@ def sphk():
         L.sphk_scene_boundary_count.restype = C.c_longlong
         L.sphk_strays_block_floats.restype = C.c_longlong
         L.sphk_implicit_viscosity_work_floats.restype = C.c_longlong
+        L.sphk_rheology_work_floats.restype = C.c_longlong
         L.sphk_destroy.restype = None
         L.sphk_mg_destroy.restype = None
         _sphk = L
@@ -315,6 +354,34 @@ class SphApp:
         if self.L.sph_app_viscosity_stats(self.h, C.byref(it), C.byref(res)):
             raise RuntimeError("sph_app_viscosity_stats failed (reference engine)")
         return int(it.value), float(res.value)
+
+    def set_rheology(self, spec):
+        """Non-Newtonian viscosity in every following step instead of the constant-nu solve (spec: a dict for capi.rheology plus
+        beta, tol, max_iter; None: off).  Not on the reference engine."""
+        if spec is None:
+            rc = self.L.sph_app_set_rheology(self.h, C.c_int(0), None, C.c_float(0), C.c_float(0), C.c_float(0), C.c_float(0), C.c_int(0))
+        else:
+            r = rheology(spec)
+            o = dict(RHEOLOGY_SOLVE_DEFAULTS, **{k: spec[k] for k in RHEOLOGY_SOLVE_DEFAULTS if k in spec})
+            rc = self.L.sph_app_set_rheology(self.h, C.c_int(r.model), r.params, C.c_float(r.nu_min), C.c_float(r.nu_max),
+                                             C.c_float(o["beta"]), C.c_float(o["tol"]), C.c_int(int(o["max_iter"])))
+        if rc:
+            raise RuntimeError("sph_app_set_rheology failed (reference engine or a refused setting)")
+
+    def rheology_stats(self) -> dict:
+        """of the last non-Newtonian solve: iterations, residual, gamma_max, nu_min, nu_max, at_nu_max"""
+        it, res, g, lo, hi, k = C.c_int(0), C.c_float(0), C.c_float(0), C.c_float(0), C.c_float(0), C.c_int(0)
+        if self.L.sph_app_rheology_stats(self.h, C.byref(it), C.byref(res), C.byref(g), C.byref(lo), C.byref(hi), C.byref(k)):
+            raise RuntimeError("sph_app_rheology_stats failed (reference engine)")
+        return {"iterations": it.value, "residual": res.value, "gamma_max": g.value, "nu_min": lo.value, "nu_max": hi.value,
+                "at_nu_max": k.value}
+
+    def download_viscosity(self) -> np.ndarray:
+        """nu_i of the last non-Newtonian solve (float32[fluid size])"""
+        out = np.zeros(int(self.L.sph_app_fluid_size(self.h)), np.float32)
+        if self.L.sph_app_download_viscosity(self.h, out.ctypes.data_as(C.c_void_p)):
+            raise RuntimeError("sph_app_download_viscosity failed (reference engine)")
+        return out
 
     def set_body_motion(self, body: int, linear_velocity, angular_velocity):
         """New motion of one kinematic body from the next step on.  Not on the reference engine."""

@@ -130,6 +130,8 @@ struct sphk_ctx {
     long long launches = 0;
     BodyState* bodies = nullptr;     // non-null after sphk_bodies_init
     float* viscStats = nullptr;      // [2] device: {iterations (int bits), |r|_M / |b|_M} of the last sphk_implicit_viscosity
+    float* rheoStats = nullptr;      // [6] device: {iterations, |r|_M / |b|_M, max gamma_dot, min nu, max nu, count at nu_max} of the
+                                     // last sphk_non_newtonian_viscosity (uint bits; the shear statistics also of sphk_shear_rate)
     // open boundaries (sphk_sinks_apply / sphk_fluid_set_count; allocated on first use)
     int* openDev = nullptr;          // device [2]: {particles the last sphk_sinks_apply removed, sticky check bits}
     int* openPinned = nullptr;       // pinned [1]: the removed count, copied behind the sink kernel

@@ -23,6 +23,8 @@
 #include <cstdlib>
 #include <cstring>
 #include <type_traits>
+#include <cooperative_groups.h>
+#include <cooperative_groups/reduce.h>
 #include "sphk_internal.cuh"
 
 // =================================================================================================
@@ -429,6 +431,151 @@ struct OpViscImplicitMatvec {
     __device__ void begin(Acc& a, int, float4, float4, const DevScene&) const { a.a = f3(0, 0, 0); }
     __device__ void pair(Acc& a, int, int, bool, float3 d, float r2, float mj, float4, float4 hi, const DevScene& s) const {
         a.a += (visc_coef(mj * nuRho, r2, s.k) * dot3(d, xyz(hi))) * d;
+    }
+    __device__ void end(Acc& a, int i, float4, float4 hi, const DevScene&) const {
+        store3(Ap, i, sym_apply(D, i, xyz(hi)) - dt * a.a);
+    }
+};
+
+// ---- non-Newtonian viscosity (no reference counterpart; DESIGN.md section 2.9) ----------------------------------------------
+// float <-> double without flushing subnormals (-use_fast_math makes the plain conversions flush them to zero)
+__device__ __forceinline__ double f2d(float x) { double d; asm("cvt.f64.f32 %0, %1;" : "=d"(d) : "f"(x)); return d; }
+__device__ __forceinline__ float d2f_rn(double x) { float f; asm("cvt.rn.f32.f64 %0, %1;" : "=f"(f) : "d"(x)); return f; }
+
+// The viscosity model nu(gamma_dot) in double, clamped to [nu_min, nu_max] (a NaN shear rate lands on nu_max); *atMax: the
+// clamp at nu_max bound (the unyielded part of a yield-stress fluid).
+__device__ __forceinline__ double rheo_nu(const sphk_rheology& r, double g, bool* atMax) {
+    double raw;
+    if (r.model == SPHK_RHEOLOGY_CROSS) {
+        const double nu0 = r.params[0], nuInf = r.params[1], lam = r.params[2], m = r.params[3];
+        raw = nuInf + (nu0 - nuInf) / (1.0 + pow(lam * g, m));
+    } else {                                   // Herschel-Bulkley, Papanastasiou-regularised
+        const double K = r.params[0], n = r.params[1], tau = r.params[2], mr = r.params[3];
+        const double power = K > 0.0 ? K * pow(g, n - 1.0) : 0.0;
+        const double yield = g > 0.0 ? tau * (-expm1(-mr * g) / g) : tau * mr;
+        raw = power + yield;
+    }
+    const double hi = r.nu_max, lo = r.nu_min;
+    *atMax = !(raw < hi);
+    return *atMax ? hi : fmax(raw, lo);
+}
+
+// Statistics of one shear sweep in the context's memory, as uint bits of non-negative floats (so atomicMax / atomicMin order them):
+// {.., .., max gamma_dot, min nu, max nu, particles at the nu_max clamp}; slots 0 and 1 take the solve's iterations and residual.
+#define SPHK_RHEO_STATS 6
+__device__ __forceinline__ void rheo_fold_stats(unsigned int* st, float gd, float nu, bool atMax) {
+    namespace cg = cooperative_groups;
+    const cg::coalesced_group g = cg::coalesced_threads();
+    const unsigned int gmax = cg::reduce(g, __float_as_uint(gd), cg::greater<unsigned int>());
+    const unsigned int nmin = cg::reduce(g, __float_as_uint(nu), cg::less<unsigned int>());
+    const unsigned int nmax = cg::reduce(g, __float_as_uint(nu), cg::greater<unsigned int>());
+    const unsigned int cnt = __popc(g.ballot(atMax));
+    if (g.thread_rank() == 0) {
+        atomicMax(st + 2, gmax); atomicMin(st + 3, nmin); atomicMax(st + 4, nmax);
+        if (cnt) atomicAdd(st + 5, cnt);
+    }
+}
+
+// Shear rate (Monaghan-style corrected gradient): with u = v_j - v_i, gradW = g d, V_j = m_j / rho0 (a boundary neighbour:
+// m_b / rho_B and the record's velocity, counted only when beta > 0)
+//   G_i = sum_j V_j u (x) gradW        M_i = -sum_j V_j g d d^T  (symmetric, {xx, yy, zz, xy, xz, yz})
+//   grad v_i = G_i M_i^-1, or G_i 3 / tr M_i where det M_i < theta (tr M_i / 3)^3 (few neighbours or one-sided support)
+//   gamma_dot_i = sqrt(2 E:E),  E = (grad v + grad v^T) / 2
+// A linear field v = A x + b gives G = A M, so the corrected gradient is A exactly.  The epilogue works in double, evaluates the
+// model, writes gamma_dot and nu_i (+ the 9-float gradient, row-major d v_a / d x_b, and the fallback flag for tests) and folds the
+// statistics.
+#define SPHK_RHEO_THETA 0.01
+struct OpShearRate {
+    float* gamma; float* nu; float* grad; int* flag; unsigned int* stats; sphk_rheology rh; float invRho0, invRhoB; bool wall;
+    static constexpr bool kFluidOnly = false, kHi = true;
+    struct Acc {
+        float G[9]; float M[6]; float3 vi;
+        template <class F> __device__ void sums(F f) { for (int k = 0; k < 9; ++k) f(G[k]); for (int k = 0; k < 6; ++k) f(M[k]); }
+    };
+    __device__ void begin(Acc& a, int, float4, float4 hi, const DevScene&) const {
+        for (int k = 0; k < 9; ++k) a.G[k] = 0.f;
+        for (int k = 0; k < 6; ++k) a.M[k] = 0.f;
+        a.vi = xyz(hi);
+    }
+    __device__ void pair(Acc& a, int, int, bool isB, float3 d, float r2, float mj, float4, float4 hi, const DevScene& s) const {
+        if (isB && !wall) return;
+        const float Vg = mj * (isB ? invRhoB : invRho0) * grad_w_factor(sqrtf(r2), s.k);
+        const float3 u = xyz(hi) - a.vi, w = Vg * d;          // V_j gradW
+        a.G[0] += u.x * w.x; a.G[1] += u.x * w.y; a.G[2] += u.x * w.z;
+        a.G[3] += u.y * w.x; a.G[4] += u.y * w.y; a.G[5] += u.y * w.z;
+        a.G[6] += u.z * w.x; a.G[7] += u.z * w.y; a.G[8] += u.z * w.z;
+        a.M[0] -= w.x * d.x; a.M[1] -= w.y * d.y; a.M[2] -= w.z * d.z;
+        a.M[3] -= w.x * d.y; a.M[4] -= w.x * d.z; a.M[5] -= w.y * d.z;
+    }
+    __device__ void end(Acc& a, int i, float4, float4, const DevScene&) const {
+        const double m0 = f2d(a.M[0]), m1 = f2d(a.M[1]), m2 = f2d(a.M[2]), m3 = f2d(a.M[3]), m4 = f2d(a.M[4]), m5 = f2d(a.M[5]);
+        const double tr = m0 + m1 + m2;
+        const double c00 = m1 * m2 - m5 * m5, c11 = m0 * m2 - m4 * m4, c22 = m0 * m1 - m3 * m3;
+        const double c01 = m4 * m5 - m3 * m2, c02 = m3 * m5 - m1 * m4, c12 = m3 * m4 - m0 * m5;
+        const double det = m0 * c00 + m3 * c01 + m4 * c02;
+        const double t3 = tr / 3.0;
+        const bool corrected = tr > 0.0 && det >= SPHK_RHEO_THETA * t3 * t3 * t3;
+        double inv[9];
+        if (corrected) {
+            const double q = 1.0 / det;
+            inv[0] = c00 * q; inv[1] = c01 * q; inv[2] = c02 * q;
+            inv[3] = c01 * q; inv[4] = c11 * q; inv[5] = c12 * q;
+            inv[6] = c02 * q; inv[7] = c12 * q; inv[8] = c22 * q;
+        } else {
+            const double q = tr > 0.0 ? 1.0 / t3 : 0.0;
+            for (int k = 0; k < 9; ++k) inv[k] = (k % 4 == 0) ? q : 0.0;
+        }
+        double L[9];
+        for (int r = 0; r < 3; ++r)
+            for (int col = 0; col < 3; ++col)
+                L[3 * r + col] = f2d(a.G[3 * r]) * inv[col] + f2d(a.G[3 * r + 1]) * inv[3 + col] + f2d(a.G[3 * r + 2]) * inv[6 + col];
+        double ee = 0.0;
+        for (int r = 0; r < 3; ++r)
+            for (int col = 0; col < 3; ++col) {
+                const double e = 0.5 * (L[3 * r + col] + L[3 * col + r]);
+                ee += e * e;
+            }
+        const double gd = sqrt(2.0 * ee);
+        bool atMax;
+        const float gf = d2f_rn(gd), nf = d2f_rn(rheo_nu(rh, gd, &atMax));
+        gamma[i] = gf;
+        nu[i] = nf;
+        if (grad) for (int k = 0; k < 9; ++k) grad[9 * static_cast<size_t>(i) + k] = d2f_rn(L[k]);
+        if (flag) flag[i] = corrected ? 0 : 1;
+        rheo_fold_stats(stats, gf, nf, atMax);
+    }
+};
+
+// The implicit viscosity sweeps with a per-particle viscosity: rec.s = nu_i / rho0 (mirrored by the entry, k_rheo_mirror), a
+// fluid pair takes the mean nu_ij V_j = (s_i + s_j) / 2 m_j (so m_i c_ij = m_j c_ji: A stays self-adjoint in the mass inner
+// product), a boundary pair beta nu_i m_b / rho_B.  With nu_i = nu everywhere and beta = 1 every coefficient is the one the
+// constant-nu sweeps form (the same float operations on the same values).
+struct OpViscImplicitSetupField {
+    OpViscImplicitSetup base; const float* nuField; float beta, rhoB;
+    static constexpr bool kFluidOnly = false, kHi = true;
+    struct Acc : OpViscImplicitSetup::Acc { float si, sb; };
+    __device__ void begin(Acc& a, int i, float4 lo, float4 hi, const DevScene& s) const {
+        base.begin(a, i, lo, hi, s);
+        a.si = lo.w;
+        a.sb = __fdiv_rn(beta * nuField[i], rhoB);
+    }
+    __device__ void pair(Acc& a, int, int, bool isB, float3 d, float r2, float mj, float4 lo, float4 hi, const DevScene& s) const {
+        const float c = visc_coef(mj * (isB ? a.sb : 0.5f * (a.si + lo.w)), r2, s.k);
+        const float3 cd = c * d;
+        a.s[0] += cd.x * d.x; a.s[1] += cd.y * d.y; a.s[2] += cd.z * d.z;
+        a.s[3] += cd.x * d.y; a.s[4] += cd.x * d.z; a.s[5] += cd.y * d.z;
+        if (isB) a.bb += dot3(d, xyz(hi)) * cd;
+    }
+    __device__ void end(Acc& a, int i, float4 lo, float4 hi, const DevScene& s) const { base.end(a, i, lo, hi, s); }
+};
+
+struct OpViscImplicitMatvecField {
+    const float* D; float* Ap; float dt;
+    static constexpr bool kFluidOnly = true, kHi = true;
+    struct Acc : OpViscImplicitMatvec::Acc { float si; };
+    __device__ void begin(Acc& a, int, float4 lo, float4, const DevScene&) const { a.a = f3(0, 0, 0); a.si = lo.w; }
+    __device__ void pair(Acc& a, int, int, bool, float3 d, float r2, float mj, float4 lo, float4 hi, const DevScene& s) const {
+        a.a += (visc_coef(mj * (0.5f * (a.si + lo.w)), r2, s.k) * dot3(d, xyz(hi))) * d;
     }
     __device__ void end(Acc& a, int i, float4, float4 hi, const DevScene&) const {
         store3(Ap, i, sym_apply(D, i, xyz(hi)) - dt * a.a);
@@ -1860,6 +2007,50 @@ extern "C" long long sphk_implicit_viscosity_work_floats(int n) {
     return SPHK_VISC_HEAD + 2LL * 3 * SPHK_VISC_PARTS + 21LL * n;
 }
 
+struct ViscWork {
+    ViscCg* st; double* part; float *D, *Dinv, *r, *z, *Ap;
+};
+static ViscWork visc_work(float* work, int n) {
+    ViscWork w;
+    w.st = reinterpret_cast<ViscCg*>(work);
+    w.part = reinterpret_cast<double*>(work + SPHK_VISC_HEAD);
+    w.D = work + SPHK_VISC_HEAD + 2 * 3 * SPHK_VISC_PARTS;
+    w.Dinv = w.D + 6LL * n; w.r = w.Dinv + 6LL * n; w.z = w.r + 3LL * n; w.Ap = w.z + 3LL * n;
+    return w;
+}
+
+// The solve after its setup sweep (b in r, D and Dinv formed) with the matvec sweep `mv`: r = b - A v*, then max_iter PCG
+// iterations under the device-side loop test; the outcome {iterations, |r|_M / |b|_M} goes to `report` (context memory).
+template <class Mv>
+static int visc_pcg(sphk_ctx* c, const sphk_scene* s, const ViscWork& w, const Mv& mv, float tol, int max_iter, float* report) {
+    const int n = c->nF;
+    float* vel = s->fluid.vel;
+    int rc = run_sweep(c, s, mv);                                                                // A v*
+    if (rc != SPHK_OK) return rc;
+    const int m = visc_blocks(n);
+    k_visc_init<<<m, SPHK_VISC_RED, 0, c->stream>>>(c->rec, vel, w.r, w.Ap, w.Dinv, w.z, n, w.part);
+    k_visc_init_finish<<<1, SPHK_VISC_RED, 0, c->stream>>>(w.st, w.part, m, static_cast<double>(tol) * tol, max_iter);
+    c->launches += 2;
+    const int* outer = c->pred;
+    c->pred = &w.st->active;
+    for (int k = 0; k < max_iter && rc == SPHK_OK; ++k) {
+        rc = run_sweep(c, s, mv);
+        k_visc_alpha_partial<<<m, SPHK_VISC_RED, 0, c->stream>>>(w.st, c->rec, w.Ap, n, w.part);
+        k_visc_alpha_finish<<<1, SPHK_VISC_RED, 0, c->stream>>>(w.st, w.part, m);
+        k_visc_update<<<m, SPHK_VISC_RED, 0, c->stream>>>(w.st, c->rec, vel, w.r, w.Ap, w.Dinv, w.z, n, w.part);
+        k_visc_beta_finish<<<1, SPHK_VISC_RED, 0, c->stream>>>(w.st, w.part, m);
+        k_visc_direction<<<m, SPHK_VISC_RED, 0, c->stream>>>(w.st, c->rec, w.z, n);
+        c->launches += 5;
+    }
+    c->pred = outer;
+    if (n > 0) { k_visc_set_rec_vel<<<sphk_blocks(n), SPHK_BLOCK, 0, c->stream>>>(c->rec, vel, n); c->launches++; }   // records <- x
+    k_visc_report<<<1, 1, 0, c->stream>>>(w.st, report);
+    c->launches++;
+    if (rc != SPHK_OK) return rc;
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
 extern "C" int sphk_implicit_viscosity(sphk_ctx* c, const sphk_scene* s, float* work, float nu, float nu_boundary, float dt, float rho0,
                                        float rho_boundary, float tol, int max_iter) {
     SPHK_CHECK_SCENE(c, s);
@@ -1870,40 +2061,11 @@ extern "C" int sphk_implicit_viscosity(sphk_ctx* c, const sphk_scene* s, float* 
     if (rc0 != SPHK_OK) return rc0;
     // the viscous force on a dynamic body is not part of its reaction (sphk_bodies_react): the momentum would not balance
     if (nu_boundary > 0.f && c->bodies && c->bodies->acc) return SPHK_ERR_STATE;
-    const int n = c->nF;
-    ViscCg* st = reinterpret_cast<ViscCg*>(work);
-    double* part = reinterpret_cast<double*>(work + SPHK_VISC_HEAD);
-    float* D = work + SPHK_VISC_HEAD + 2 * 3 * SPHK_VISC_PARTS;
-    float *Dinv = D + 6LL * n, *r = Dinv + 6LL * n, *z = r + 3LL * n, *Ap = z + 3LL * n;
+    const ViscWork w = visc_work(work, c->nF);
     const float nuRho = nu / rho0, nuBRho = nu_boundary / rho_boundary;
-    float* vel = s->fluid.vel;
-    int rc = run_sweep(c, s, OpViscImplicitSetup{D, Dinv, r, nuRho, nuBRho, dt});          // b -> r
+    const int rc = run_sweep(c, s, OpViscImplicitSetup{w.D, w.Dinv, w.r, nuRho, nuBRho, dt});          // b -> r
     if (rc != SPHK_OK) return rc;
-    const OpViscImplicitMatvec mv{D, Ap, nuRho, dt};
-    rc = run_sweep(c, s, mv);                                                                // A v*
-    if (rc != SPHK_OK) return rc;
-    const int m = visc_blocks(n);
-    k_visc_init<<<m, SPHK_VISC_RED, 0, c->stream>>>(c->rec, vel, r, Ap, Dinv, z, n, part);
-    k_visc_init_finish<<<1, SPHK_VISC_RED, 0, c->stream>>>(st, part, m, static_cast<double>(tol) * tol, max_iter);
-    c->launches += 2;
-    const int* outer = c->pred;
-    c->pred = &st->active;
-    for (int k = 0; k < max_iter && rc == SPHK_OK; ++k) {
-        rc = run_sweep(c, s, mv);
-        k_visc_alpha_partial<<<m, SPHK_VISC_RED, 0, c->stream>>>(st, c->rec, Ap, n, part);
-        k_visc_alpha_finish<<<1, SPHK_VISC_RED, 0, c->stream>>>(st, part, m);
-        k_visc_update<<<m, SPHK_VISC_RED, 0, c->stream>>>(st, c->rec, vel, r, Ap, Dinv, z, n, part);
-        k_visc_beta_finish<<<1, SPHK_VISC_RED, 0, c->stream>>>(st, part, m);
-        k_visc_direction<<<m, SPHK_VISC_RED, 0, c->stream>>>(st, c->rec, z, n);
-        c->launches += 5;
-    }
-    c->pred = outer;
-    if (n > 0) { k_visc_set_rec_vel<<<sphk_blocks(n), SPHK_BLOCK, 0, c->stream>>>(c->rec, vel, n); c->launches++; }   // records <- x
-    k_visc_report<<<1, 1, 0, c->stream>>>(st, c->viscStats);
-    c->launches++;
-    if (rc != SPHK_OK) return rc;
-    SPHK_CUDA_TRY(cudaGetLastError());
-    return SPHK_OK;
+    return visc_pcg(c, s, w, OpViscImplicitMatvec{w.D, w.Ap, nuRho, dt}, tol, max_iter, c->viscStats);
 }
 
 extern "C" int sphk_implicit_viscosity_stats(sphk_ctx* c, int* iterations, float* rel_residual) {
@@ -1936,6 +2098,152 @@ extern "C" int sphk_visc_implicit_matvec(sphk_ctx* c, const sphk_scene* s, const
     const int n = c->nF;
     if (n > 0) k_visc_set_rec_vel<<<sphk_blocks(n), SPHK_BLOCK, 0, c->stream>>>(c->rec, p_in, n);
     const int rc = run_sweep(c, s, OpViscImplicitMatvec{d_in, ap_out, nu / rho0, dt});
+    if (n > 0) k_visc_set_rec_vel<<<sphk_blocks(n), SPHK_BLOCK, 0, c->stream>>>(c->rec, s->fluid.vel, n);   // records <- API velocities
+    if (n > 0) c->launches += 2;
+    if (rc != SPHK_OK) return rc;
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+// ---- non-Newtonian viscosity (DESIGN.md section 2.9) ------------------------------------------------------------------------
+// rec.s <- nu_i / rho0 (correctly rounded: with a uniform nu it is the constant-nu solve's nu / rho0, bit for bit).  rec.s then
+// mirrors no caller array: sTag = nullptr, so every later sweep that gathers a scalar re-mirrors or rewrites it first.
+__global__ void __launch_bounds__(SPHK_BLOCK) k_rheo_mirror(const float* __restrict__ nu, Rec rec, int n, float rho0) {
+    const int i = blockIdx.x * SPHK_BLOCK + threadIdx.x;
+    if (i < n) rec_set_s(rec + i, __fdiv_rn(nu[i], rho0));
+}
+__global__ void k_rheo_stats_reset(unsigned int* st) {
+    st[2] = 0u; st[3] = 0x7f800000u; st[4] = 0u; st[5] = 0u;      // (min nu starts at +inf)
+}
+__global__ void __launch_bounds__(SPHK_BLOCK) k_rheo_eval(sphk_rheology rh, const float* __restrict__ g, float* __restrict__ nu, int n) {
+    const int i = blockIdx.x * SPHK_BLOCK + threadIdx.x;
+    if (i >= n) return;
+    bool atMax;
+    nu[i] = d2f_rn(rheo_nu(rh, f2d(g[i]), &atMax));
+}
+
+static bool finite_f(float x) { return x - x == 0.f; }
+static int check_rheology(const sphk_rheology* r) {
+    if (!r) return SPHK_ERR_INVALID;
+    for (int k = 0; k < 6; ++k) if (!finite_f(r->params[k])) return SPHK_ERR_INVALID;
+    if (!finite_nonneg(r->nu_min) || !finite_nonneg(r->nu_max) || r->nu_min > r->nu_max) return SPHK_ERR_INVALID;
+    const float* p = r->params;
+    if (r->model == SPHK_RHEOLOGY_CROSS) {                  // nu0, nu_inf, lambda >= 0, m > 0
+        if (!(p[0] >= 0.f && p[1] >= 0.f && p[2] >= 0.f && p[3] > 0.f)) return SPHK_ERR_INVALID;
+    } else if (r->model == SPHK_RHEOLOGY_HERSCHEL_BULKLEY) { // K >= 0, n > 0, tau_y >= 0, m_reg >= 0
+        if (!(p[0] >= 0.f && p[1] > 0.f && p[2] >= 0.f && p[3] >= 0.f)) return SPHK_ERR_INVALID;
+    } else {
+        return SPHK_ERR_INVALID;
+    }
+    return SPHK_OK;
+}
+static unsigned int* rheo_stats(sphk_ctx* c) { return reinterpret_cast<unsigned int*>(c->rheoStats); }
+
+// the shear sweep: statistics reset, then gamma_dot and nu (+ gradient and flag) of every particle
+static int shear_sweep(sphk_ctx* c, const sphk_scene* s, float* gamma, float* nu, float* grad, int* flag, const sphk_rheology& rh,
+                       float beta, float rho0, float rho_boundary) {
+    k_rheo_stats_reset<<<1, 1, 0, c->stream>>>(rheo_stats(c));
+    c->launches++;
+    return run_sweep(c, s, OpShearRate{gamma, nu, grad, flag, rheo_stats(c), rh, 1.0f / rho0, 1.0f / rho_boundary, beta > 0.f});
+}
+static void rheo_mirror(sphk_ctx* c, const float* nu, float rho0) {
+    if (c->nF > 0) { k_rheo_mirror<<<sphk_blocks(c->nF), SPHK_BLOCK, 0, c->stream>>>(nu, c->rec, c->nF, rho0); c->launches++; }
+    c->sTag = nullptr;
+}
+static int check_field_common(sphk_ctx* c, float beta, float dt, float rho0, float rho_boundary) {
+    if (!finite_nonneg(beta) || !(rho_boundary > 0.f)) return SPHK_ERR_INVALID;
+    const int rc = check_visc(c, 0.0f, dt, rho0);
+    if (rc != SPHK_OK) return rc;
+    // the viscous force on a dynamic body is not part of its reaction (sphk_bodies_react): the momentum would not balance
+    if (beta > 0.f && c->bodies && c->bodies->acc) return SPHK_ERR_STATE;
+    return SPHK_OK;
+}
+
+extern "C" long long sphk_rheology_work_floats(int n) {
+    if (n < 0) return -1;
+    return sphk_implicit_viscosity_work_floats(n) + n;          // + gamma_dot
+}
+
+extern "C" int sphk_non_newtonian_viscosity(sphk_ctx* c, const sphk_scene* s, float* work, float* nu_field, const sphk_rheology* rheology,
+                                            float beta, float dt, float rho0, float rho_boundary, float tol, int max_iter) {
+    SPHK_CHECK_SCENE(c, s);
+    if (!work || !nu_field || work == nu_field || aliases(work, s) || aliases(nu_field, s) || !(tol > 0.f) || max_iter < 1 ||
+        max_iter > SPHK_IMPLICIT_VISCOSITY_MAX_ITER || check_rheology(rheology) != SPHK_OK)
+        return SPHK_ERR_INVALID;
+    const int rc0 = check_field_common(c, beta, dt, rho0, rho_boundary);
+    if (rc0 != SPHK_OK) return rc0;
+    const int n = c->nF;
+    const ViscWork w = visc_work(work, n);
+    float* gamma = work + sphk_implicit_viscosity_work_floats(n);
+    int rc = shear_sweep(c, s, gamma, nu_field, nullptr, nullptr, *rheology, beta, rho0, rho_boundary);   // from v*
+    if (rc != SPHK_OK) return rc;
+    rheo_mirror(c, nu_field, rho0);
+    rc = run_sweep(c, s, OpViscImplicitSetupField{OpViscImplicitSetup{w.D, w.Dinv, w.r, 0.f, 0.f, dt}, nu_field, beta, rho_boundary});
+    if (rc != SPHK_OK) return rc;
+    return visc_pcg(c, s, w, OpViscImplicitMatvecField{w.D, w.Ap, dt}, tol, max_iter, c->rheoStats);
+}
+
+extern "C" int sphk_non_newtonian_stats(sphk_ctx* c, int* iterations, float* rel_residual, float* gamma_max, float* nu_min,
+                                        float* nu_max, int* n_at_max) {
+    if (!c) return SPHK_ERR_INVALID;
+    unsigned int h[SPHK_RHEO_STATS];
+    SPHK_CUDA_TRY(cudaMemcpyAsync(h, c->rheoStats, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
+    SPHK_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    float f[SPHK_RHEO_STATS];
+    memcpy(f, h, sizeof(h));
+    if (iterations) *iterations = static_cast<int>(h[0]);
+    if (rel_residual) *rel_residual = f[1];
+    if (gamma_max) *gamma_max = f[2];
+    if (nu_min) *nu_min = h[3] == 0x7f800000u ? 0.0f : f[3];     // (no fluid particle: 0)
+    if (nu_max) *nu_max = f[4];
+    if (n_at_max) *n_at_max = static_cast<int>(h[5]);
+    return SPHK_OK;
+}
+
+extern "C" int sphk_shear_rate(sphk_ctx* c, const sphk_scene* s, float* gamma_out, float* nu_out, float* grad_out_or_null,
+                               int* flag_out_or_null, const sphk_rheology* rheology, float beta, float rho0, float rho_boundary) {
+    SPHK_CHECK_SCENE(c, s);
+    if (!gamma_out || !nu_out || gamma_out == nu_out || aliases(gamma_out, s) || aliases(nu_out, s) ||
+        (grad_out_or_null && (aliases(grad_out_or_null, s) || grad_out_or_null == gamma_out || grad_out_or_null == nu_out)) ||
+        check_rheology(rheology) != SPHK_OK)
+        return SPHK_ERR_INVALID;
+    const int rc = check_field_common(c, beta, 0.0f, rho0, rho_boundary);
+    if (rc != SPHK_OK) return rc;
+    if (c->sTag == nu_out) c->sTag = nullptr;
+    return shear_sweep(c, s, gamma_out, nu_out, grad_out_or_null, flag_out_or_null, *rheology, beta, rho0, rho_boundary);
+}
+
+extern "C" int sphk_rheology_eval(sphk_ctx* c, const sphk_rheology* rheology, const float* gamma, float* nu_out, int n) {
+    if (!c || !gamma || !nu_out || gamma == nu_out || n < 0 || check_rheology(rheology) != SPHK_OK) return SPHK_ERR_INVALID;
+    if (n == 0) return SPHK_OK;
+    k_rheo_eval<<<sphk_blocks(n), SPHK_BLOCK, 0, c->stream>>>(*rheology, gamma, nu_out, n);
+    c->launches++;
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+extern "C" int sphk_visc_field_setup(sphk_ctx* c, const sphk_scene* s, float* d_out, float* b_out, const float* nu, float beta,
+                                     float dt, float rho0, float rho_boundary) {
+    SPHK_CHECK_SCENE(c, s);
+    if (!d_out || !b_out || !nu || d_out == b_out || nu == d_out || nu == b_out || aliases(d_out, s) || aliases(b_out, s))
+        return SPHK_ERR_INVALID;
+    const int rc = check_field_common(c, beta, dt, rho0, rho_boundary);
+    if (rc != SPHK_OK) return rc;
+    rheo_mirror(c, nu, rho0);
+    return run_sweep(c, s, OpViscImplicitSetupField{OpViscImplicitSetup{d_out, nullptr, b_out, 0.f, 0.f, dt}, nu, beta, rho_boundary});
+}
+
+extern "C" int sphk_visc_field_matvec(sphk_ctx* c, const sphk_scene* s, const float* d_in, const float* p_in, float* ap_out,
+                                      const float* nu, float dt, float rho0) {
+    SPHK_CHECK_SCENE(c, s);
+    if (!d_in || !p_in || !ap_out || !nu || d_in == p_in || ap_out == d_in || ap_out == p_in || ap_out == nu || aliases(ap_out, s))
+        return SPHK_ERR_INVALID;
+    const int rc0 = check_field_common(c, 0.0f, dt, rho0, 1.0f);
+    if (rc0 != SPHK_OK) return rc0;
+    const int n = c->nF;
+    rheo_mirror(c, nu, rho0);
+    if (n > 0) k_visc_set_rec_vel<<<sphk_blocks(n), SPHK_BLOCK, 0, c->stream>>>(c->rec, p_in, n);
+    const int rc = run_sweep(c, s, OpViscImplicitMatvecField{d_in, ap_out, dt});
     if (n > 0) k_visc_set_rec_vel<<<sphk_blocks(n), SPHK_BLOCK, 0, c->stream>>>(c->rec, s->fluid.vel, n);   // records <- API velocities
     if (n > 0) c->launches += 2;
     if (rc != SPHK_OK) return rc;

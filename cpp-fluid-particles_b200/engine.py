@@ -84,6 +84,8 @@ class SphkOps:
     list_capacity = 96               # SPHK_OPT_LIST_CAPACITY of ctx (set_option keeps it current)
     vorticity_eps = 0.0              # vorticity confinement strength (BasicSPHSolver::setVorticityConfinement); 0: off
     implicit_nu = 0.0                # implicit viscosity (BasicSPHSolver::setImplicitViscosity); 0: off
+    rheology = None                  # non-Newtonian viscosity (BasicSPHSolver::setRheology): a dict for capi.rheology plus beta,
+                                     # tol, max_iter; replaces the implicit_nu solve.  None: off
     implicit_nu_boundary = 0.0
     implicit_tol = 1e-4
     implicit_max_iter = 20
@@ -384,6 +386,52 @@ class SphkOps:
         check(self.L.sphk_visc_implicit_matvec(self.ctx, self._s(), _ptr(d_in), _ptr(p_in), _ptr(ap_out), C.c_float(nu),
                                                C.c_float(self.dt), C.c_float(self.p.rho0)), "sphk_visc_implicit_matvec")
 
+    # ---- non-Newtonian viscosity (no reference counterpart; DESIGN.md section 2.9) ---------------------------------------
+    def _rheo_buffers(self):
+        if getattr(self, "rheo_work", None) is None:   # allocated on first use, like the class layer's
+            n = self.buffer3.shape[0]
+            self.rheo_work = torch.zeros(int(self.L.sphk_rheology_work_floats(C.c_int(n))), dtype=torch.float32, device=self.device)
+            self.nu_field = torch.zeros(n, dtype=torch.float32, device=self.device)
+        return _ptr(self.rheo_work), _ptr(self.nu_field)
+
+    def non_newtonian_viscosity(self, spec=None):
+        """The non-Newtonian viscosity solve with the `rheology` attribute's setting (or `spec`)."""
+        spec = self.rheology if spec is None else spec
+        r = capi.rheology(spec)
+        o = dict(capi.RHEOLOGY_SOLVE_DEFAULTS, **{k: spec[k] for k in capi.RHEOLOGY_SOLVE_DEFAULTS if k in spec})
+        work, nu = self._rheo_buffers()
+        check(self.L.sphk_non_newtonian_viscosity(self.ctx, self._s(), work, nu, C.byref(r), C.c_float(o["beta"]), C.c_float(self.dt),
+                                                  C.c_float(self.p.rho0), C.c_float(self.p.rho_boundary), C.c_float(o["tol"]),
+                                                  C.c_int(int(o["max_iter"]))), "sphk_non_newtonian_viscosity")
+
+    def non_newtonian_stats(self) -> dict:
+        """of the last solve (as capi.SphApp.rheology_stats); synchronises"""
+        it, res, g, lo, hi, k = C.c_int(0), C.c_float(0), C.c_float(0), C.c_float(0), C.c_float(0), C.c_int(0)
+        check(self.L.sphk_non_newtonian_stats(self.ctx, C.byref(it), C.byref(res), C.byref(g), C.byref(lo), C.byref(hi), C.byref(k)),
+              "sphk_non_newtonian_stats")
+        return {"iterations": it.value, "residual": res.value, "gamma_max": g.value, "nu_min": lo.value, "nu_max": hi.value,
+                "at_nu_max": k.value}
+
+    def shear_rate(self, gamma_out, nu_out, spec, grad_out=None, flag_out=None, beta=0.0):
+        """gamma_dot (n), nu (n) and optionally grad v (n, 9) and the fallback flag (n, int32) of the shear sweep alone"""
+        r = capi.rheology(spec)
+        check(self.L.sphk_shear_rate(self.ctx, self._s(), _ptr(gamma_out), _ptr(nu_out), _ptr(grad_out) if grad_out is not None else None,
+                                     _ptr(flag_out) if flag_out is not None else None, C.byref(r), C.c_float(beta),
+                                     C.c_float(self.p.rho0), C.c_float(self.p.rho_boundary)), "sphk_shear_rate")
+
+    def rheology_eval(self, spec, gamma, nu_out):
+        r = capi.rheology(spec)
+        check(self.L.sphk_rheology_eval(self.ctx, C.byref(r), _ptr(gamma), _ptr(nu_out), C.c_int(gamma.numel())), "sphk_rheology_eval")
+
+    def visc_field_setup(self, d_out, b_out, nu, beta):
+        """D_i (n, 6) and b_i (n, 3) with the per-particle nu (n) (one mirror + one sweep)"""
+        check(self.L.sphk_visc_field_setup(self.ctx, self._s(), _ptr(d_out), _ptr(b_out), _ptr(nu), C.c_float(beta), C.c_float(self.dt),
+                                           C.c_float(self.p.rho0), C.c_float(self.p.rho_boundary)), "sphk_visc_field_setup")
+
+    def visc_field_matvec(self, d_in, p_in, ap_out, nu):
+        check(self.L.sphk_visc_field_matvec(self.ctx, self._s(), _ptr(d_in), _ptr(p_in), _ptr(ap_out), _ptr(nu), C.c_float(self.dt),
+                                            C.c_float(self.p.rho0)), "sphk_visc_field_matvec")
+
     def pressure(self):
         check(self.L.sphk_pressure(self.ctx, self._s(), C.c_float(self.p.rho0), C.c_float(self.p.stiff)), "sphk_pressure")
 
@@ -494,7 +542,9 @@ class SphkOps:
             if surface:              # handleSurface, BasicSPHSolver.cu:262-275
                 self._run(self.color_grad, "array", self.buffer3)
                 self._run(self.surface, "vel")
-        if self.implicit_nu > 0:
+        if self.rheology is not None:       # replaces the constant-nu solve
+            self._run(self.non_newtonian_viscosity, "vel")
+        elif self.implicit_nu > 0:
             self._run(self.implicit_viscosity, "vel")
         if vort:
             self._run(self.vorticity_confinement, "vel")

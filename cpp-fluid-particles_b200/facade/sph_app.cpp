@@ -500,6 +500,59 @@ extern "C" int sph_app_viscosity_stats(sph_app* app, int* iterations, float* rel
 #endif
 }
 
+extern "C" int sph_app_set_rheology(sph_app* app, int model, const float* params, float nu_min, float nu_max, float boundary_factor,
+                                    float tol, int max_iter) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)model; (void)params; (void)nu_min; (void)nu_max; (void)boundary_factor; (void)tol; (void)max_iter;
+    return 1;
+#else
+    auto* b = dynamic_cast<BasicSPHSolver*>(app->solver);
+    if (!b) return 1;
+    if (model == 0) {                      // off
+        b->clearRheology();
+        return 0;
+    }
+    if (!params) return 1;
+    sphb200::Rheology r;
+    r.model = model;
+    for (int k = 0; k < 6; ++k) r.params[k] = params[k];
+    r.nu_min = nu_min; r.nu_max = nu_max;
+    return b->setRheology(r, boundary_factor, tol, max_iter) ? 0 : 1;     // (refused: the setting is kept)
+#endif
+}
+
+extern "C" int sph_app_rheology_stats(sph_app* app, int* iterations, float* rel_residual, float* gamma_max, float* nu_min,
+                                      float* nu_max, int* n_at_max) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)iterations; (void)rel_residual; (void)gamma_max; (void)nu_min; (void)nu_max; (void)n_at_max;
+    return 1;
+#else
+    auto* b = dynamic_cast<BasicSPHSolver*>(app->solver);
+    if (!b) return 1;
+    const sphb200::RheologyStats s = b->lastRheologyStats();
+    if (iterations) *iterations = s.iterations;
+    if (rel_residual) *rel_residual = s.residual;
+    if (gamma_max) *gamma_max = s.gammaMax;
+    if (nu_min) *nu_min = s.nuMin;
+    if (nu_max) *nu_max = s.nuMax;
+    if (n_at_max) *n_at_max = s.atNuMax;
+    return 0;
+#endif
+}
+
+extern "C" int sph_app_download_viscosity(sph_app* app, float* nu_host) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)nu_host;
+    return 1;
+#else
+    auto* b = dynamic_cast<BasicSPHSolver*>(app->solver);
+    if (!b || !nu_host) return 1;
+    const DArray<float>& nu = b->viscosityField();
+    const size_t n = std::min<size_t>(nu.length(), app->system->getFluids()->size());
+    return d2h(nu_host, nu.addr(), n * sizeof(float));
+#endif
+}
+
 extern "C" int sph_app_set_adaptive_dt(sph_app* app, float C, float dt_min, float dt_max) {
 #ifdef SPH_APP_REFERENCE_ENGINE
     (void)app; (void)C; (void)dt_min; (void)dt_max;

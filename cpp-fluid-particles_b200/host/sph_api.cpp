@@ -6,6 +6,7 @@
 #include <algorithm>
 #include <cmath>
 #include <cstdlib>
+#include <cstring>
 #include <limits>
 #include <numeric>
 
@@ -159,7 +160,8 @@ void BasicSPHSolver::velocityStage(std::shared_ptr<SPHParticles>& fluids, const 
             handleSurface(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, rhoB, cellSize, cellLength, radius,
                           dt, surfaceTensionIntensity, airPressure);
     }
-    if (implicitViscosityOn()) implicitViscosity(fluids, rho0, rhoB, dt);
+    if (rheoOn_) rheology(fluids, rho0, rhoB, dt);        // replaces the constant-nu solve
+    else if (implicitViscosityOn()) implicitViscosity(fluids, rho0, rhoB, dt);
     if (vorticityOn()) confine(fluids, rho0, dt);
 }
 
@@ -221,6 +223,63 @@ void BasicSPHSolver::viscStats(int& iters, float& residual) const {
 }
 int BasicSPHSolver::lastViscosityIterations() const { int it; float r; viscStats(it, r); return it; }
 float BasicSPHSolver::lastViscosityResidual() const { int it; float r; viscStats(it, r); return r; }
+
+// addition (no reference counterpart): non-Newtonian viscosity, sphk.h
+static bool rheologyValid(const sphb200::Rheology& r) {
+    for (float p : r.params) if (!std::isfinite(p)) return false;
+    if (!std::isfinite(r.nu_min) || !std::isfinite(r.nu_max) || !(r.nu_min >= 0.0f) || r.nu_min > r.nu_max) return false;
+    const float* p = r.params;
+    if (r.model == SPHK_RHEOLOGY_CROSS) return p[0] >= 0.0f && p[1] >= 0.0f && p[2] >= 0.0f && p[3] > 0.0f;
+    if (r.model == SPHK_RHEOLOGY_HERSCHEL_BULKLEY) return p[0] >= 0.0f && p[1] > 0.0f && p[2] >= 0.0f && p[3] >= 0.0f;
+    return false;
+}
+
+bool BasicSPHSolver::setRheology(const sphb200::Rheology& r, float boundaryFactor, float tol, int maxIter) {
+    if (!rheologyValid(r) || !(boundaryFactor >= 0.0f) || !std::isfinite(boundaryFactor) || !(tol > 0.0f) || maxIter < 1 ||
+        maxIter > SPHK_IMPLICIT_VISCOSITY_MAX_ITER) {
+        printf("setRheology: need a known model with finite parameters in range, 0 <= nuMin <= nuMax (finite), boundaryFactor >= 0, "
+               "tol > 0 and 1 <= maxIter <= %d; the setting is kept\n", SPHK_IMPLICIT_VISCOSITY_MAX_ITER);
+        return false;
+    }
+    if (boundaryFactor > 0.0f && reacting_) {
+        printf("setRheology: boundaryFactor > 0 is not supported with dynamic bodies (the viscous wall force is not part of their "
+               "reaction); the setting is kept\n");
+        return false;
+    }
+    if (!rheoWork_)
+        rheoWork_ = std::make_unique<DArray<float>>(static_cast<unsigned int>(sphk_rheology_work_floats(num_)));
+    viscosityField();
+    if (!rheoOn_ || std::memcmp(&r, &rheo_, sizeof(sphk_rheology)) != 0 || boundaryFactor != rheoBeta_ || tol != rheoTol_ ||
+        maxIter != rheoMaxIter_)
+        ++configEpoch_;
+    rheoOn_ = true; rheo_ = r; rheoBeta_ = boundaryFactor; rheoTol_ = tol; rheoMaxIter_ = maxIter;
+    return true;
+}
+
+void BasicSPHSolver::clearRheology() {
+    if (rheoOn_) ++configEpoch_;
+    rheoOn_ = false;
+}
+
+const DArray<float>& BasicSPHSolver::viscosityField() const {
+    if (!nuField_) nuField_ = std::make_unique<DArray<float>>(static_cast<unsigned int>(num_));
+    return *nuField_;
+}
+
+void BasicSPHSolver::rheology(const std::shared_ptr<SPHParticles>& fluids, float rho0, float rhoB, float dt) {
+    check(sphk_non_newtonian_viscosity(current_.ctx, &current_.abi, rheoWork_->addr(), nuField_->addr(), &rheo_, rheoBeta_, dt, rho0,
+                                       rhoB, rheoTol_, rheoMaxIter_),
+          "sphk_non_newtonian_viscosity");
+    producedVel(fluids);
+}
+
+sphb200::RheologyStats BasicSPHSolver::lastRheologyStats() const {
+    sphb200::RheologyStats s;
+    if (current_.ctx)
+        check(sphk_non_newtonian_stats(current_.ctx, &s.iterations, &s.residual, &s.gammaMax, &s.nuMin, &s.nuMax, &s.atNuMax),
+              "sphk_non_newtonian_stats");
+    return s;
+}
 
 // :227-235
 void BasicSPHSolver::force(std::shared_ptr<SPHParticles>&, float dt, float3 G) {

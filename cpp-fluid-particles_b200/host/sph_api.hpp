@@ -111,6 +111,30 @@ struct AdaptiveStats {
     long long nonFiniteSteps = 0;    // steps whose bound left out non-finite velocities, or was not finite
     float frameMinDt = 0.0f;         // the smallest dt of the last advance()
 };
+// addition: non-Newtonian viscosity (DESIGN.md section 2.9; sphk_rheology in sphk.h).  Kinematic viscosities (m^2/s in the
+// scene's units); nuMax must be finite -- it bounds the solve's conditioning and so its iterations.
+struct Rheology : sphk_rheology {
+    Rheology() : sphk_rheology{} {}
+    // shear-thinning (or Newtonian with nu0 = nuInf): nu = nuInf + (nu0 - nuInf) / (1 + (lambda gamma_dot)^m)
+    static Rheology cross(float nu0, float nuInf, float lambda, float m, float nuMax, float nuMin = 0.0f) {
+        Rheology r; r.model = SPHK_RHEOLOGY_CROSS;
+        r.params[0] = nu0; r.params[1] = nuInf; r.params[2] = lambda; r.params[3] = m; r.nu_min = nuMin; r.nu_max = nuMax;
+        return r;
+    }
+    // yield stress tauY (kinematic), consistency K, flow index n (1: Bingham; < 1 thinning, > 1 thickening), regularisation mReg
+    static Rheology herschelBulkley(float K, float n, float tauY, float mReg, float nuMax, float nuMin = 0.0f) {
+        Rheology r; r.model = SPHK_RHEOLOGY_HERSCHEL_BULKLEY;
+        r.params[0] = K; r.params[1] = n; r.params[2] = tauY; r.params[3] = mReg; r.nu_min = nuMin; r.nu_max = nuMax;
+        return r;
+    }
+};
+struct RheologyStats {
+    int iterations = 0;              // PCG iterations of the last solve
+    float residual = 0.0f;           // its |r|_M / |b|_M
+    float gammaMax = 0.0f;           // largest shear rate
+    float nuMin = 0.0f, nuMax = 0.0f;
+    int atNuMax = 0;                 // particles at the nuMax clamp (the unyielded part of a yield-stress fluid)
+};
 }  // namespace sphb200
 
 // ---- DArray.h:21-54 ---------------------------------------------------------------------------
@@ -241,6 +265,19 @@ public:
     // iterations and final relative residual of the last solve (0 before the first); synchronise
     int lastViscosityIterations() const;
     float lastViscosityResidual() const;
+    // addition: non-Newtonian viscosity (sphk_non_newtonian_viscosity; DESIGN.md section 2.9).  When set, every step solves the
+    // implicit viscosity system with nu_i = model(gamma_dot_i) frozen for the step, INSTEAD of the constant-nu solve of
+    // setImplicitViscosity (same place in the step).  boundaryFactor beta: walls and bodies act with beta nu_i (0: free slip,
+    // 1: no-slip).  A non-finite value, nuMin > nuMax, an unknown model or a parameter outside its range, beta < 0, tol <= 0,
+    // maxIter outside [1, SPHK_IMPLICIT_VISCOSITY_MAX_ITER], and beta > 0 with dynamic bodies are refused (printed, setting kept;
+    // returns false).  The workspace and the viscosity field are allocated on the first setting.
+    bool setRheology(const sphb200::Rheology& r, float boundaryFactor = 0.0f, float tol = 1e-4f, int maxIter = 20);
+    void clearRheology();
+    bool rheologyOn() const { return rheoOn_; }
+    // nu_i of the last solve, device, sized by capacity (zeros before the first)
+    const DArray<float>& viscosityField() const;
+    // statistics of the last solve (zeros before the first); synchronises
+    sphb200::RheologyStats lastRheologyStats() const;
     // addition: true when step() enqueues the same kernel sequence every call and never synchronises the host.
     // Only the three shipped solver types can say so: a user-derived solver (the reference API allows subclassing
     // BasicSPHSolver) has per-step host logic of its own, so it is never captured into a step graph.
@@ -328,6 +365,13 @@ private:
     int implMaxIter_ = 20;
     std::unique_ptr<DArray<float>> viscWork_;    // workspace of sphk_implicit_viscosity
     void viscStats(int& iters, float& residual) const;
+    bool rheoOn_ = false;
+    sphb200::Rheology rheo_;
+    float rheoBeta_ = 0.0f, rheoTol_ = 1e-4f;
+    int rheoMaxIter_ = 20;
+    std::unique_ptr<DArray<float>> rheoWork_;    // workspace of sphk_non_newtonian_viscosity
+    mutable std::unique_ptr<DArray<float>> nuField_;   // nu_i (zeros until the first solve)
+    void rheology(const std::shared_ptr<SPHParticles>& fluids, float rho0, float rhoB, float dt);
 };
 
 // ---- DFSPHSolver.h:20-64 ----------------------------------------------------------------------

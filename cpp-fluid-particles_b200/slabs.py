@@ -990,6 +990,16 @@ class SlabSystem(SphkOps):
         if nu != 0.0:
             raise ValueError("implicit viscosity is not supported on slab ranks (single-GPU engine.SphkSystem only)")
 
+    # non-Newtonian viscosity: the same solve, and a shear sweep that would need the ghosts' velocity gradients
+    @property
+    def rheology(self):
+        return None
+
+    @rheology.setter
+    def rheology(self, spec):
+        if spec is not None:
+            raise ValueError("non-Newtonian viscosity is not supported on slab ranks (single-GPU engine.SphkSystem only)")
+
     def step(self):
         self._step_no += 1
         if self.stray_cap and self._ranges is not None:

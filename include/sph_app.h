@@ -86,6 +86,18 @@ int   sph_app_set_implicit_viscosity(sph_app* app, float nu, float nu_boundary, 
 /* iterations and relative residual |r|_M / |b|_M of the last implicit viscosity solve (0, 0 before the first); synchronises;
  * 1 on the reference build */
 int   sph_app_viscosity_stats(sph_app* app, int* iterations, float* rel_residual);
+/* Non-Newtonian viscosity in every following step (BasicSPHSolver::setRheology; DESIGN.md section 2.9), replacing the
+ * constant-nu implicit solve: model 1 = Cross, params {nu0, nu_inf, lambda, m}; 2 = Herschel-Bulkley, params {K, n, tau_y, m_reg}
+ * (6 floats, the unused ones 0); nu clamped to [nu_min, nu_max]; walls and bodies act with boundary_factor * nu_i.  model 0 = off.
+ * Returns 1 on the reference build and for a setting the class layer refuses (the setting is then kept). */
+int   sph_app_set_rheology(sph_app* app, int model, const float* params, float nu_min, float nu_max, float boundary_factor,
+                           float tol, int max_iter);
+/* of the last non-Newtonian solve (zeros before the first): iterations, |r|_M / |b|_M, max shear rate, min / max nu, particles at
+ * the nu_max clamp (any pointer may be NULL); synchronises; 1 on the reference build */
+int   sph_app_rheology_stats(sph_app* app, int* iterations, float* rel_residual, float* gamma_max, float* nu_min, float* nu_max,
+                             int* n_at_max);
+/* nu_i of the last non-Newtonian solve (float[fluid size]; zeros before the first); 1 on the reference build */
+int   sph_app_download_viscosity(sph_app* app, float* nu_host);
 /* Kinematic rigid bodies (SPHSystem's constructor with a vector of sphb200::KinematicBody; DESIGN.md section 2.3).  No
  * reference counterpart: NULL / 1 on the reference build.  Body b is the points body_xyz[body_begin[b] .. body_begin[b+1])
  * (body coordinates; body_begin[0] = 0), pose[7 b ..] = {cx, cy, cz, qx, qy, qz, qw} (quaternion scalar part last),

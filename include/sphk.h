@@ -293,6 +293,50 @@ int sphk_visc_implicit_setup(sphk_ctx* ctx, const sphk_scene* s, float* d_out, f
 int sphk_visc_implicit_matvec(sphk_ctx* ctx, const sphk_scene* s, const float* d_in, const float* p_in, float* ap_out, float nu,
                               float dt, float rho0);
 
+/* ---- non-Newtonian viscosity (no reference counterpart; DESIGN.md section 2.9) -----------------------------------------------
+ * The implicit viscosity solve above with a per-particle kinematic viscosity nu_i = model(gamma_dot_i), frozen for the step (one
+ * Picard linearisation: gamma_dot from v*, the velocities entering the solve).
+ *   shear rate: G_i = sum_j V_j (v_j - v_i) (x) gradW_ij, M_i = -sum_j V_j g d d^T (boundary neighbours only when beta > 0, with
+ *               V_b = m_b / rho_boundary and the record's velocity), grad v_i = G_i M_i^-1 -- or G_i 3 / tr M_i where
+ *               det M_i < 0.01 (tr M_i / 3)^3 --, E = (grad v + grad v^T) / 2, gamma_dot = sqrt(2 E:E)
+ *   models (double, rounded to float once, clamped to [nu_min, nu_max]; stresses kinematic, i.e. divided by rho0):
+ *     SPHK_RHEOLOGY_CROSS            params {nu0, nu_inf, lambda, m}:  nu = nu_inf + (nu0 - nu_inf) / (1 + (lambda gamma_dot)^m)
+ *     SPHK_RHEOLOGY_HERSCHEL_BULKLEY params {K, n, tau_y, m_reg}:     nu = K gamma_dot^(n-1) + tau_y (1 - exp(-m_reg gamma_dot)) / gamma_dot
+ *                                                                      (tau_y m_reg at gamma_dot = 0)
+ *   pairs: fluid c_ij with nu_ij = (nu_i + nu_j) / 2 (so m_i c_ij = m_j c_ji: the PCG applies unchanged), boundary nu_ib = beta nu_i
+ *   (beta = 0: free slip; 1: no-slip with the fluid's own viscosity).
+ * nu_max must be finite: it bounds the largest eigenvalue of A and so the iterations the solve needs.  nu_field = caller-owned
+ * device float[n]: receives nu_i.  work = sphk_rheology_work_floats(n) device floats.
+ * SPHK_ERR_INVALID: NULL or aliased buffers, a non-finite parameter, nu_min < 0, nu_min > nu_max, a parameter outside its model's
+ * range (Cross: nu0, nu_inf, lambda >= 0, m > 0; HB: K >= 0, n > 0, tau_y >= 0, m_reg >= 0), an unknown model, beta < 0, rho0 or
+ * rho_boundary <= 0, tol <= 0, max_iter outside [1, SPHK_IMPLICIT_VISCOSITY_MAX_ITER].  SPHK_ERR_STATE: an active range (slab
+ * ranks), or beta > 0 with dynamic bodies declared. */
+#define SPHK_RHEOLOGY_CROSS 1
+#define SPHK_RHEOLOGY_HERSCHEL_BULKLEY 2
+typedef struct sphk_rheology {
+    int model;
+    float params[6];          /* the model's parameters in the order above; the unused ones must be finite (0) */
+    float nu_min, nu_max;
+} sphk_rheology;
+long long sphk_rheology_work_floats(int n);
+int sphk_non_newtonian_viscosity(sphk_ctx* ctx, const sphk_scene* s, float* work, float* nu_field, const sphk_rheology* rheology,
+                                 float beta, float dt, float rho0, float rho_boundary, float tol, int max_iter);
+/* of the last sphk_non_newtonian_viscosity (0 before the first; the shear statistics also of a later sphk_shear_rate): PCG
+ * iterations and |r|_M / |b|_M, max gamma_dot, min and max nu, and the particles at the nu_max clamp; any pointer may be NULL.
+ * Synchronises. */
+int sphk_non_newtonian_stats(sphk_ctx* ctx, int* iterations, float* rel_residual, float* gamma_max, float* nu_min, float* nu_max,
+                             int* n_at_max);
+/* Per-element entries (tests): the shear sweep alone (gamma_dot, nu; optionally grad v as float[9n] row-major d v_a / d x_b and
+ * int[n] = 1 where the scalar normalisation replaced M_i^-1); the model on a given gamma_dot array (no scene needed); the setup and
+ * matvec sweeps with an explicit nu array (the matvec leaves the records' velocities as the API array holds them). */
+int sphk_shear_rate(sphk_ctx* ctx, const sphk_scene* s, float* gamma_out, float* nu_out, float* grad_out_or_null,
+                    int* flag_out_or_null, const sphk_rheology* rheology, float beta, float rho0, float rho_boundary);
+int sphk_rheology_eval(sphk_ctx* ctx, const sphk_rheology* rheology, const float* gamma, float* nu_out, int n);
+int sphk_visc_field_setup(sphk_ctx* ctx, const sphk_scene* s, float* d_out, float* b_out, const float* nu, float beta, float dt,
+                          float rho0, float rho_boundary);
+int sphk_visc_field_matvec(sphk_ctx* ctx, const sphk_scene* s, const float* d_in, const float* p_in, float* ap_out, const float* nu,
+                           float dt, float rho0);
+
 /* ---- kinematic rigid bodies (no reference counterpart; DESIGN.md section 2.3) ---------------------------------------------
  * A body is a rigid set of boundary particles given in body coordinates r_k, with a pose (centre c, unit quaternion q) and
  * a motion (linear velocity V, angular velocity Omega, both in the world frame).  Poses and motions live in device memory.
