@@ -11,6 +11,14 @@
 //                [--dt DT] [--iters K] [--vorticity EPS] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] [--ranks N [--rank R --rendezvous DIR]]
 //                [--bullets K] [--stir OMEGA] [--float REL] [--implicit-viscosity NU] [--tap SPEED] [--drain SIDE] [--capacity N]
 //                [--cfl C [--dt-min X]] [--rheology cross:NU0,NUINF,LAMBDA,M | hb:K,N,TAU[,MREG] [--rheology-max NU_MAX] [--no-slip]]
+//                [--heat ALPHA,BETA[,TREF] [--heater T] [--wall-temp T[,H]] [--tap-temp T] [--thermal-viscosity NUREF,E[,NUMAX]]]
+// --heat turns on heat transfer (BasicSPHSolver::setThermal, DESIGN.md section 2.10) after the constructor's step 0: diffusivity ALPHA,
+// buoyancy BETA, reference temperature TREF (default 0, also the fluid's initial temperature).  --heater T adds a held, motionless
+// plate body on the floor under the block at T with conductance 1 (not together with --stir or --float); --wall-temp T[,H] sets the
+// tank walls' temperature and conductance (default TREF, 0: adiabatic); --tap-temp T the --tap emitter's temperature (default TREF).
+// --thermal-viscosity NUREF,E[,NUMAX] solves nu = clamp(NUREF exp(-E (T - TREF)), 0, NUMAX) (default NUMAX = 100 NUREF) with no-slip
+// walls instead of a constant nu (not with --rheology, --implicit-viscosity or --float).  Every frame prints min, max and mean T, the
+// heat content sum m T, the substeps and the particle-substeps above the stability bound.  Single GPU only.
 // --rheology turns on non-Newtonian viscosity (BasicSPHSolver::setRheology, DESIGN.md section 2.9) after the constructor's step 0,
 // for every solver, instead of --implicit-viscosity: a Cross fluid (shear-thinning; Newtonian with NU0 = NUINF) or a
 // Herschel-Bulkley fluid with yield stress TAU (kinematic; Bingham with N = 1), regularisation MREG (default 1000 s).  nu is
@@ -99,6 +107,8 @@ struct Options {
     std::string rheology;                     // --rheology MODEL:PARAMS (empty: off)
     float rheologyMax = -1.0f;                // --rheology-max NU_MAX (< 0: the model's default)
     bool noSlip = false;                      // --no-slip: boundary factor 1 for --rheology
+    std::string heat;                         // --heat ALPHA,BETA[,TREF] (empty: off)
+    std::string heater, wallTemp, tapTemp, thermalVisc;   // --heater T, --wall-temp T[,H], --tap-temp T, --thermal-viscosity NUREF,E[,NUMAX]
     float cfl = 0.0f;                         // --cfl C: CFL-adaptive substeps, --dt of simulated time per frame (0: off)
     float dtMin = 0.0f;                       // --dt-min X: their smallest dt (0: dt / 64)
     int bullets = 0;                          // test aid: this many top-layer particles start at ~3 cell planes per step
@@ -134,6 +144,49 @@ bool rheology_of(const Options& o, sphb200::Rheology& r) {
     return std::isfinite(o.rheologyMax);
 }
 
+// "a,b,c" -> finite floats (false for an empty item, a non-number or a non-finite value)
+bool floats_of(const std::string& spec, std::vector<float>& v) {
+    v.clear();
+    size_t at = 0;
+    while (at <= spec.size()) {
+        const size_t comma = std::min(spec.find(',', at), spec.size());
+        const std::string item = spec.substr(at, comma - at);
+        char* end = nullptr;
+        const float x = std::strtof(item.c_str(), &end);
+        if (item.empty() || *end != '\0' || !std::isfinite(x)) return false;
+        v.push_back(x);
+        at = comma + 1;
+    }
+    return true;
+}
+
+// --heat and its companions -> the thermal setting and the viscosity law (ranges are checked by the setters)
+bool thermal_of(const Options& o, sphb200::Thermal& t, sphb200::ThermalViscosity& tv) {
+    std::vector<float> v;
+    if (!floats_of(o.heat, v) || v.size() < 2 || v.size() > 3) return false;
+    t = sphb200::Thermal();
+    t.alpha = v[0]; t.beta = v[1]; t.Tref = v.size() == 3 ? v[2] : 0.0f;
+    t.wall = {t.Tref, 0.0f};
+    if (!o.wallTemp.empty()) {
+        if (!floats_of(o.wallTemp, v) || v.size() > 2) return false;
+        t.wall = {v[0], v.size() == 2 ? v[1] : 1.0f};
+    }
+    if (!o.heater.empty()) {
+        if (!floats_of(o.heater, v) || v.size() != 1) return false;
+        t.bodies.push_back({v[0], 1.0f});
+    }
+    if (!o.tapTemp.empty()) {
+        if (!floats_of(o.tapTemp, v) || v.size() != 1) return false;
+        t.emitterT.push_back(v[0]);
+    }
+    if (!o.thermalVisc.empty()) {
+        if (!floats_of(o.thermalVisc, v) || v.size() < 2 || v.size() > 3) return false;
+        tv = sphb200::ThermalViscosity();
+        tv.nuRef = v[0]; tv.E = v[1]; tv.nuMax = v.size() == 3 ? v[2] : 100.0f * v[0]; tv.wallFactor = 1.0f;
+    }
+    return true;
+}
+
 bool parse(int argc, char** argv, Options& o) {
     auto need = [&](int i, int k) { return i + k < argc; };
     for (int i = 1; i < argc; ++i) {
@@ -156,6 +209,11 @@ bool parse(int argc, char** argv, Options& o) {
         else if (a == "--rheology" && need(i, 1)) o.rheology = argv[++i];
         else if (a == "--rheology-max" && need(i, 1)) o.rheologyMax = static_cast<float>(std::atof(argv[++i]));
         else if (a == "--no-slip") o.noSlip = true;
+        else if (a == "--heat" && need(i, 1)) o.heat = argv[++i];
+        else if (a == "--heater" && need(i, 1)) o.heater = argv[++i];
+        else if (a == "--wall-temp" && need(i, 1)) o.wallTemp = argv[++i];
+        else if (a == "--tap-temp" && need(i, 1)) o.tapTemp = argv[++i];
+        else if (a == "--thermal-viscosity" && need(i, 1)) o.thermalVisc = argv[++i];
         else if (a == "--cfl" && need(i, 1)) o.cfl = static_cast<float>(std::atof(argv[++i]));
         else if (a == "--dt-min" && need(i, 1)) o.dtMin = static_cast<float>(std::atof(argv[++i]));
         else if (a == "--ranks" && need(i, 1)) o.ranks = std::atoi(argv[++i]);
@@ -216,6 +274,25 @@ bool parse(int argc, char** argv, Options& o) {
         }
     } else if (o.noSlip || o.rheologyMax >= 0.0f) {
         std::fprintf(stderr, "sph_headless: --no-slip and --rheology-max go with --rheology\n");
+        return false;
+    }
+    if (!o.heat.empty()) {
+        sphb200::Thermal t;
+        sphb200::ThermalViscosity tv;
+        if (!thermal_of(o, t, tv)) {
+            std::fprintf(stderr, "sph_headless: --heat needs ALPHA,BETA[,TREF], --heater T, --wall-temp T[,H], --tap-temp T and "
+                                 "--thermal-viscosity NUREF,E[,NUMAX] with finite values\n");
+            return false;
+        }
+        if (o.ranks > 1 || (!o.heater.empty() && (o.stir || o.floating)) || (!o.tapTemp.empty() && !(o.tap > 0.0f)) ||
+            (!o.thermalVisc.empty() && (!o.rheology.empty() || o.implicitNu > 0.0f || o.floating))) {
+            std::fprintf(stderr, "sph_headless: --heat runs on one GPU only (not with --ranks); --heater not together with --stir or "
+                                 "--float; --tap-temp needs --tap; --thermal-viscosity not together with --rheology, "
+                                 "--implicit-viscosity or --float\n");
+            return false;
+        }
+    } else if (!o.heater.empty() || !o.wallTemp.empty() || !o.tapTemp.empty() || !o.thermalVisc.empty()) {
+        std::fprintf(stderr, "sph_headless: --heater, --wall-temp, --tap-temp and --thermal-viscosity go with --heat\n");
         return false;
     }
     if (!(o.cfl >= 0.0f) || !std::isfinite(o.cfl) || !(o.dtMin >= 0.0f) || !std::isfinite(o.dtMin)) {
@@ -279,6 +356,24 @@ sphb200::KinematicBody paddle(const Options& o, float spacing, float boundarySpa
 }
 
 constexpr float kSphM0 = 76.596750762082e-6f;   // the fluid particle mass m0, main.cpp
+
+// --heater: a held plate (two boundary layers) on the floor under the block, one spacing wider than the block on every side
+sphb200::KinematicBody heater_plate(const Options& o, float spacing, float boundarySpacing) {
+    sphb200::KinematicBody b;
+    const float sb = boundarySpacing;
+    const float ex = spacing * (o.block[0] - 1) + 2.0f * spacing, ez = spacing * (o.block[2] - 1) + 2.0f * spacing;
+    const int nx = std::max(2, static_cast<int>(ex / sb) + 1), nz = std::max(2, static_cast<int>(ez / sb) + 1);
+    for (int i = 0; i < nx; ++i)
+        for (int k = 0; k < nz; ++k)
+            for (int j = 0; j < 2; ++j)
+                b.points.push_back(make_float3((i - 0.5f * (nx - 1)) * sb, (j - 0.5f) * sb, (k - 0.5f * (nz - 1)) * sb));
+    b.position = make_float3(o.origin[0] + 0.5f * spacing * (o.block[0] - 1), 2.5f * sb,
+                             o.origin[2] + 0.5f * spacing * (o.block[2] - 1));
+    b.orientation = make_float4(0.0f, 0.0f, 0.0f, 1.0f);
+    b.linearVelocity = make_float3(0.0f, 0.0f, 0.0f);
+    b.angularVelocity = make_float3(0.0f, 0.0f, 0.0f);
+    return b;
+}
 
 // --float: the hollow cube (body coordinates, centred on the block's centre, at rest), mass and moments of a solid cube
 sphb200::KinematicBody floating_cube(const Options& o, float spacing, float boundarySpacing) {
@@ -388,7 +483,8 @@ int main(int argc, char** argv) {
         std::fprintf(stderr, "usage: sph_headless [--solver sph|dfsph|pbd] [--frames N] [--box L | LX LY LZ] [--block NX NY NZ] "
                              "[--origin X Y Z] [--dt DT] [--iters K] [--vorticity EPS] [--implicit-viscosity NU] [--stir OMEGA | --float REL] "
                              "[--tap SPEED] [--drain SIDE] [--capacity N] [--cfl C [--dt-min X]] [--rheology cross:NU0,NUINF,LAMBDA,M | hb:K,N,TAU[,MREG] "
-                             "[--rheology-max NU_MAX] [--no-slip]] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] "
+                             "[--rheology-max NU_MAX] [--no-slip]] [--heat ALPHA,BETA[,TREF] [--heater T] [--wall-temp T[,H]] "
+                             "[--tap-temp T] [--thermal-viscosity NUREF,E[,NUMAX]]] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] "
                              "[--ranks N [--rank R --rendezvous DIR]]\n");
         return 2;
     }
@@ -405,6 +501,7 @@ int main(int argc, char** argv) {
     std::vector<float3> fluidPoints = fluid_block(o, sphSpacing);
     if (o.stir) bodies.push_back(paddle(o, sphSpacing, boundarySpacing));
     if (o.floating) bodies.push_back(floating_cube(o, sphSpacing, boundarySpacing));
+    if (!o.heater.empty()) bodies.push_back(heater_plate(o, sphSpacing, boundarySpacing));
     if (!bodies.empty()) fluidPoints = clear_of(fluidPoints, bodies[0], boundarySpacing);
     const sphb200::OpenBoundaries openB = open_boundaries(o, sphSpacing);
     const bool open = !openB.emitters.empty() || !openB.sinks.empty();
@@ -538,6 +635,15 @@ int main(int argc, char** argv) {
             return 4;
         }
     }
+    if (!o.heat.empty()) {
+        sphb200::Thermal t;
+        sphb200::ThermalViscosity tv;
+        thermal_of(o, t, tv);
+        if (!basicSolver->setThermal(t) || (!o.thermalVisc.empty() && !basicSolver->setThermalViscosity(tv))) {
+            std::fprintf(stderr, "sph_headless: --heat %s was refused\n", o.heat.c_str());
+            return 4;
+        }
+    }
     if (o.cfl > 0.0f && !pSystem->setAdaptiveTimeStep(o.cfl, o.dtMin)) {
         std::fprintf(stderr, "sph_headless: --cfl %g --dt-min %g was refused\n", o.cfl, o.dtMin);
         return 4;
@@ -579,6 +685,12 @@ int main(int argc, char** argv) {
         if (slab && o.bullets > 0) straysRouted += pSlab->straysRouted();
         totalTime += milliseconds;
         worst = milliseconds > worst ? milliseconds : worst;
+        if (!o.quiet && !o.heat.empty()) {
+            const sphb200::ThermalStats ts = basicSolver->lastThermalStats();
+            const int nf = static_cast<int>(pSystem->getFluids()->size());
+            std::printf("Frame %d heat - T min %g max %g mean %g, heat %.9g, %d substeps, %d above the stability bound\n", frameId,
+                        ts.Tmin, ts.Tmax, nf > 0 ? ts.heat / (double(kSphM0) * nf) : 0.0, ts.heat, ts.substeps, ts.violators);
+        }
         if (!o.quiet && !o.rheology.empty()) {
             const sphb200::RheologyStats rs = basicSolver->lastRheologyStats();
             std::printf("Frame %d rheology - %d iterations, residual %.3g, max shear rate %g 1/s, %d particles at nu_max\n", frameId,

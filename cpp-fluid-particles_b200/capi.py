@@ -39,6 +39,8 @@ SPHK_FUNCTIONS = [
     "sphk_open_check", "sphk_time_step", "sphk_step_speed", "sphk_step_speed_result",
     "sphk_rheology_work_floats", "sphk_non_newtonian_viscosity", "sphk_non_newtonian_stats", "sphk_shear_rate", "sphk_rheology_eval",
     "sphk_visc_field_setup", "sphk_visc_field_matvec",
+    "sphk_heat_substeps", "sphk_heat_step", "sphk_heat_conduction", "sphk_heat_stats", "sphk_thermal_viscosity",
+    "sphk_thermal_viscosity_eval",
 ]
 SPH_APP_FUNCTIONS = [
     "sph_app_create", "sph_app_destroy", "sph_app_step", "sph_app_fluid_size", "sph_app_boundary_size",
@@ -48,7 +50,60 @@ SPH_APP_FUNCTIONS = [
     "sph_app_create_with_dynamic_bodies", "sph_app_body_motion", "sph_app_body_impulse", "sph_app_set_implicit_viscosity",
     "sph_app_viscosity_stats", "sph_app_create_open", "sph_app_open_boundary_stats", "sph_app_set_adaptive_dt", "sph_app_advance",
     "sph_app_adaptive_stats", "sph_app_set_rheology", "sph_app_rheology_stats", "sph_app_download_viscosity",
+    "sph_app_set_thermal", "sph_app_set_thermal_viscosity", "sph_app_upload_temperature", "sph_app_download_temperature",
+    "sph_app_thermal_stats",
 ]
+
+BODY_LIMIT = 64                      # SPHK_BODY_LIMIT
+THERMAL_GROUPS = 1 + BODY_LIMIT      # SPHK_THERMAL_GROUPS
+
+
+class ThermalGroup(C.Structure):
+    """sphk_thermal_group of sphk.h"""
+    _fields_ = [("t", C.c_float), ("h", C.c_float)]
+
+
+class Thermal(C.Structure):
+    """sphk_thermal of sphk.h"""
+    _fields_ = [("alpha", C.c_float), ("beta", C.c_float), ("t_ref", C.c_float), ("n_groups", C.c_int),
+                ("groups", ThermalGroup * THERMAL_GROUPS)]
+
+
+class ViscosityLaw(C.Structure):
+    """sphk_viscosity_law of sphk.h"""
+    _fields_ = [("nu_ref", C.c_float), ("e", C.c_float), ("t_ref", C.c_float), ("nu_min", C.c_float), ("nu_max", C.c_float)]
+
+
+def thermal(spec: dict) -> Thermal:
+    """sphk_thermal from dict(alpha, beta=0, t_ref=0, wall=(T, h) = (0, 0), bodies=[(T, h), ...], emitters=[T, ...]) (emitters is
+    ignored here).  Unknown keys and more than BODY_LIMIT bodies raise ValueError; the ranges are checked by the library."""
+    extra = set(spec) - {"alpha", "beta", "t_ref", "wall", "bodies", "emitters"}
+    if extra:
+        raise ValueError(f"unknown thermal keys {sorted(extra)}")
+    bodies = list(spec.get("bodies", ()))
+    if len(bodies) > BODY_LIMIT:
+        raise ValueError(f"at most {BODY_LIMIT} bodies")
+    t = Thermal()
+    t.alpha, t.beta, t.t_ref = float(spec["alpha"]), float(spec.get("beta", 0.0)), float(spec.get("t_ref", 0.0))
+    t.n_groups = 1 + len(bodies)
+    for g, (T, h) in enumerate([tuple(spec.get("wall", (0.0, 0.0)))] + [tuple(b) for b in bodies]):
+        t.groups[g].t, t.groups[g].h = float(T), float(h)
+    return t
+
+
+# the solve's settings of a thermal viscosity dict, beside the law's own keys
+THERMAL_VISCOSITY_DEFAULTS = {"nu_min": 0.0, "wall_factor": 0.0, "tol": 1e-4, "max_iter": 20}
+
+
+def viscosity_law(spec: dict, t_ref: float) -> ViscosityLaw:
+    """sphk_viscosity_law from dict(nu_ref, e, nu_max[, nu_min]) and the thermal setting's t_ref"""
+    extra = set(spec) - {"nu_ref", "e", "nu_max"} - set(THERMAL_VISCOSITY_DEFAULTS)
+    if extra:
+        raise ValueError(f"unknown thermal viscosity keys {sorted(extra)}")
+    v = ViscosityLaw()
+    v.nu_ref, v.e, v.t_ref = float(spec["nu_ref"]), float(spec["e"]), float(t_ref)
+    v.nu_min, v.nu_max = float(spec.get("nu_min", 0.0)), float(spec["nu_max"])
+    return v
 
 RHEOLOGY_CROSS, RHEOLOGY_HERSCHEL_BULKLEY = 1, 2   # SPHK_RHEOLOGY_* of sphk.h
 
@@ -382,6 +437,53 @@ class SphApp:
         if self.L.sph_app_download_viscosity(self.h, out.ctypes.data_as(C.c_void_p)):
             raise RuntimeError("sph_app_download_viscosity failed (reference engine)")
         return out
+
+    def set_thermal(self, spec):
+        """Heat transfer in every following step (spec: a dict for capi.thermal, with "emitters": [T, ...]; None: off).  Not on the
+        reference engine."""
+        if spec is None:
+            rc = self.L.sph_app_set_thermal(self.h, C.c_int(0), *(C.c_float(0),) * 5, C.c_int(0), None, C.c_int(0), None)
+        else:
+            t = thermal(spec)
+            bodies = np.ascontiguousarray(np.asarray(spec.get("bodies", []), np.float32).reshape(-1, 2))
+            em = np.ascontiguousarray(np.asarray(spec.get("emitters", []), np.float32).reshape(-1))
+            rc = self.L.sph_app_set_thermal(self.h, C.c_int(1), C.c_float(t.alpha), C.c_float(t.beta), C.c_float(t.t_ref),
+                                            C.c_float(t.groups[0].t), C.c_float(t.groups[0].h), C.c_int(bodies.shape[0]),
+                                            bodies.ctypes.data_as(C.c_void_p), C.c_int(em.size), em.ctypes.data_as(C.c_void_p))
+        if rc:
+            raise RuntimeError("sph_app_set_thermal failed (reference engine or a refused setting)")
+
+    def set_thermal_viscosity(self, spec):
+        """nu(T) instead of the constant-nu solve (spec: dict(nu_ref, e, nu_max, nu_min, wall_factor, tol, max_iter); None: off)"""
+        if spec is None:
+            rc = self.L.sph_app_set_thermal_viscosity(self.h, C.c_int(0), *(C.c_float(0),) * 6, C.c_int(0))
+        else:
+            v = viscosity_law(spec, 0.0)
+            o = dict(THERMAL_VISCOSITY_DEFAULTS, **{k: spec[k] for k in THERMAL_VISCOSITY_DEFAULTS if k in spec})
+            rc = self.L.sph_app_set_thermal_viscosity(self.h, C.c_int(1), C.c_float(v.nu_ref), C.c_float(v.e), C.c_float(v.nu_min),
+                                                      C.c_float(v.nu_max), C.c_float(o["wall_factor"]), C.c_float(o["tol"]),
+                                                      C.c_int(int(o["max_iter"])))
+        if rc:
+            raise RuntimeError("sph_app_set_thermal_viscosity failed (reference engine or a refused setting)")
+
+    def upload_temperature(self, t):
+        a = np.ascontiguousarray(t, np.float32)
+        if a.size != int(self.L.sph_app_fluid_size(self.h)) or self.L.sph_app_upload_temperature(self.h, a.ctypes.data_as(C.c_void_p)):
+            raise RuntimeError("sph_app_upload_temperature failed (reference engine or a wrong size)")
+
+    def download_temperature(self) -> np.ndarray:
+        out = np.zeros(int(self.L.sph_app_fluid_size(self.h)), np.float32)
+        if self.L.sph_app_download_temperature(self.h, out.ctypes.data_as(C.c_void_p)):
+            raise RuntimeError("sph_app_download_temperature failed (reference engine)")
+        return out
+
+    def thermal_stats(self) -> dict:
+        """substeps, max_courant, violators of the last step; t_min, t_max, heat (sum m T) now"""
+        k, cmax, v, lo, hi, q = C.c_int(0), C.c_float(0), C.c_int(0), C.c_float(0), C.c_float(0), C.c_double(0)
+        if self.L.sph_app_thermal_stats(self.h, C.byref(k), C.byref(cmax), C.byref(v), C.byref(lo), C.byref(hi), C.byref(q)):
+            raise RuntimeError("sph_app_thermal_stats failed (reference engine)")
+        return {"substeps": k.value, "max_courant": cmax.value, "violators": v.value, "t_min": lo.value, "t_max": hi.value,
+                "heat": q.value}
 
     def set_body_motion(self, body: int, linear_velocity, angular_velocity):
         """New motion of one kinematic body from the next step on.  Not on the reference engine."""

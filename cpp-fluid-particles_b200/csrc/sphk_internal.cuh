@@ -10,7 +10,7 @@
 #define SPHK_BLOCK 128
 #define SPHK_TILE_CAP 1535                      // records of a tile's staged neighbour windows (+1 dummy slot = 24 KiB per half)
 #define SPHK_TILE_WINS 18                       // 9 (dx,dy) rows of the fluid set + 9 of the boundary set
-#define SPHK_MAX_BODIES 64                      // kinematic bodies per context (sphk_bodies_init)
+#define SPHK_MAX_BODIES SPHK_BODY_LIMIT         // kinematic bodies per context (sphk_bodies_init)
 
 // Packed particle records, two 16-byte halves in two arrays (unified index: fluid j < capF, boundary capF + b,
 // one far-away zero-mass dummy at capF + capB used as list padding):
@@ -132,6 +132,9 @@ struct sphk_ctx {
     float* viscStats = nullptr;      // [2] device: {iterations (int bits), |r|_M / |b|_M} of the last sphk_implicit_viscosity
     float* rheoStats = nullptr;      // [6] device: {iterations, |r|_M / |b|_M, max gamma_dot, min nu, max nu, count at nu_max} of the
                                      // last sphk_non_newtonian_viscosity (uint bits; the shear statistics also of sphk_shear_rate)
+    float2* heatGroups = nullptr;    // [SPHK_THERMAL_GROUPS] device: {T_g, h_g} of the step's sphk_thermal (heat transfer)
+    unsigned int* heatStats = nullptr;   // [2] device: {max dt_k sum_j c_ij (float bits), particle-substeps above 1} of the last step
+    double* heatRed = nullptr;       // [3 * 1024 + 3] device: partials and result {min T, max T, sum m T} of sphk_heat_stats
     // open boundaries (sphk_sinks_apply / sphk_fluid_set_count; allocated on first use)
     int* openDev = nullptr;          // device [2]: {particles the last sphk_sinks_apply removed, sticky check bits}
     int* openPinned = nullptr;       // pinned [1]: the removed count, copied behind the sink kernel

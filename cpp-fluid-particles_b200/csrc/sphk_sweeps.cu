@@ -23,6 +23,9 @@
 #include <cstdlib>
 #include <cstring>
 #include <type_traits>
+#include <algorithm>
+#include <cmath>
+#include <math_constants.h>
 #include <cooperative_groups.h>
 #include <cooperative_groups/reduce.h>
 #include "sphk_internal.cuh"
@@ -582,6 +585,50 @@ struct OpViscImplicitMatvecField {
     }
 };
 
+// ---- heat transfer (no reference counterpart; DESIGN.md section 2.10) -------------------------------------------------------
+// Brookshaw / Cleary-Monaghan conduction, rec.s = T (ensure_scalar): c_ij = -2 alpha V_j f r^2 / (r^2 + eta^2), eta^2 = 0.0025 R^2,
+// V_j = m_j / rho0; a boundary neighbour of group g takes V_b = m_b / rho_B, h_g alpha and T_g.  Without bodies every boundary
+// particle is in group 0, whose {T, h} the operator carries (no extra load); with bodies the group is local[b].w and {T_g, h_g}
+// come from the context's table.  The epilogue writes dT/dt and folds max dt_k sum_j c_ij and the count above 1.
+__device__ __forceinline__ float heat_coef(float aV, float r2, const KConst& k) {
+    return -2.0f * aV * grad_w_factor(sqrtf(r2), k) * __fdividef(r2, r2 + 0.0025f * k.R * k.R);
+}
+struct OpHeatConduction {
+    float* dTdt; unsigned int* stats; const float4* local; const float2* groups;
+    float alphaRho0, alphaRhoB, t0, h0, dtSub; int nB;
+    static constexpr bool kFluidOnly = false, kHi = false, kIndex = true;
+    struct Acc { float q, c, ti; template <class F> __device__ void sums(F f) { f(q); f(c); } };
+    __device__ void begin(Acc& a, int, float4 lo, float4, const DevScene&) const { a.q = 0.f; a.c = 0.f; a.ti = lo.w; }
+    __device__ void pair(Acc& a, int, int j, bool isB, float3, float r2, float mj, float4 lo, float4, const DevScene& s) const {
+        float tj = lo.w, h = 1.0f;
+        if (isB) {
+            tj = t0; h = h0;
+            if (local) {
+                const int b = j - s.bOff;
+                if (b >= 0 && b < nB) {
+                    const float2 g = groups[static_cast<int>(body_group(local[b]))];
+                    tj = g.x; h = g.y;
+                }
+            }
+        }
+        const float c = heat_coef(mj * (isB ? h * alphaRhoB : alphaRho0), r2, s.k);
+        a.q += c * (tj - a.ti);
+        a.c += c;
+    }
+    __device__ void end(Acc& a, int i, float4, float4, const DevScene&) const {
+        dTdt[i] = a.q;
+        namespace cg = cooperative_groups;
+        const float cour = dtSub * a.c > 0.f ? dtSub * a.c : 0.f;      // (no -0: its bits would top the unsigned max)
+        const cg::coalesced_group g = cg::coalesced_threads();
+        const unsigned int cmax = cg::reduce(g, __float_as_uint(cour), cg::greater<unsigned int>());
+        const unsigned int cnt = __popc(g.ballot(cour > 1.0f));
+        if (g.thread_rank() == 0) {
+            atomicMax(stats, cmax);
+            if (cnt) atomicAdd(stats + 1, cnt);
+        }
+    }
+};
+
 // =================================================================================================
 // Sweep drivers
 // =================================================================================================
@@ -993,16 +1040,29 @@ k_build_list_staged(const DevScene s, int* __restrict__ nbr, int* __restrict__ c
 }
 
 // ---- sweep ----------------------------------------------------------------------------------------------------------------
+// Operators that read a boundary neighbour's own data (heat transfer: its group) declare kIndex = true; the tile walk then
+// recovers the record index of a boundary slot from the staged windows (the other operators get j = -1 there).
+template <class Op, class = void> struct op_index : std::false_type {};
+template <class Op> struct op_index<Op, std::void_t<decltype(Op::kIndex)>> : std::bool_constant<Op::kIndex> {};
+
 template <class Op>
 __device__ __forceinline__ void tile_pair(const DevScene& s, const Op& op, typename Op::Acc& acc, int i, float3 xi, int slot, int preB,
-                                          const float4* smA, const float4* smB, float m0) {
+                                          const float4* smA, const float4* smB, float m0, const int2* sWin, const int* sPre) {
     const bool isB = slot >= preB;
     if (Op::kFluidOnly && isB) return;
     const float4 lo = smA[slot];
     float4 hi = make_float4(0.f, 0.f, 0.f, 0.f);
     if (Op::kHi) hi = smB[slot];
     const float3 d = xi - xyz(lo);
-    feed_pair(s, op, acc, i, xi, -1, isB, lo, hi, m0, d, dot3(d, d));
+    int j = -1;
+    if constexpr (op_index<Op>::value) {
+        if (isB && slot < sPre[SPHK_TILE_WINS]) {   // (the dummy slot past the windows keeps -1)
+            int w = SPHK_TILE_WINS - 1;
+            while (w > 9 && sPre[w] > slot) --w;
+            j = sWin[w].x + (slot - sPre[w]);
+        }
+    }
+    feed_pair(s, op, acc, i, xi, j, isB, lo, hi, m0, d, dot3(d, d));
 }
 
 template <class Op>
@@ -1051,14 +1111,14 @@ __global__ void __launch_bounds__(SPHK_BLOCK) k_sweep_tile(const DevScene s, con
             const uint4 j8 = jn;
             row += s.nbrStride;
             if (b + 1 < nb8) jn = __ldcs(row);
-            tile_pair(s, op, acc, i, xi, static_cast<int>(j8.x & 0xffffu), preB, smA, smB, m0);
-            tile_pair(s, op, acc, i, xi, static_cast<int>(j8.x >> 16), preB, smA, smB, m0);
-            tile_pair(s, op, acc, i, xi, static_cast<int>(j8.y & 0xffffu), preB, smA, smB, m0);
-            tile_pair(s, op, acc, i, xi, static_cast<int>(j8.y >> 16), preB, smA, smB, m0);
-            tile_pair(s, op, acc, i, xi, static_cast<int>(j8.z & 0xffffu), preB, smA, smB, m0);
-            tile_pair(s, op, acc, i, xi, static_cast<int>(j8.z >> 16), preB, smA, smB, m0);
-            tile_pair(s, op, acc, i, xi, static_cast<int>(j8.w & 0xffffu), preB, smA, smB, m0);
-            tile_pair(s, op, acc, i, xi, static_cast<int>(j8.w >> 16), preB, smA, smB, m0);
+            tile_pair(s, op, acc, i, xi, static_cast<int>(j8.x & 0xffffu), preB, smA, smB, m0, sWin, sPre);
+            tile_pair(s, op, acc, i, xi, static_cast<int>(j8.x >> 16), preB, smA, smB, m0, sWin, sPre);
+            tile_pair(s, op, acc, i, xi, static_cast<int>(j8.y & 0xffffu), preB, smA, smB, m0, sWin, sPre);
+            tile_pair(s, op, acc, i, xi, static_cast<int>(j8.y >> 16), preB, smA, smB, m0, sWin, sPre);
+            tile_pair(s, op, acc, i, xi, static_cast<int>(j8.z & 0xffffu), preB, smA, smB, m0, sWin, sPre);
+            tile_pair(s, op, acc, i, xi, static_cast<int>(j8.z >> 16), preB, smA, smB, m0, sWin, sPre);
+            tile_pair(s, op, acc, i, xi, static_cast<int>(j8.w & 0xffffu), preB, smA, smB, m0, sWin, sPre);
+            tile_pair(s, op, acc, i, xi, static_cast<int>(j8.w >> 16), preB, smA, smB, m0, sWin, sPre);
         }
     } else {
         if (T > 0 && T <= SPHK_TILE_CAP) mbar_wait(&bar, 0);
@@ -2247,6 +2307,209 @@ extern "C" int sphk_visc_field_matvec(sphk_ctx* c, const sphk_scene* s, const fl
     if (n > 0) k_visc_set_rec_vel<<<sphk_blocks(n), SPHK_BLOCK, 0, c->stream>>>(c->rec, s->fluid.vel, n);   // records <- API velocities
     if (n > 0) c->launches += 2;
     if (rc != SPHK_OK) return rc;
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+// ---- heat transfer (DESIGN.md section 2.10) ----------------------------------------------------------------------------------
+// the step's group table {T_g, h_g} (groups past n_groups adiabatic) from the setting passed by value, and the statistics reset
+__global__ void k_heat_begin(sphk_thermal th, float2* __restrict__ groups, unsigned int* __restrict__ stats) {
+    const int g = threadIdx.x;
+    if (g < SPHK_THERMAL_GROUPS) groups[g] = g < th.n_groups ? make_float2(th.groups[g].t, th.groups[g].h) : make_float2(0.f, 0.f);
+    if (g == 0) { stats[0] = 0u; stats[1] = 0u; }
+}
+// T += dt_k dT/dt (also into rec.s, which keeps mirroring T); on the last substep v += -beta (T - T_ref) G dt on the API array and the
+// records.  A particle at T_ref gets no velocity write at all, so its bits stay those of a step without the stage.
+__global__ void __launch_bounds__(SPHK_BLOCK) k_heat_commit(float* __restrict__ T, const float* __restrict__ dTdt, Rec rec,
+                                                            float* __restrict__ vel, int n, float dtSub, bool last, float beta,
+                                                            float tRef, float3 Gdt) {
+    const int i = blockIdx.x * SPHK_BLOCK + threadIdx.x;
+    if (i >= n) return;
+    const float t = T[i] + dtSub * dTdt[i];
+    T[i] = t;
+    rec_set_s(rec + i, t);
+    const float dT = t - tRef;
+    if (last && dT != 0.f && beta != 0.f) {
+        const float3 v = load3(vel, i) - (beta * dT) * Gdt;
+        store3(vel, i, v);
+        rec_set_vel(rec + i, v);
+    }
+}
+// min T, max T and sum m T (double) in a fixed shape: clamp(ceil(n / 2048), 1, 1024) blocks of 256 threads, each thread's
+// grid-stride run, a warp butterfly, the 8 warp values in lane order; then one block over the partials in the same shape.
+#define SPHK_HEAT_RED 256
+__device__ __forceinline__ void heat_fold(double& lo, double& hi, double& sum) {
+    for (int o = 16; o > 0; o >>= 1) {
+        lo = fmin(lo, __shfl_xor_sync(0xffffffffu, lo, o));
+        hi = fmax(hi, __shfl_xor_sync(0xffffffffu, hi, o));
+        sum += __shfl_xor_sync(0xffffffffu, sum, o);
+    }
+}
+__device__ __forceinline__ void heat_block(double lo, double hi, double sum, double* out) {
+    __shared__ double sh[3][SPHK_HEAT_RED / 32];
+    heat_fold(lo, hi, sum);
+    const int w = threadIdx.x >> 5, l = threadIdx.x & 31;
+    if (l == 0) { sh[0][w] = lo; sh[1][w] = hi; sh[2][w] = sum; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        for (int k = 1; k < SPHK_HEAT_RED / 32; ++k) { lo = fmin(lo, sh[0][k]); hi = fmax(hi, sh[1][k]); sum += sh[2][k]; }
+        out[0] = lo; out[1] = hi; out[2] = sum;
+    }
+}
+__global__ void __launch_bounds__(SPHK_HEAT_RED) k_heat_partial(const float* __restrict__ T, const float* __restrict__ m, int n,
+                                                                double* __restrict__ part) {
+    double lo = CUDART_INF, hi = -CUDART_INF, sum = 0.0;
+    for (int i = blockIdx.x * SPHK_HEAT_RED + threadIdx.x; i < n; i += gridDim.x * SPHK_HEAT_RED) {
+        const double t = f2d(T[i]);
+        lo = fmin(lo, t); hi = fmax(hi, t); sum += f2d(m[i]) * t;
+    }
+    heat_block(lo, hi, sum, part + 3 * blockIdx.x);
+}
+__global__ void __launch_bounds__(SPHK_HEAT_RED) k_heat_finish(const double* __restrict__ part, int m, double* __restrict__ out) {
+    double lo = CUDART_INF, hi = -CUDART_INF, sum = 0.0;
+    for (int k = threadIdx.x; k < m; k += SPHK_HEAT_RED) { lo = fmin(lo, part[3 * k]); hi = fmax(hi, part[3 * k + 1]); sum += part[3 * k + 2]; }
+    heat_block(lo, hi, sum, out);
+}
+// nu(T) = clamp(nu_ref exp(-e (T - t_ref)), nu_min, nu_max) in double, rounded once (a NaN lands on nu_max)
+__device__ __forceinline__ float thermal_nu(const sphk_viscosity_law& v, float t) {
+    const double raw = static_cast<double>(v.nu_ref) * exp(-static_cast<double>(v.e) * (f2d(t) - static_cast<double>(v.t_ref)));
+    return d2f_rn(!(raw < static_cast<double>(v.nu_max)) ? static_cast<double>(v.nu_max) : fmax(raw, static_cast<double>(v.nu_min)));
+}
+__global__ void __launch_bounds__(SPHK_BLOCK) k_thermal_nu(sphk_viscosity_law v, const float* __restrict__ T, float* __restrict__ nu,
+                                                           int n) {
+    const int i = blockIdx.x * SPHK_BLOCK + threadIdx.x;
+    if (i < n) nu[i] = thermal_nu(v, T[i]);
+}
+
+static int check_thermal(const sphk_ctx* c, const sphk_thermal* th) {
+    if (!th || !finite_nonneg(th->alpha) || !finite_f(th->beta) || !finite_f(th->t_ref) || th->n_groups < 0 ||
+        th->n_groups > SPHK_THERMAL_GROUPS)
+        return SPHK_ERR_INVALID;
+    for (int g = 0; g < th->n_groups; ++g)
+        if (!finite_f(th->groups[g].t) || !finite_nonneg(th->groups[g].h)) return SPHK_ERR_INVALID;
+    if (c && th->n_groups > 1 + (c->bodies ? c->bodies->nBodies : 0)) return SPHK_ERR_STATE;
+    return SPHK_OK;
+}
+
+extern "C" int sphk_heat_substeps(const sphk_thermal* th, float radius, float dt, int* substeps) {
+    if (!substeps || check_thermal(nullptr, th) != SPHK_OK || !(radius > 0.f) || !finite_nonneg(dt) || radius - radius != 0.f)
+        return SPHK_ERR_INVALID;
+    double hMax = 0.0;
+    for (int g = 0; g < th->n_groups; ++g) hMax = std::max(hMax, static_cast<double>(th->groups[g].h));
+    const double R = radius;
+    const double k = std::ceil(static_cast<double>(dt) * SPHK_HEAT_COP * th->alpha * (1.0 + hMax) / (R * R));
+    if (!(k <= 65536.0)) return SPHK_ERR_INVALID;
+    *substeps = std::max(1, static_cast<int>(k));
+    return SPHK_OK;
+}
+
+// table + statistics reset (substep 0 only), mirror, conduction sweep
+static int heat_sweep(sphk_ctx* c, const sphk_scene* s, const sphk_thermal& th, const float* T, float* dTdt, float dtSub, float rho0,
+                      float rhoB, bool begin) {
+    if (begin) { k_heat_begin<<<1, 96, 0, c->stream>>>(th, c->heatGroups, c->heatStats); c->launches++; }
+    ensure_scalar(c, T);
+    // with bodies every boundary particle's group is read (body b without an entry is adiabatic: the table holds {0, 0} there)
+    const float t0 = th.n_groups > 0 ? th.groups[0].t : 0.f, h0 = th.n_groups > 0 ? th.groups[0].h : 0.f;
+    return run_sweep(c, s, OpHeatConduction{dTdt, c->heatStats, c->bodies ? c->bodies->local : nullptr, c->heatGroups, th.alpha / rho0,
+                                            th.alpha / rhoB, t0, h0, dtSub, c->nB});
+}
+static int check_heat_call(sphk_ctx* c, const sphk_scene* s, const sphk_thermal* th, const float* T, const float* out, float rho0,
+                           float rhoB) {
+    if (!T || !out || T == out || aliases(T, s) || aliases(out, s) || !(rho0 > 0.f) || !(rhoB > 0.f)) return SPHK_ERR_INVALID;
+    const int rc = check_thermal(c, th);
+    if (rc != SPHK_OK) return rc;
+    if (c->actCount >= 0 || c->rangeDev) return SPHK_ERR_STATE;      // slab ranks: ghosts would need their temperatures
+    return SPHK_OK;
+}
+
+extern "C" int sphk_heat_step(sphk_ctx* c, const sphk_scene* s, const sphk_thermal* th, float* T, float* work, float dt, int k,
+                              int substeps, float rho0, float rho_boundary, const float* gravity) {
+    SPHK_CHECK_SCENE(c, s);
+    if (!gravity || !finite_nonneg(dt) || substeps < 1 || k < 0 || k >= substeps) return SPHK_ERR_INVALID;
+    const int rc0 = check_heat_call(c, s, th, T, work, rho0, rho_boundary);
+    if (rc0 != SPHK_OK) return rc0;
+    const float dtSub = dt / static_cast<float>(substeps);
+    const int rc = heat_sweep(c, s, *th, T, work, dtSub, rho0, rho_boundary, k == 0);
+    if (rc != SPHK_OK) return rc;
+    const int n = c->nF;
+    if (n > 0) {
+        const float3 Gdt = make_float3(gravity[0] * dt, gravity[1] * dt, gravity[2] * dt);
+        k_heat_commit<<<sphk_blocks(n), SPHK_BLOCK, 0, c->stream>>>(T, work, c->rec, s->fluid.vel, n, dtSub, k == substeps - 1, th->beta,
+                                                                  th->t_ref, Gdt);
+        c->launches++;
+    }
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+extern "C" int sphk_heat_conduction(sphk_ctx* c, const sphk_scene* s, const sphk_thermal* th, const float* T, float* dtdt_out,
+                                    float dt_sub, float rho0, float rho_boundary) {
+    SPHK_CHECK_SCENE(c, s);
+    if (!finite_nonneg(dt_sub)) return SPHK_ERR_INVALID;
+    const int rc = check_heat_call(c, s, th, T, dtdt_out, rho0, rho_boundary);
+    if (rc != SPHK_OK) return rc;
+    if (c->sTag == dtdt_out) c->sTag = nullptr;
+    return heat_sweep(c, s, *th, T, dtdt_out, dt_sub, rho0, rho_boundary, true);
+}
+
+extern "C" int sphk_heat_stats(sphk_ctx* c, const float* T, const float* mass, int n, float* max_courant, int* violators, float* t_min,
+                               float* t_max, double* heat) {
+    if (!c || n < 0 || (n > 0 && (!T || !mass))) return SPHK_ERR_INVALID;
+    const bool reduce = T && mass && n > 0;
+    if (reduce) {
+        const int m = std::min(std::max((n + 2047) / 2048, 1), 1024);
+        k_heat_partial<<<m, SPHK_HEAT_RED, 0, c->stream>>>(T, mass, n, c->heatRed);
+        k_heat_finish<<<1, SPHK_HEAT_RED, 0, c->stream>>>(c->heatRed, m, c->heatRed + 3 * 1024);
+        c->launches += 2;
+        SPHK_CUDA_TRY(cudaGetLastError());
+    }
+    unsigned int st[2];
+    double red[3] = {0.0, 0.0, 0.0};
+    SPHK_CUDA_TRY(cudaMemcpyAsync(st, c->heatStats, sizeof(st), cudaMemcpyDeviceToHost, c->stream));
+    if (reduce) SPHK_CUDA_TRY(cudaMemcpyAsync(red, c->heatRed + 3 * 1024, sizeof(red), cudaMemcpyDeviceToHost, c->stream));
+    SPHK_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    float cour;
+    memcpy(&cour, &st[0], sizeof(cour));
+    if (max_courant) *max_courant = cour;
+    if (violators) *violators = static_cast<int>(st[1]);
+    if (t_min) *t_min = static_cast<float>(red[0]);
+    if (t_max) *t_max = static_cast<float>(red[1]);
+    if (heat) *heat = red[2];
+    return SPHK_OK;
+}
+
+static int check_thermal_viscosity(const sphk_viscosity_law* v) {
+    if (!v || !finite_nonneg(v->nu_ref) || !finite_f(v->e) || !finite_f(v->t_ref) || !finite_nonneg(v->nu_min) ||
+        !finite_nonneg(v->nu_max) || v->nu_min > v->nu_max)
+        return SPHK_ERR_INVALID;
+    return SPHK_OK;
+}
+
+extern "C" int sphk_thermal_viscosity(sphk_ctx* c, const sphk_scene* s, float* work, float* nu_field, const float* T,
+                                      const sphk_viscosity_law* law, float beta, float dt, float rho0, float rho_boundary, float tol,
+                                      int max_iter) {
+    SPHK_CHECK_SCENE(c, s);
+    if (!work || !nu_field || !T || work == nu_field || T == nu_field || T == work || aliases(work, s) || aliases(nu_field, s) ||
+        !(tol > 0.f) || max_iter < 1 || max_iter > SPHK_IMPLICIT_VISCOSITY_MAX_ITER || check_thermal_viscosity(law) != SPHK_OK)
+        return SPHK_ERR_INVALID;
+    const int rc0 = check_field_common(c, beta, dt, rho0, rho_boundary);
+    if (rc0 != SPHK_OK) return rc0;
+    const int n = c->nF;
+    if (c->sTag == nu_field) c->sTag = nullptr;
+    if (n > 0) { k_thermal_nu<<<sphk_blocks(n), SPHK_BLOCK, 0, c->stream>>>(*law, T, nu_field, n); c->launches++; }
+    const ViscWork w = visc_work(work, n);
+    rheo_mirror(c, nu_field, rho0);
+    const int rc = run_sweep(c, s, OpViscImplicitSetupField{OpViscImplicitSetup{w.D, w.Dinv, w.r, 0.f, 0.f, dt}, nu_field, beta, rho_boundary});
+    if (rc != SPHK_OK) return rc;
+    return visc_pcg(c, s, w, OpViscImplicitMatvecField{w.D, w.Ap, dt}, tol, max_iter, c->viscStats);
+}
+
+extern "C" int sphk_thermal_viscosity_eval(sphk_ctx* c, const sphk_viscosity_law* law, const float* T, float* nu_out, int n) {
+    if (!c || !T || !nu_out || T == nu_out || n < 0 || check_thermal_viscosity(law) != SPHK_OK) return SPHK_ERR_INVALID;
+    if (n == 0) return SPHK_OK;
+    if (c->sTag == nu_out) c->sTag = nullptr;
+    k_thermal_nu<<<sphk_blocks(n), SPHK_BLOCK, 0, c->stream>>>(*law, T, nu_out, n);
+    c->launches++;
     SPHK_CUDA_TRY(cudaGetLastError());
     return SPHK_OK;
 }

@@ -84,8 +84,10 @@ class SphkOps:
     list_capacity = 96               # SPHK_OPT_LIST_CAPACITY of ctx (set_option keeps it current)
     vorticity_eps = 0.0              # vorticity confinement strength (BasicSPHSolver::setVorticityConfinement); 0: off
     implicit_nu = 0.0                # implicit viscosity (BasicSPHSolver::setImplicitViscosity); 0: off
-    rheology = None                  # non-Newtonian viscosity (BasicSPHSolver::setRheology): a dict for capi.rheology plus beta,
-                                     # tol, max_iter; replaces the implicit_nu solve.  None: off
+    _thermal = None
+    _thermal_viscosity = None
+    _rheology = None
+    heat_substeps = 0                # conduction substeps of the last step
     implicit_nu_boundary = 0.0
     implicit_tol = 1e-4
     implicit_max_iter = 20
@@ -432,6 +434,101 @@ class SphkOps:
         check(self.L.sphk_visc_field_matvec(self.ctx, self._s(), _ptr(d_in), _ptr(p_in), _ptr(ap_out), _ptr(nu), C.c_float(self.dt),
                                             C.c_float(self.p.rho0)), "sphk_visc_field_matvec")
 
+    # ---- heat transfer (no reference counterpart; DESIGN.md section 2.10) -------------------------------------------------
+    @property
+    def rheology(self):
+        """non-Newtonian viscosity (BasicSPHSolver::setRheology): a dict for capi.rheology plus beta, tol, max_iter; replaces the
+        implicit_nu solve.  None: off.  Refused (ValueError) while `thermal_viscosity` is set."""
+        return self._rheology
+
+    @rheology.setter
+    def rheology(self, spec):
+        if spec is not None and self._thermal_viscosity is not None:
+            raise ValueError("a rheology is not supported together with a temperature-dependent viscosity")
+        self._rheology = spec
+
+    @property
+    def thermal_viscosity(self):
+        """temperature-dependent viscosity (BasicSPHSolver::setThermalViscosity): dict(nu_ref, e, nu_max, nu_min, wall_factor, tol,
+        max_iter), solved instead of the implicit_nu solve while `thermal` is set.  Refused (ValueError) while `rheology` is set."""
+        return self._thermal_viscosity
+
+    @thermal_viscosity.setter
+    def thermal_viscosity(self, spec):
+        if spec is not None and self._rheology is not None:
+            raise ValueError("a temperature-dependent viscosity is not supported together with a rheology")
+        self._thermal_viscosity = spec
+
+    @property
+    def thermal(self):
+        """heat transfer (BasicSPHSolver::setThermal): a dict for capi.thermal plus "emitters": [T, ...]; None: off.  The first
+        setting allocates `temperature` (capacity-sized, the fluid's current order) filled with t_ref."""
+        return self._thermal
+
+    @thermal.setter
+    def thermal(self, spec):
+        if spec is not None:
+            t = capi.thermal(spec)
+            if len(spec.get("bodies", ())) > self.n_bodies:
+                raise ValueError(f"{len(spec['bodies'])} body entries, but the system has {self.n_bodies} bodies")
+            if self.L.sphk_heat_substeps(C.byref(t), C.c_float(self.p.radius), C.c_float(0.0), C.byref(C.c_int(0))):
+                raise ValueError(f"thermal setting refused: {spec}")
+            if getattr(self, "temperature", None) is None:
+                n = self.buffer3.shape[0]
+                self.temperature = torch.full((n,), float(np.float32(t.t_ref)), dtype=torch.float32, device=self.device)
+                self.heat_work = torch.zeros(n, dtype=torch.float32, device=self.device)
+            self._thermal_abi = t
+        self._thermal = spec
+
+    def heat(self):
+        """the heat stage of one step: sphk_heat_substeps, then that many sphk_heat_step"""
+        k = C.c_int(1)
+        check(self.L.sphk_heat_substeps(C.byref(self._thermal_abi), C.c_float(self.p.radius), C.c_float(self.dt), C.byref(k)),
+              "sphk_heat_substeps")
+        self.heat_substeps = k.value
+        g = (C.c_float * 3)(*[float(x) for x in self.p.gravity])
+        for j in range(k.value):
+            check(self.L.sphk_heat_step(self.ctx, self._s(), C.byref(self._thermal_abi), _ptr(self.temperature), _ptr(self.heat_work),
+                                        C.c_float(self.dt), C.c_int(j), C.c_int(k.value), C.c_float(self.p.rho0),
+                                        C.c_float(self.p.rho_boundary), g), "sphk_heat_step")
+
+    def heat_conduction(self, temperature, out, dt_sub=0.0, spec=None):
+        """dT/dt (n) of the conduction sweep alone (and its statistics with dt_sub)"""
+        t = capi.thermal(spec) if spec is not None else self._thermal_abi
+        check(self.L.sphk_heat_conduction(self.ctx, self._s(), C.byref(t), _ptr(temperature), _ptr(out), C.c_float(dt_sub),
+                                          C.c_float(self.p.rho0), C.c_float(self.p.rho_boundary)), "sphk_heat_conduction")
+
+    def thermal_stats(self) -> dict:
+        """as capi.SphApp.thermal_stats; synchronises"""
+        cmax, v, lo, hi, q = C.c_float(0), C.c_int(0), C.c_float(0), C.c_float(0), C.c_double(0)
+        t = getattr(self, "temperature", None)
+        n = self.fluid.n if t is not None else 0
+        check(self.L.sphk_heat_stats(self.ctx, _ptr(t) if n else None, _ptr(self.fluid.mass) if n else None, C.c_int(n), C.byref(cmax), C.byref(v),
+                                     C.byref(lo), C.byref(hi), C.byref(q)), "sphk_heat_stats")
+        return {"substeps": self.heat_substeps, "max_courant": cmax.value, "violators": v.value, "t_min": lo.value, "t_max": hi.value,
+                "heat": q.value}
+
+    def _thermal_law(self, spec=None):
+        spec = self.thermal_viscosity if spec is None else spec
+        o = dict(capi.THERMAL_VISCOSITY_DEFAULTS, **{k: spec[k] for k in capi.THERMAL_VISCOSITY_DEFAULTS if k in spec})
+        return capi.viscosity_law(spec, self._thermal_abi.t_ref), o
+
+    def thermal_viscosity_solve(self):
+        """the nu(T) solve with the `thermal_viscosity` setting, from the current temperatures"""
+        law, o = self._thermal_law()
+        if getattr(self, "nu_field", None) is None:
+            self.nu_field = torch.zeros(self.buffer3.shape[0], dtype=torch.float32, device=self.device)
+        work, nu = self._visc_work(), _ptr(self.nu_field)
+        check(self.L.sphk_thermal_viscosity(self.ctx, self._s(), work, nu, _ptr(self.temperature), C.byref(law),
+                                            C.c_float(o["wall_factor"]), C.c_float(self.dt), C.c_float(self.p.rho0),
+                                            C.c_float(self.p.rho_boundary), C.c_float(o["tol"]), C.c_int(int(o["max_iter"]))),
+              "sphk_thermal_viscosity")
+
+    def thermal_viscosity_eval(self, spec, t_ref, temperature, nu_out):
+        law = capi.viscosity_law(spec, t_ref)
+        check(self.L.sphk_thermal_viscosity_eval(self.ctx, C.byref(law), _ptr(temperature), _ptr(nu_out), C.c_int(temperature.numel())),
+              "sphk_thermal_viscosity_eval")
+
     def pressure(self):
         check(self.L.sphk_pressure(self.ctx, self._s(), C.c_float(self.p.rho0), C.c_float(self.p.stiff)), "sphk_pressure")
 
@@ -544,13 +641,23 @@ class SphkOps:
                 self._run(self.surface, "vel")
         if self.rheology is not None:       # replaces the constant-nu solve
             self._run(self.non_newtonian_viscosity, "vel")
+        elif self.thermal is not None and self.thermal_viscosity is not None:
+            self._run(self.thermal_viscosity_solve, "vel")
         elif self.implicit_nu > 0:
             self._run(self.implicit_viscosity, "vel")
         if vort:
             self._run(self.vorticity_confinement, "vel")
+        if self.thermal is not None:
+            self._run(self.heat, "vel")
+
+    def _carry_temperature(self):
+        """the temperatures follow their particles through this step's search (BasicSPHSolver::beginStep)"""
+        if self.thermal is not None:
+            self.permute(self.temperature, 1)
 
     def step_wcsph(self):            # BasicSPHSolver.cu:237-260
         self.set_use_list(self.use_list)
+        self._carry_temperature()
         self.gravity()
         if self.fused:               # density (+ colour gradient) before the velocity terms: it reads positions and masses only
             if self._surface_enabled():
@@ -568,6 +675,7 @@ class SphkOps:
 
     def step_dfsph(self):            # DFSPHSolver.cu:33-72
         self.set_use_list(self.use_list)
+        self._carry_temperature()
         n, rho0 = self.n_total(), self.p.rho0
         if self.fused:               # density/alpha (+ colour gradient) + the first divergence error (:341) in one sweep
             surface = self._surface_enabled()
@@ -613,6 +721,7 @@ class SphkOps:
             self.pos_last_init = True
             return False
         self.set_use_list(self.use_list, 150 if self.use_list else 0)   # skin list: positions move inside the step
+        self._carry_temperature()
         self.permute(self.pos_last, 3)
         c = np.float32(1.0) / (np.float32(self.p.rho0) * np.float32(self.pbd_dt_prev()))
         for _ in range(self.max_iter):
@@ -667,6 +776,10 @@ class SphkOps:
                 continue
             check(self.L.sphk_emit(self.ctx, C.byref(p), C.c_int(n + e), C.byref(em), C.c_int(layers), off, C.c_float(self.p.m0),
                                    C.c_float(hist_dt), _ptr(hist), C.c_int(kind)), "sphk_emit")
+            if self.thermal is not None:     # the emitter's temperature (default t_ref) into its new slots
+                ts = self.thermal.get("emitters", [])
+                check(self.L.sphk_fill(self.ctx, _ptr(self.temperature[n + e:]), C.c_int(layers * per),
+                                       C.c_float(ts[k] if k < len(ts) else self._thermal_abi.t_ref)), "sphk_fill")
             e += layers * per
             self._open_stats["emitted"] += layers * per
         return e

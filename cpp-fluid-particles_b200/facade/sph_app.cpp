@@ -553,6 +553,88 @@ extern "C" int sph_app_download_viscosity(sph_app* app, float* nu_host) {
 #endif
 }
 
+extern "C" int sph_app_set_thermal(sph_app* app, int on, float alpha, float beta, float t_ref, float wall_t, float wall_h, int n_bodies,
+                                   const float* body_t_h, int n_emitters, const float* emitter_t) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)on; (void)alpha; (void)beta; (void)t_ref; (void)wall_t; (void)wall_h; (void)n_bodies; (void)body_t_h;
+    (void)n_emitters; (void)emitter_t;
+    return 1;
+#else
+    auto* b = dynamic_cast<BasicSPHSolver*>(app->solver);
+    if (!b) return 1;
+    if (!on) {
+        b->clearThermal();
+        return 0;
+    }
+    if (n_bodies < 0 || n_emitters < 0 || (n_bodies > 0 && !body_t_h) || (n_emitters > 0 && !emitter_t)) return 1;
+    sphb200::Thermal t;
+    t.alpha = alpha; t.beta = beta; t.Tref = t_ref; t.wall = {wall_t, wall_h};
+    for (int k = 0; k < n_bodies; ++k) t.bodies.push_back({body_t_h[2 * k], body_t_h[2 * k + 1]});
+    t.emitterT.assign(emitter_t, emitter_t + n_emitters);
+    return b->setThermal(t) ? 0 : 1;        // (refused: the setting is kept)
+#endif
+}
+
+extern "C" int sph_app_set_thermal_viscosity(sph_app* app, int on, float nu_ref, float e, float nu_min, float nu_max, float wall_factor,
+                                             float tol, int max_iter) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)on; (void)nu_ref; (void)e; (void)nu_min; (void)nu_max; (void)wall_factor; (void)tol; (void)max_iter;
+    return 1;
+#else
+    auto* b = dynamic_cast<BasicSPHSolver*>(app->solver);
+    if (!b) return 1;
+    if (!on) {
+        b->clearThermalViscosity();
+        return 0;
+    }
+    sphb200::ThermalViscosity v;
+    v.nuRef = nu_ref; v.E = e; v.nuMin = nu_min; v.nuMax = nu_max; v.wallFactor = wall_factor; v.tol = tol; v.maxIter = max_iter;
+    return b->setThermalViscosity(v) ? 0 : 1;
+#endif
+}
+
+extern "C" int sph_app_upload_temperature(sph_app* app, const float* t_host) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)t_host;
+    return 1;
+#else
+    auto* b = dynamic_cast<BasicSPHSolver*>(app->solver);
+    if (!b || !t_host) return 1;
+    const size_t n = app->system->getFluids()->size();
+    return cudaMemcpy(b->temperatureField().addr(), t_host, n * sizeof(float), cudaMemcpyHostToDevice) == cudaSuccess ? 0 : 1;
+#endif
+}
+
+extern "C" int sph_app_download_temperature(sph_app* app, float* t_host) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)t_host;
+    return 1;
+#else
+    auto* b = dynamic_cast<BasicSPHSolver*>(app->solver);
+    if (!b || !t_host) return 1;
+    return d2h(t_host, b->temperatureField().addr(), app->system->getFluids()->size() * sizeof(float));
+#endif
+}
+
+extern "C" int sph_app_thermal_stats(sph_app* app, int* substeps, float* max_courant, int* violators, float* t_min, float* t_max,
+                                     double* heat) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)substeps; (void)max_courant; (void)violators; (void)t_min; (void)t_max; (void)heat;
+    return 1;
+#else
+    auto* b = dynamic_cast<BasicSPHSolver*>(app->solver);
+    if (!b) return 1;
+    const sphb200::ThermalStats s = b->lastThermalStats();
+    if (substeps) *substeps = s.substeps;
+    if (max_courant) *max_courant = s.maxCourant;
+    if (violators) *violators = s.violators;
+    if (t_min) *t_min = s.Tmin;
+    if (t_max) *t_max = s.Tmax;
+    if (heat) *heat = s.heat;
+    return 0;
+#endif
+}
+
 extern "C" int sph_app_set_adaptive_dt(sph_app* app, float C, float dt_min, float dt_max) {
 #ifdef SPH_APP_REFERENCE_ENGINE
     (void)app; (void)C; (void)dt_min; (void)dt_max;

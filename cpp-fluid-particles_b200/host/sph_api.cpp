@@ -78,9 +78,12 @@ bool BasicSPHSolver::beginStep(std::shared_ptr<SPHParticles>& fluids, const std:
     current_.abi.cell_start_boundary = cellStartBoundary.addr();
     current_.abi.radius = radius;
     reacting_ = eng->bodiesDynamic;
+    bodies_ = eng->bodies;
     check(sphk_set_option(current_.ctx, SPHK_OPT_NEIGHBOR_LIST, neighborList ? 1 : 0), "sphk_set_option");
     check(sphk_set_option(current_.ctx, SPHK_OPT_LIST_SKIN, listSkinPermille), "sphk_set_option");
     if (eng->shadowsStale) { check(sphk_refresh(current_.ctx, &current_.abi), "sphk_refresh"); eng->shadowsStale = false; }
+    // the temperatures follow their particles through the search of this step (once per search, like the solvers' history arrays)
+    if (thermalOn_) check(sphk_permute(current_.ctx, temperature_->addr(), 1, static_cast<int>(fluids->size())), "sphk_permute");
     return true;
 }
 
@@ -102,7 +105,7 @@ void BasicSPHSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shar
         }
     }
     velocityStage(fluids, boundaries, cellStartFluid, cellStartBoundary, cellSize, cellLength, radius, rho0, rhoB, visc, dt,
-                  surfaceTensionIntensity, airPressure, false);
+                  surfaceTensionIntensity, airPressure, false, G);
     if (fusedSweeps_) {
         check(sphk_pressure(current_.ctx, &current_.abi, rho0, stiff), "sphk_pressure");
         produced(0, fluids->getDensityPtr(), 1); produced(0, fluids->getPressurePtr(), 1);
@@ -120,7 +123,7 @@ void BasicSPHSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shar
 void BasicSPHSolver::velocityStage(std::shared_ptr<SPHParticles>& fluids, const std::shared_ptr<SPHParticles>& boundaries,
                                    const DArray<int>& cellStartFluid, const DArray<int>& cellStartBoundary, int3 cellSize,
                                    float cellLength, float radius, float rho0, float rhoB, float visc, float dt,
-                                   float surfaceTensionIntensity, float airPressure, bool xsph) {
+                                   float surfaceTensionIntensity, float airPressure, bool xsph, float3 G) {
     const bool surface = surfaceTensionIntensity > EPSILON || airPressure > EPSILON;
     float* dv = reinterpret_cast<float*>(bufferFloat3.addr());
     float* cg = colorGradBuffer();
@@ -161,8 +164,10 @@ void BasicSPHSolver::velocityStage(std::shared_ptr<SPHParticles>& fluids, const 
                           dt, surfaceTensionIntensity, airPressure);
     }
     if (rheoOn_) rheology(fluids, rho0, rhoB, dt);        // replaces the constant-nu solve
+    else if (thermalOn_ && thermalViscOn_) thermalViscosity(fluids, rho0, rhoB, dt);
     else if (implicitViscosityOn()) implicitViscosity(fluids, rho0, rhoB, dt);
     if (vorticityOn()) confine(fluids, rho0, dt);
+    if (thermalOn_) heat(fluids, rho0, rhoB, dt, G);
 }
 
 // addition (no reference counterpart): vorticity confinement, sphk.h
@@ -241,6 +246,10 @@ bool BasicSPHSolver::setRheology(const sphb200::Rheology& r, float boundaryFacto
                "tol > 0 and 1 <= maxIter <= %d; the setting is kept\n", SPHK_IMPLICIT_VISCOSITY_MAX_ITER);
         return false;
     }
+    if (thermalViscOn_) {
+        printf("setRheology: not together with a temperature-dependent viscosity; the setting is kept\n");
+        return false;
+    }
     if (boundaryFactor > 0.0f && reacting_) {
         printf("setRheology: boundaryFactor > 0 is not supported with dynamic bodies (the viscous wall force is not part of their "
                "reaction); the setting is kept\n");
@@ -278,6 +287,111 @@ sphb200::RheologyStats BasicSPHSolver::lastRheologyStats() const {
     if (current_.ctx)
         check(sphk_non_newtonian_stats(current_.ctx, &s.iterations, &s.residual, &s.gammaMax, &s.nuMin, &s.nuMax, &s.atNuMax),
               "sphk_non_newtonian_stats");
+    return s;
+}
+
+// addition (no reference counterpart): heat transfer, sphk.h
+static bool finiteNonneg(float x) { return std::isfinite(x) && x >= 0.0f; }
+
+bool BasicSPHSolver::setThermal(const sphb200::Thermal& t) {
+    bool ok = finiteNonneg(t.alpha) && std::isfinite(t.beta) && std::isfinite(t.Tref) && std::isfinite(t.wall.T) && finiteNonneg(t.wall.h) &&
+              t.bodies.size() <= SPHK_BODY_LIMIT;
+    for (const auto& g : t.bodies) ok = ok && std::isfinite(g.T) && finiteNonneg(g.h);
+    for (float T : t.emitterT) ok = ok && std::isfinite(T);
+    if (!ok) {
+        printf("setThermal: need alpha >= 0, finite beta, Tref and temperatures, conductances h >= 0 (finite) and at most %d bodies; "
+               "the setting is kept\n", SPHK_BODY_LIMIT);
+        return false;
+    }
+    if (bodies_ >= 0 && static_cast<int>(t.bodies.size()) > bodies_) {
+        printf("setThermal: %d body entries, but the system has %d bodies; the setting is kept\n", static_cast<int>(t.bodies.size()),
+               bodies_);
+        return false;
+    }
+    if (!temperatureSet_) {
+        const std::vector<float> init(static_cast<size_t>(num_), t.Tref);
+        CUDA_CALL(cudaMemcpy(temperatureField().addr(), init.data(), sizeof(float) * init.size(), cudaMemcpyHostToDevice));
+        temperatureSet_ = true;
+    }
+    sphk_thermal a{};
+    a.alpha = t.alpha; a.beta = t.beta; a.t_ref = t.Tref;
+    a.n_groups = 1 + static_cast<int>(t.bodies.size());
+    a.groups[0] = {t.wall.T, t.wall.h};
+    for (size_t b = 0; b < t.bodies.size(); ++b) a.groups[b + 1] = {t.bodies[b].T, t.bodies[b].h};
+    if (!thermalOn_ || std::memcmp(&a, &thermalAbi_, sizeof(a)) != 0) ++configEpoch_;
+    thermalOn_ = true; thermal_ = t; thermalAbi_ = a;
+    return true;
+}
+
+void BasicSPHSolver::clearThermal() {
+    if (thermalOn_) ++configEpoch_;
+    thermalOn_ = false;
+}
+
+DArray<float>& BasicSPHSolver::temperatureField() {
+    if (!temperature_) {
+        temperature_ = std::make_unique<DArray<float>>(static_cast<unsigned int>(num_));
+        heatWork_ = std::make_unique<DArray<float>>(static_cast<unsigned int>(num_));
+    }
+    return *temperature_;
+}
+
+bool BasicSPHSolver::setThermalViscosity(const sphb200::ThermalViscosity& v) {
+    if (!finiteNonneg(v.nuRef) || !std::isfinite(v.E) || !finiteNonneg(v.nuMin) || !finiteNonneg(v.nuMax) || v.nuMin > v.nuMax ||
+        !finiteNonneg(v.wallFactor) || !(v.tol > 0.0f) || v.maxIter < 1 || v.maxIter > SPHK_IMPLICIT_VISCOSITY_MAX_ITER) {
+        printf("setThermalViscosity: need nuRef >= 0, finite E, 0 <= nuMin <= nuMax (finite), wallFactor >= 0, tol > 0 and 1 <= maxIter "
+               "<= %d; the setting is kept\n", SPHK_IMPLICIT_VISCOSITY_MAX_ITER);
+        return false;
+    }
+    if (rheoOn_) {
+        printf("setThermalViscosity: not together with a shear-rate rheology; the setting is kept\n");
+        return false;
+    }
+    if (v.wallFactor > 0.0f && reacting_) {
+        printf("setThermalViscosity: wallFactor > 0 is not supported with dynamic bodies (the viscous wall force is not part of their "
+               "reaction); the setting is kept\n");
+        return false;
+    }
+    if (!viscWork_)
+        viscWork_ = std::make_unique<DArray<float>>(static_cast<unsigned int>(sphk_implicit_viscosity_work_floats(num_)));
+    viscosityField();
+    if (!thermalViscOn_ || std::memcmp(&v, &thermalVisc_, sizeof(v)) != 0) ++configEpoch_;
+    thermalViscOn_ = true; thermalVisc_ = v;
+    return true;
+}
+
+void BasicSPHSolver::clearThermalViscosity() {
+    if (thermalViscOn_) ++configEpoch_;
+    thermalViscOn_ = false;
+}
+
+void BasicSPHSolver::thermalViscosity(const std::shared_ptr<SPHParticles>& fluids, float rho0, float rhoB, float dt) {
+    const sphb200::ThermalViscosity& v = thermalVisc_;
+    const sphk_viscosity_law law{v.nuRef, v.E, thermal_.Tref, v.nuMin, v.nuMax};
+    check(sphk_thermal_viscosity(current_.ctx, &current_.abi, viscWork_->addr(), nuField_->addr(), temperature_->addr(), &law,
+                                 v.wallFactor, dt, rho0, rhoB, v.tol, v.maxIter),
+          "sphk_thermal_viscosity");
+    producedVel(fluids);
+}
+
+void BasicSPHSolver::heat(const std::shared_ptr<SPHParticles>& fluids, float rho0, float rhoB, float dt, float3 G) {
+    int k = 1;
+    check(sphk_heat_substeps(&thermalAbi_, current_.abi.radius, dt, &k), "sphk_heat_substeps");
+    heatSubsteps_ = k;
+    const float g[3] = {G.x, G.y, G.z};
+    for (int j = 0; j < k; ++j)
+        check(sphk_heat_step(current_.ctx, &current_.abi, &thermalAbi_, temperature_->addr(), heatWork_->addr(), dt, j, k, rho0, rhoB, g),
+              "sphk_heat_step");
+    producedVel(fluids);
+}
+
+sphb200::ThermalStats BasicSPHSolver::lastThermalStats() {
+    sphb200::ThermalStats s;
+    s.substeps = heatSubsteps_;
+    if (current_.ctx && temperature_)
+        check(sphk_heat_stats(current_.ctx, temperature_->addr(), current_.abi.fluid.mass, current_.abi.fluid.n, &s.maxCourant,
+                              &s.violators, &s.Tmin, &s.Tmax, &s.heat),
+              "sphk_heat_stats");
     return s;
 }
 
@@ -350,7 +464,7 @@ void DFSPHSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shared_
     itDiv_ = correctDivergenceError(rho0, dt, divergenceErrorThreshold, maxIter, num, fusedSweeps_);
     force(fluids, dt, G);
     velocityStage(fluids, boundaries, cellStartFluid, cellStartBoundary, cellSize, cellLength, radius, rho0, rhoB, visc, dt,
-                  surfaceTensionIntensity, airPressure, false);
+                  surfaceTensionIntensity, airPressure, false, G);
     itDen_ = project(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, cellSize, cellLength, radius, dt,
                      densityErrorThreshold, maxIter);
     advect(fluids, dt, spaceSize);
@@ -490,7 +604,7 @@ void PBDSolver::step(std::shared_ptr<SPHParticles>& fluids, const std::shared_pt
     check(sphk_pbd_velocity_from_positions(current_.ctx, &current_.abi, reinterpret_cast<float*>(fluidPosLast.addr()), dtPrev),
           "sphk_pbd_velocity_from_positions");
     velocityStage(fluids, boundaries, cellStartFluid, cellStartBoundary, cellSize, cellLength, radius, rho0, rhoB, xSPH_c, dt,
-                  surfaceTensionIntensity, airPressure, true);
+                  surfaceTensionIntensity, airPressure, true, G);
     force(fluids, dt, G);
     predict(fluids, dt, spaceSize);
 }
@@ -627,7 +741,7 @@ SPHSystem::SPHSystem(std::shared_ptr<SPHParticles>& fluidParticles, std::shared_
         const int rc = sphk_bodies_init(_engine->ctx(), &bp, nStatic, static_cast<int>(bodies.size()), begin.data(),
                                         local.data(), pose.data(), motion.data());
         check(rc, "sphk_bodies_init");
-        if (rc == 0) _bodyMotion = motion;
+        if (rc == 0) { _bodyMotion = motion; _engine->bodies = static_cast<int>(bodies.size()); }
         const bool dynamic = std::any_of(bodies.begin(), bodies.end(), [](const sphb200::KinematicBody& b) { return b.mass > 0.0f; });
         if (rc == 0 && dynamic) {
             std::vector<float> mi;
@@ -717,6 +831,11 @@ int SPHSystem::openEmit(int n) {
         _openStats.refused += static_cast<long long>(scheduled - layers) * per;
         if (layers == 0) continue;
         check(sphk_emit(ctx, &f, n + e, &em, layers, _layerOffsets.data(), _sphM0, historyDt, kind ? history : nullptr, kind), "sphk_emit");
+        if (solver->thermalOn()) {          // the emitter's temperature (default Tref) into its new slots
+            const sphb200::Thermal& th = solver->thermal();
+            check(sphk_fill(ctx, solver->temperatureField().addr(n + e), layers * per, k < th.emitterT.size() ? th.emitterT[k] : th.Tref),
+                  "sphk_fill");
+        }
         e += layers * per;
         _openStats.emitted += static_cast<long long>(layers) * per;
     }

@@ -62,6 +62,7 @@ public:
     bool ok() const { return ctx_ != nullptr; }
     bool shadowsStale = false;   // set when a caller moved particles behind the engine's back
     bool bodiesDynamic = false;  // set by SPHSystem: the solvers follow every reacting sweep with sphk_bodies_react
+    int bodies = 0;              // set by SPHSystem: the bodies of the context (sphk_bodies_init)
 private:
     sphk_ctx* ctx_ = nullptr;
     cudaStream_t stream_ = nullptr;
@@ -134,6 +135,32 @@ struct RheologyStats {
     float gammaMax = 0.0f;           // largest shear rate
     float nuMin = 0.0f, nuMax = 0.0f;
     int atNuMax = 0;                 // particles at the nuMax clamp (the unyielded part of a yield-stress fluid)
+};
+// addition: heat transfer (DESIGN.md section 2.10; sphk_thermal in sphk.h).  Temperatures in the user's units.
+struct ThermalGroup {
+    float T = 0.0f;                  // temperature of the group's boundary particles
+    float h = 0.0f;                  // relative conductance >= 0 (0: adiabatic)
+};
+struct Thermal {
+    float alpha = 0.0f;              // diffusivity >= 0
+    float beta = 0.0f;               // buoyancy: dv = -beta (T - Tref) G dt
+    float Tref = 0.0f;               // temperature without buoyancy; the initial and the default emitted temperature
+    ThermalGroup wall;               // the static walls (default adiabatic)
+    std::vector<ThermalGroup> bodies;    // body b (missing entries: adiabatic); at most SPHK_BODY_LIMIT
+    std::vector<float> emitterT;     // temperature of emitter k's particles (missing entries: Tref)
+};
+// nu_i = clamp(nuRef exp(-E (T_i - Tref)), nuMin, nuMax), solved like a rheology (section 2.9); walls act with wallFactor nu_i
+struct ThermalViscosity {
+    float nuRef = 0.0f, E = 0.0f, nuMin = 0.0f, nuMax = 0.0f;
+    float wallFactor = 0.0f, tol = 1e-4f;
+    int maxIter = 20;
+};
+struct ThermalStats {
+    int substeps = 0;                // conduction substeps of the last step
+    float maxCourant = 0.0f;         // largest dt_k sum_j c_ij of the last step (<= 1 keeps the maximum principle)
+    int violators = 0;               // particle-substeps of the last step above 1
+    float Tmin = 0.0f, Tmax = 0.0f;  // over the live fluid particles
+    double heat = 0.0;               // sum m T
 };
 }  // namespace sphb200
 
@@ -278,6 +305,25 @@ public:
     const DArray<float>& viscosityField() const;
     // statistics of the last solve (zeros before the first); synchronises
     sphb200::RheologyStats lastRheologyStats() const;
+    // addition: heat transfer (DESIGN.md section 2.10).  When set, the last term of every step's velocity stage conducts heat in
+    // explicit substeps (sphk_heat_substeps) and applies the Boussinesq buoyancy.  A negative or non-finite alpha, a non-finite
+    // beta or Tref, a group with a non-finite T or h < 0, more than SPHK_BODY_LIMIT bodies and (after the first step) more body
+    // entries than the system has bodies are refused (printed, setting kept; returns false).  Bodies without an entry are adiabatic.
+    // The first setting fills temperatureField() with Tref (values written into it before are replaced).
+    bool setThermal(const sphb200::Thermal& t);
+    void clearThermal();
+    bool thermalOn() const { return thermalOn_; }
+    const sphb200::Thermal& thermal() const { return thermal_; }
+    // T_i, device, sized by capacity, in the fluid's current order (permuted with the particles every step while heat transfer is
+    // on); the caller may write it between steps
+    DArray<float>& temperatureField();
+    // statistics of the last step's conduction and of the current temperatures; synchronises
+    sphb200::ThermalStats lastThermalStats();
+    // temperature-dependent viscosity, solved instead of the constant-nu solve while heat transfer is on, from the temperatures the
+    // previous step ended with.  Refused (printed, setting kept, false) for values out of range, together with a rheology, and
+    // wallFactor > 0 with dynamic bodies.  Its iterations are lastViscosityIterations().
+    bool setThermalViscosity(const sphb200::ThermalViscosity& v);
+    void clearThermalViscosity();
     // addition: true when step() enqueues the same kernel sequence every call and never synchronises the host.
     // Only the three shipped solver types can say so: a user-derived solver (the reference API allows subclassing
     // BasicSPHSolver) has per-step host logic of its own, so it is never captured into a step graph.
@@ -323,12 +369,12 @@ protected:
     };
     StepScene current_;
     // the velocity terms of every solver's step, in this order: vorticity omega, viscosity (xsph: PBD's XSPH with coefficient
-    // visc), surface tension, implicit viscosity, vorticity confinement.  With fused sweeps and xsph false the colour gradient
+    // visc), surface tension, implicit viscosity, vorticity confinement, heat transfer (with buoyancy along G).  With fused sweeps and xsph false the colour gradient
     // must be in colorGradBuffer() already (the density sweep computes it).
     void velocityStage(std::shared_ptr<SPHParticles>& fluids, const std::shared_ptr<SPHParticles>& boundaries,
                        const DArray<int>& cellStartFluid, const DArray<int>& cellStartBoundary, int3 cellSize, float cellLength,
                        float radius, float rho0, float rhoB, float visc, float dt, float surfaceTensionIntensity, float airPressure,
-                       bool xsph);
+                       bool xsph, float3 G);
     bool fusedSweeps_ = true;
     unsigned int configEpoch_ = 0;
     FieldHook fieldHook_;
@@ -372,6 +418,16 @@ private:
     std::unique_ptr<DArray<float>> rheoWork_;    // workspace of sphk_non_newtonian_viscosity
     mutable std::unique_ptr<DArray<float>> nuField_;   // nu_i (zeros until the first solve)
     void rheology(const std::shared_ptr<SPHParticles>& fluids, float rho0, float rhoB, float dt);
+    bool thermalOn_ = false, thermalViscOn_ = false;
+    bool temperatureSet_ = false;    // temperature_ holds temperatures (filled with Tref by the first setThermal)
+    int bodies_ = -1;                // bodies of the engine of the last step (-1: no step yet)
+    sphb200::Thermal thermal_;
+    sphb200::ThermalViscosity thermalVisc_;
+    sphk_thermal thermalAbi_{};      // thermal_ as the C-ABI takes it
+    std::unique_ptr<DArray<float>> temperature_, heatWork_;
+    int heatSubsteps_ = 0;
+    void heat(const std::shared_ptr<SPHParticles>& fluids, float rho0, float rhoB, float dt, float3 G);
+    void thermalViscosity(const std::shared_ptr<SPHParticles>& fluids, float rho0, float rhoB, float dt);
 };
 
 // ---- DFSPHSolver.h:20-64 ----------------------------------------------------------------------

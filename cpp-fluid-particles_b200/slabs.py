@@ -1000,6 +1000,16 @@ class SlabSystem(SphkOps):
         if spec is not None:
             raise ValueError("non-Newtonian viscosity is not supported on slab ranks (single-GPU engine.SphkSystem only)")
 
+    # heat transfer: ghosts and strays would need their temperatures carried as a second array
+    @property
+    def thermal(self):
+        return None
+
+    @thermal.setter
+    def thermal(self, spec):
+        if spec is not None:
+            raise ValueError("heat transfer is not supported on slab ranks (single-GPU engine.SphkSystem only)")
+
     def step(self):
         self._step_no += 1
         if self.stray_cap and self._ranges is not None:

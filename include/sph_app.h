@@ -98,6 +98,22 @@ int   sph_app_rheology_stats(sph_app* app, int* iterations, float* rel_residual,
                              int* n_at_max);
 /* nu_i of the last non-Newtonian solve (float[fluid size]; zeros before the first); 1 on the reference build */
 int   sph_app_download_viscosity(sph_app* app, float* nu_host);
+/* Heat transfer in every following step (BasicSPHSolver::setThermal; DESIGN.md section 2.10): diffusivity alpha, buoyancy
+ * dv = -beta (T - t_ref) G dt, the static walls at wall_t with conductance wall_h (0: adiabatic), body b at body_t_h[2b] with
+ * conductance body_t_h[2b+1], emitter k's particles at emitter_t[k] (missing: t_ref).  on = 0: off.  Returns 1 on the reference
+ * build and for a setting the class layer refuses (the setting is then kept). */
+int   sph_app_set_thermal(sph_app* app, int on, float alpha, float beta, float t_ref, float wall_t, float wall_h, int n_bodies,
+                          const float* body_t_h, int n_emitters, const float* emitter_t);
+/* nu = clamp(nu_ref exp(-e (T - t_ref)), nu_min, nu_max) solved instead of the constant-nu solve while heat transfer is on
+ * (BasicSPHSolver::setThermalViscosity); on = 0: off.  1 on the reference build and for a refused setting. */
+int   sph_app_set_thermal_viscosity(sph_app* app, int on, float nu_ref, float e, float nu_min, float nu_max, float wall_factor,
+                                    float tol, int max_iter);
+/* the fluid's temperatures (float[fluid size], the fluid's current order); 1 on the reference build */
+int   sph_app_upload_temperature(sph_app* app, const float* t_host);
+int   sph_app_download_temperature(sph_app* app, float* t_host);
+/* conduction substeps, largest dt_k sum c_ij and particle-substeps above 1 of the last step; min, max and sum m T of the current
+ * temperatures (any pointer may be NULL); synchronises; 1 on the reference build */
+int   sph_app_thermal_stats(sph_app* app, int* substeps, float* max_courant, int* violators, float* t_min, float* t_max, double* heat);
 /* Kinematic rigid bodies (SPHSystem's constructor with a vector of sphb200::KinematicBody; DESIGN.md section 2.3).  No
  * reference counterpart: NULL / 1 on the reference build.  Body b is the points body_xyz[body_begin[b] .. body_begin[b+1])
  * (body coordinates; body_begin[0] = 0), pose[7 b ..] = {cx, cy, cz, qx, qy, qz, qw} (quaternion scalar part last),

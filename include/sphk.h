@@ -337,6 +337,61 @@ int sphk_visc_field_setup(sphk_ctx* ctx, const sphk_scene* s, float* d_out, floa
 int sphk_visc_field_matvec(sphk_ctx* ctx, const sphk_scene* s, const float* d_in, const float* p_in, float* ap_out, const float* nu,
                            float dt, float rho0);
 
+/* ---- heat transfer (no reference counterpart; DESIGN.md section 2.10) ----------------------------------------------------------
+ * Every fluid particle carries a temperature T_i (a caller-owned device float[n] in the fluid's current order).  With d = x_i - x_j,
+ * r = |d|, f = the kernel gradient factor (grad W = d f, f <= 0), eta^2 = 0.0025 R^2:
+ *   dT_i/dt = sum_j c_ij (T_j - T_i),   c_ij = -2 alpha V_j f r^2 / (r^2 + eta^2) >= 0
+ *   fluid neighbour: V_j = m_j / rho0 (so m_i c_ij = m_j c_ji: sum m T is conserved); boundary neighbour of group g (0 = the static
+ *   walls, b + 1 = body b): V_b = m_b / rho_boundary, alpha -> h_g alpha, T_j -> T_g.  Groups at or past n_groups are adiabatic.
+ * One substep k of K (dt_k = dt / K, K from sphk_heat_substeps): T += dt_k dT/dt (Jacobi: the sweep reads the old T only); on the
+ * last substep the buoyancy v += -beta (T - t_ref) G dt (the step's dt, the new T) on the API velocities and the records.
+ * The sweep records max dt_k sum_j c_ij and the count of particles above 1 (the discrete maximum principle holds below 1):
+ * statistics, not a clamp.
+ * SPHK_ERR_INVALID: NULL or aliased buffers, alpha < 0, a non-finite beta or t_ref, a group with a non-finite T or h < 0, n_groups
+ * outside [0, SPHK_THERMAL_GROUPS], rho0 or rho_boundary <= 0, dt < 0, K < 1 or k outside [0, K).  SPHK_ERR_STATE: an active range
+ * (slab ranks), or n_groups above 1 + the bodies of the context. */
+#define SPHK_BODY_LIMIT 64                              /* bodies per context (sphk_bodies_init) */
+#define SPHK_THERMAL_GROUPS (1 + SPHK_BODY_LIMIT)
+typedef struct sphk_thermal_group {
+    float t;                  /* temperature of the group's boundary particles */
+    float h;                  /* relative conductance >= 0 (0: adiabatic) */
+} sphk_thermal_group;
+typedef struct sphk_thermal {
+    float alpha;              /* diffusivity >= 0 (m^2/s in the scene's units) */
+    float beta;               /* expansion coefficient of the buoyancy term */
+    float t_ref;              /* temperature without buoyancy */
+    int n_groups;             /* entries of groups[] in use */
+    sphk_thermal_group groups[SPHK_THERMAL_GROUPS];
+} sphk_thermal;
+/* Host only, no context: the substep count K = max(1, ceil(dt S)), S = SPHK_HEAT_COP alpha (1 + h_max) / R^2 (h_max over the groups in
+ * use), so that dt_k sum_j c_ij <= 1 in the scenes DESIGN.md section 2.10 derives SPHK_HEAT_COP from.  SPHK_ERR_INVALID for a bad
+ * setting, radius <= 0, dt < 0 or non-finite, or K above 65536. */
+#define SPHK_HEAT_COP 100.0
+int sphk_heat_substeps(const sphk_thermal* thermal, float radius, float dt, int* substeps);
+/* substep k of K of a step of length dt; work = n device floats (dT/dt); gravity = {gx, gy, gz} (host) */
+int sphk_heat_step(sphk_ctx* ctx, const sphk_scene* s, const sphk_thermal* thermal, float* temperature, float* work, float dt, int k,
+                   int substeps, float rho0, float rho_boundary, const float* gravity);
+/* per element (tests): dT/dt of every particle; the statistics with dt_sub as dt_k */
+int sphk_heat_conduction(sphk_ctx* ctx, const sphk_scene* s, const sphk_thermal* thermal, const float* temperature, float* dtdt_out,
+                         float dt_sub, float rho0, float rho_boundary);
+/* Statistics of the last step's substeps (0 before the first: the largest dt_k sum_j c_ij and the particle-substeps above 1), and,
+ * when temperature and mass are given, min T, max T and sum m T (double) over n particles by a fixed-shape reduction (the same
+ * bits for the same input).  Any output pointer may be NULL.  Synchronises. */
+int sphk_heat_stats(sphk_ctx* ctx, const float* temperature, const float* mass, int n, float* max_courant, int* violators,
+                    float* t_min, float* t_max, double* heat);
+/* Temperature-dependent viscosity nu_i = clamp(nu_ref exp(-e (T_i - t_ref)), nu_min, nu_max) (double, rounded once; nu_max finite),
+ * solved by the per-particle-nu PCG of section 2.9 (walls with beta nu_i); iterations and residual in
+ * sphk_implicit_viscosity_stats.  work = sphk_implicit_viscosity_work_floats(n) floats, nu_field = n floats (receives nu_i).
+ * SPHK_ERR_INVALID as sphk_non_newtonian_viscosity, and nu_ref < 0 or a non-finite e or t_ref; SPHK_ERR_STATE: slab ranks, beta > 0
+ * with dynamic bodies. */
+typedef struct sphk_viscosity_law {
+    float nu_ref, e, t_ref, nu_min, nu_max;
+} sphk_viscosity_law;
+int sphk_thermal_viscosity(sphk_ctx* ctx, const sphk_scene* s, float* work, float* nu_field, const float* temperature,
+                           const sphk_viscosity_law* law, float beta, float dt, float rho0, float rho_boundary, float tol,
+                           int max_iter);
+int sphk_thermal_viscosity_eval(sphk_ctx* ctx, const sphk_viscosity_law* law, const float* temperature, float* nu_out, int n);
+
 /* ---- kinematic rigid bodies (no reference counterpart; DESIGN.md section 2.3) ---------------------------------------------
  * A body is a rigid set of boundary particles given in body coordinates r_k, with a pose (centre c, unit quaternion q) and
  * a motion (linear velocity V, angular velocity Omega, both in the world frame).  Poses and motions live in device memory.
