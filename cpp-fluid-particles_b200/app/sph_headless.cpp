@@ -12,6 +12,11 @@
 //                [--bullets K] [--stir OMEGA] [--float REL] [--implicit-viscosity NU] [--tap SPEED] [--drain SIDE] [--capacity N]
 //                [--cfl C [--dt-min X]] [--rheology cross:NU0,NUINF,LAMBDA,M | hb:K,N,TAU[,MREG] [--rheology-max NU_MAX] [--no-slip]]
 //                [--heat ALPHA,BETA[,TREF] [--heater T] [--wall-temp T[,H]] [--tap-temp T] [--thermal-viscosity NUREF,E[,NUMAX]]]
+//                [--adhesion BETA[,BODYBETA]]
+// --adhesion turns on fluid-solid adhesion (BasicSPHSolver::setAdhesion, DESIGN.md section 2.11) after the constructor's step 0: the
+// tank walls with BETA, the --stir paddle, the --float cube or the --heater plate with BODYBETA (default BETA).  Every frame prints
+// the wetted particles and the largest adhesion acceleration; with --float the result line also carries the cube's position and its
+// last step's impulse.  Single GPU only.
 // --heat turns on heat transfer (BasicSPHSolver::setThermal, DESIGN.md section 2.10) after the constructor's step 0: diffusivity ALPHA,
 // buoyancy BETA, reference temperature TREF (default 0, also the fluid's initial temperature).  --heater T adds a held, motionless
 // plate body on the floor under the block at T with conductance 1 (not together with --stir or --float); --wall-temp T[,H] sets the
@@ -108,6 +113,7 @@ struct Options {
     float rheologyMax = -1.0f;                // --rheology-max NU_MAX (< 0: the model's default)
     bool noSlip = false;                      // --no-slip: boundary factor 1 for --rheology
     std::string heat;                         // --heat ALPHA,BETA[,TREF] (empty: off)
+    std::string adhesion;                     // --adhesion BETA[,BODYBETA] (empty: off)
     std::string heater, wallTemp, tapTemp, thermalVisc;   // --heater T, --wall-temp T[,H], --tap-temp T, --thermal-viscosity NUREF,E[,NUMAX]
     float cfl = 0.0f;                         // --cfl C: CFL-adaptive substeps, --dt of simulated time per frame (0: off)
     float dtMin = 0.0f;                       // --dt-min X: their smallest dt (0: dt / 64)
@@ -157,6 +163,16 @@ bool floats_of(const std::string& spec, std::vector<float>& v) {
         v.push_back(x);
         at = comma + 1;
     }
+    return true;
+}
+
+// --adhesion BETA[,BODYBETA] -> the setting (the walls, and the scene's body if it has one); false for malformed or negative values
+bool adhesion_of(const Options& o, bool hasBody, sphb200::Adhesion& a) {
+    std::vector<float> v;
+    if (!floats_of(o.adhesion, v) || v.size() > 2 || v[0] < 0.0f || v.back() < 0.0f) return false;
+    a = sphb200::Adhesion();
+    a.wall = v[0];
+    if (hasBody) a.bodies.push_back(v.back());
     return true;
 }
 
@@ -210,6 +226,7 @@ bool parse(int argc, char** argv, Options& o) {
         else if (a == "--rheology-max" && need(i, 1)) o.rheologyMax = static_cast<float>(std::atof(argv[++i]));
         else if (a == "--no-slip") o.noSlip = true;
         else if (a == "--heat" && need(i, 1)) o.heat = argv[++i];
+        else if (a == "--adhesion" && need(i, 1)) o.adhesion = argv[++i];
         else if (a == "--heater" && need(i, 1)) o.heater = argv[++i];
         else if (a == "--wall-temp" && need(i, 1)) o.wallTemp = argv[++i];
         else if (a == "--tap-temp" && need(i, 1)) o.tapTemp = argv[++i];
@@ -294,6 +311,14 @@ bool parse(int argc, char** argv, Options& o) {
     } else if (!o.heater.empty() || !o.wallTemp.empty() || !o.tapTemp.empty() || !o.thermalVisc.empty()) {
         std::fprintf(stderr, "sph_headless: --heater, --wall-temp, --tap-temp and --thermal-viscosity go with --heat\n");
         return false;
+    }
+    if (!o.adhesion.empty()) {
+        sphb200::Adhesion a;
+        if (!adhesion_of(o, false, a) || o.ranks > 1) {
+            std::fprintf(stderr, "sph_headless: --adhesion needs BETA[,BODYBETA] with finite values >= 0 and runs on one GPU only (not "
+                                 "with --ranks)\n");
+            return false;
+        }
     }
     if (!(o.cfl >= 0.0f) || !std::isfinite(o.cfl) || !(o.dtMin >= 0.0f) || !std::isfinite(o.dtMin)) {
         std::fprintf(stderr, "sph_headless: --cfl C and --dt-min X need finite values > 0\n");
@@ -484,7 +509,8 @@ int main(int argc, char** argv) {
                              "[--origin X Y Z] [--dt DT] [--iters K] [--vorticity EPS] [--implicit-viscosity NU] [--stir OMEGA | --float REL] "
                              "[--tap SPEED] [--drain SIDE] [--capacity N] [--cfl C [--dt-min X]] [--rheology cross:NU0,NUINF,LAMBDA,M | hb:K,N,TAU[,MREG] "
                              "[--rheology-max NU_MAX] [--no-slip]] [--heat ALPHA,BETA[,TREF] [--heater T] [--wall-temp T[,H]] "
-                             "[--tap-temp T] [--thermal-viscosity NUREF,E[,NUMAX]]] [--dump PREFIX] [--quiet] [--emit-scene PREFIX] "
+                             "[--tap-temp T] [--thermal-viscosity NUREF,E[,NUMAX]]] [--adhesion BETA[,BODYBETA]] [--dump PREFIX] [--quiet] "
+                             "[--emit-scene PREFIX] "
                              "[--ranks N [--rank R --rendezvous DIR]]\n");
         return 2;
     }
@@ -644,6 +670,14 @@ int main(int argc, char** argv) {
             return 4;
         }
     }
+    if (!o.adhesion.empty()) {
+        sphb200::Adhesion a;
+        adhesion_of(o, !bodies.empty(), a);
+        if (!basicSolver->setAdhesion(a)) {
+            std::fprintf(stderr, "sph_headless: --adhesion %s was refused\n", o.adhesion.c_str());
+            return 4;
+        }
+    }
     if (o.cfl > 0.0f && !pSystem->setAdaptiveTimeStep(o.cfl, o.dtMin)) {
         std::fprintf(stderr, "sph_headless: --cfl %g --dt-min %g was refused\n", o.cfl, o.dtMin);
         return 4;
@@ -690,6 +724,10 @@ int main(int argc, char** argv) {
             const int nf = static_cast<int>(pSystem->getFluids()->size());
             std::printf("Frame %d heat - T min %g max %g mean %g, heat %.9g, %d substeps, %d above the stability bound\n", frameId,
                         ts.Tmin, ts.Tmax, nf > 0 ? ts.heat / (double(kSphM0) * nf) : 0.0, ts.heat, ts.substeps, ts.violators);
+        }
+        if (!o.quiet && !o.adhesion.empty()) {
+            const sphb200::AdhesionStats as = basicSolver->lastAdhesionStats();
+            std::printf("Frame %d adhesion - %d wetted particles, max acceleration %g m/s^2\n", frameId, as.wetted, as.maxAccel);
         }
         if (!o.quiet && !o.rheology.empty()) {
             const sphb200::RheologyStats rs = basicSolver->lastRheologyStats();
@@ -744,6 +782,22 @@ int main(int argc, char** argv) {
         std::snprintf(buf, sizeof buf, ", \"simulated_time\": %.17g, \"dt_min_clamps\": %lld, \"nonfinite_steps\": %lld, \"last_dt\": %.9g",
                       pSystem->simulatedTime(), st.minClamps, st.nonFiniteSteps, pSystem->lastTimeStep());
         openJson += ", \"frame_substeps\": [" + substepsJson + "]" + buf;
+    }
+    if (!o.adhesion.empty()) {
+        const sphb200::AdhesionStats as = basicSolver->lastAdhesionStats();
+        char buf[96];
+        std::snprintf(buf, sizeof buf, ", \"adhesion_wetted\": %d, \"adhesion_max_accel\": %.9g", as.wetted, as.maxAccel);
+        openJson += buf;
+        if (o.floating) {
+            float3 c, J, H;
+            float4 q;
+            pSystem->getBodyPose(0, c, q);
+            pSystem->getBodyImpulse(0, J, H);
+            char bb[192];
+            std::snprintf(bb, sizeof bb, ", \"body_position\": [%.9g, %.9g, %.9g], \"body_impulse\": [%.9g, %.9g, %.9g]", c.x, c.y, c.z,
+                          J.x, J.y, J.z);
+            openJson += bb;
+        }
     }
     if (open) {
         const sphb200::OpenBoundaryStats st = pSystem->openBoundaryStats();

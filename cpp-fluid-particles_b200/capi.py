@@ -40,7 +40,7 @@ SPHK_FUNCTIONS = [
     "sphk_rheology_work_floats", "sphk_non_newtonian_viscosity", "sphk_non_newtonian_stats", "sphk_shear_rate", "sphk_rheology_eval",
     "sphk_visc_field_setup", "sphk_visc_field_matvec",
     "sphk_heat_substeps", "sphk_heat_step", "sphk_heat_conduction", "sphk_heat_stats", "sphk_thermal_viscosity",
-    "sphk_thermal_viscosity_eval",
+    "sphk_thermal_viscosity_eval", "sphk_adhesion", "sphk_adhesion_accel", "sphk_adhesion_stats",
 ]
 SPH_APP_FUNCTIONS = [
     "sph_app_create", "sph_app_destroy", "sph_app_step", "sph_app_fluid_size", "sph_app_boundary_size",
@@ -51,7 +51,7 @@ SPH_APP_FUNCTIONS = [
     "sph_app_viscosity_stats", "sph_app_create_open", "sph_app_open_boundary_stats", "sph_app_set_adaptive_dt", "sph_app_advance",
     "sph_app_adaptive_stats", "sph_app_set_rheology", "sph_app_rheology_stats", "sph_app_download_viscosity",
     "sph_app_set_thermal", "sph_app_set_thermal_viscosity", "sph_app_upload_temperature", "sph_app_download_temperature",
-    "sph_app_thermal_stats",
+    "sph_app_thermal_stats", "sph_app_set_adhesion", "sph_app_adhesion_stats",
 ]
 
 BODY_LIMIT = 64                      # SPHK_BODY_LIMIT
@@ -89,6 +89,30 @@ def thermal(spec: dict) -> Thermal:
     for g, (T, h) in enumerate([tuple(spec.get("wall", (0.0, 0.0)))] + [tuple(b) for b in bodies]):
         t.groups[g].t, t.groups[g].h = float(T), float(h)
     return t
+
+
+ADHESION_GROUPS = 1 + BODY_LIMIT     # SPHK_ADHESION_GROUPS
+
+
+class Adhesion(C.Structure):
+    """sphk_adhesion_setting of sphk.h"""
+    _fields_ = [("n_groups", C.c_int), ("beta", C.c_float * ADHESION_GROUPS)]
+
+
+def adhesion(spec: dict) -> Adhesion:
+    """sphk_adhesion_setting from dict(wall=beta, bodies=[beta, ...]).  Unknown keys and more than BODY_LIMIT bodies raise
+    ValueError; the ranges are checked by the library."""
+    extra = set(spec) - {"wall", "bodies"}
+    if extra:
+        raise ValueError(f"unknown adhesion keys {sorted(extra)}")
+    bodies = [float(b) for b in spec.get("bodies", ())]
+    if len(bodies) > BODY_LIMIT:
+        raise ValueError(f"at most {BODY_LIMIT} bodies")
+    a = Adhesion()
+    a.n_groups = 1 + len(bodies)
+    for g, beta in enumerate([float(spec.get("wall", 0.0))] + bodies):
+        a.beta[g] = beta
+    return a
 
 
 # the solve's settings of a thermal viscosity dict, beside the law's own keys
@@ -476,6 +500,25 @@ class SphApp:
         if self.L.sph_app_download_temperature(self.h, out.ctypes.data_as(C.c_void_p)):
             raise RuntimeError("sph_app_download_temperature failed (reference engine)")
         return out
+
+    def set_adhesion(self, spec):
+        """Fluid-solid adhesion in every following step (spec: a dict for capi.adhesion; None: off).  Not on the reference engine."""
+        if spec is None:
+            rc = self.L.sph_app_set_adhesion(self.h, C.c_int(0), C.c_float(0), C.c_int(0), None)
+        else:
+            a = adhesion(spec)
+            bodies = np.ascontiguousarray(np.asarray(spec.get("bodies", []), np.float32).reshape(-1))
+            rc = self.L.sph_app_set_adhesion(self.h, C.c_int(1), C.c_float(a.beta[0]), C.c_int(bodies.size),
+                                             bodies.ctypes.data_as(C.c_void_p))
+        if rc:
+            raise RuntimeError("sph_app_set_adhesion failed (reference engine or a refused setting)")
+
+    def adhesion_stats(self) -> dict:
+        """wetted particles and the largest |a_i| of the last step's adhesion sweep"""
+        w, am = C.c_int(0), C.c_float(0)
+        if self.L.sph_app_adhesion_stats(self.h, C.byref(w), C.byref(am)):
+            raise RuntimeError("sph_app_adhesion_stats failed (reference engine)")
+        return {"wetted": w.value, "max_accel": am.value}
 
     def thermal_stats(self) -> dict:
         """substeps, max_courant, violators of the last step; t_min, t_max, heat (sum m T) now"""

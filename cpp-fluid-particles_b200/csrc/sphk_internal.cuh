@@ -135,6 +135,8 @@ struct sphk_ctx {
     float2* heatGroups = nullptr;    // [SPHK_THERMAL_GROUPS] device: {T_g, h_g} of the step's sphk_thermal (heat transfer)
     unsigned int* heatStats = nullptr;   // [2] device: {max dt_k sum_j c_ij (float bits), particle-substeps above 1} of the last step
     double* heatRed = nullptr;       // [3 * 1024 + 3] device: partials and result {min T, max T, sum m T} of sphk_heat_stats
+    float* adhGroups = nullptr;      // [SPHK_ADHESION_GROUPS] device: beta_g of the last sphk_adhesion (fluid-solid adhesion)
+    unsigned int* adhStats = nullptr;    // [2] device: {wetted particles, max |a_i| (float bits)} of the last adhesion sweep
     // open boundaries (sphk_sinks_apply / sphk_fluid_set_count; allocated on first use)
     int* openDev = nullptr;          // device [2]: {particles the last sphk_sinks_apply removed, sticky check bits}
     int* openPinned = nullptr;       // pinned [1]: the removed count, copied behind the sink kernel

@@ -216,6 +216,8 @@ extern "C" int sphk_create(sphk_ctx** out, int max_fluid, int max_boundary, cons
     if (e == cudaSuccess) e = dalloc(&c->heatGroups, SPHK_THERMAL_GROUPS);
     if (e == cudaSuccess) e = dalloc(&c->heatStats, 2);
     if (e == cudaSuccess) e = dalloc(&c->heatRed, 3 * 1024 + 3);
+    if (e == cudaSuccess) e = dalloc(&c->adhGroups, SPHK_ADHESION_GROUPS);
+    if (e == cudaSuccess) e = dalloc(&c->adhStats, 2);
     if (e == cudaSuccess) e = dalloc(&c->cnt, static_cast<size_t>(max_fluid));
     if (e == cudaSuccess) e = dalloc(&c->tileWin, (static_cast<size_t>(max_fluid) / SPHK_BLOCK + 1) * SPHK_TILE_WINS);
     if (e == cudaSuccess) {
@@ -247,7 +249,7 @@ extern "C" void sphk_destroy(sphk_ctx* c) {
     if (!c) return;
     cudaFree(c->keys); cudaFree(c->keysSorted); cudaFree(c->idx); cudaFree(c->idxSorted);
     cudaFree(c->snapA); cudaFree(c->snapB); cudaFree(c->rec.a); cudaFree(c->rec.b); cudaFree(c->massRange); cudaFree(c->dispMax); cudaFree(c->cellFlag);
-    cudaFree(c->tmpF); cudaFree(c->partial); cudaFree(c->loops); cudaFree(c->viscStats); cudaFree(c->rheoStats); cudaFree(c->heatGroups); cudaFree(c->heatStats); cudaFree(c->heatRed); cudaFree(c->cnt); cudaFree(c->nbr); cudaFree(c->cubTemp); cudaFree(c->tileWin);
+    cudaFree(c->tmpF); cudaFree(c->partial); cudaFree(c->loops); cudaFree(c->viscStats); cudaFree(c->rheoStats); cudaFree(c->heatGroups); cudaFree(c->heatStats); cudaFree(c->heatRed); cudaFree(c->adhGroups); cudaFree(c->adhStats); cudaFree(c->cnt); cudaFree(c->nbr); cudaFree(c->cubTemp); cudaFree(c->tileWin);
     if (c->pinned) cudaFreeHost(c->pinned);
     cudaFree(c->openDev);
     if (c->openPinned) cudaFreeHost(c->openPinned);

@@ -1627,12 +1627,46 @@ extern "C" int sphk_pbd_delta_pos_apply(sphk_ctx* c, const sphk_scene* s, const 
 
 // ---- two-way coupled bodies: the fluid's reaction on them (DESIGN.md section 2.4) ---------------------------------------------
 // One thread per boundary slot; body particles only.  Walks the fluid cells within `reach` cells of the particle with the
-// fluid cell ranges of the search and forms each pair term as the fluid sweep forms it, g = (m_k s_i) (d gradWfactor),
-// d = x_i - x_k (the fluid particle received c m_i g).  The body particle gathers -c m_i g and its moment about the body's
-// centre into its own declaration slot of acc, in double (no atomics: every slot has one writer, sums are in walk order).
+// fluid cell ranges of the search and forms each pair term as the fluid sweep forms it.  The body particle gathers the pair's
+// reaction and its moment about the body's centre into its own declaration slot of acc, in double (no atomics: every slot has
+// one writer, sums are in walk order).  The pair term is a template:
+//   ReactGradW     g = (m_k s_i) (d gradWfactor), d = x_i - x_k; the fluid particle received c m_i g, the body gathers -c m_i g
+//   ReactAdhesion  the fluid particle received dt beta_g Psi_k A(r) (-d / r) per unit mass (section 2.11), the body gathers
+//                  +dt beta_g Psi_k m_i A(r) d / r; bodies whose beta is 0 are skipped
+struct ReactGradW {
+    float coef;
+    static constexpr bool kByGroup = false;
+    __device__ double body_coef(int) const { return coef; }
+    __device__ bool term(float3 d, float r2, float mk, float4 lo, const KConst& k, float3& t) const {
+        t = (mk * lo.w) * (d * grad_w_factor(sqrtf(r2), k));
+        return true;
+    }
+    __device__ double gather(double cc, float mi) const { return -cc * static_cast<double>(mi); }
+};
+// A(r) of section 2.11 with cA = 0.007 / R^3.25: -4 r^2 / R + 6 r - 2 R = 2 (2 r - R)(R - r) / R, >= 0 in the band
+__device__ __forceinline__ float adhesion_w(float r, float R, float cA) {
+    const float t = 2.0f * (2.0f * r - R) * (R - r) / R;
+    return (2.0f * r > R && r <= R) ? cA * sqrtf(sqrtf(t)) : 0.0f;
+}
+struct ReactAdhesion {
+    const float* beta;                // the group table of sphk_adhesion
+    double dtPsi;                     // dt rho0 / rho_B
+    float cA;
+    static constexpr bool kByGroup = true;
+    __device__ double body_coef(int g) const { return dtPsi * static_cast<double>(beta[g]); }
+    __device__ bool term(float3 d, float r2, float mk, float4, const KConst& k, float3& t) const {
+        const float r = sqrtf(r2);
+        const float a = adhesion_w(r, k.R, cA);
+        if (a == 0.0f) return false;
+        t = (mk * __fdividef(a, r)) * d;
+        return true;
+    }
+    __device__ double gather(double cc, float mi) const { return cc * static_cast<double>(mi); }
+};
+template <class Pair>
 __global__ void __launch_bounds__(SPHK_BLOCK)
 k_bodies_react(const DevScene s, const float* __restrict__ massF, const float4* __restrict__ local, const int* __restrict__ decl,
-               const float* __restrict__ pose, int nB, int nStatic, int reach, float coef, double* __restrict__ acc) {
+               const float* __restrict__ pose, int nB, int nStatic, int reach, const Pair pair, double* __restrict__ acc) {
     if (s.pred && *s.pred == 0) return;     // a device-controlled loop has ended: its sweeps did not run
     const int kb = blockIdx.x * SPHK_BLOCK + threadIdx.x;
     if (kb >= nB) return;
@@ -1645,7 +1679,8 @@ k_bodies_react(const DevScene s, const float* __restrict__ massF, const float4* 
               cz = cell_coord(pk.z, s.cellLength) - s.org.z;
     if (cx < 0 || cx >= s.cs.x || cy < 0 || cy >= s.cs.y || cz < 0 || cz >= s.cs.z) return;   // off the grid: no interaction
     const int zlo = max(cz - reach, 0), zhi = min(cz + reach, s.cs.z - 1);
-    const double cc = coef;
+    const double cc = pair.body_coef(g);
+    if (Pair::kByGroup && !(cc > 0.0)) return;
     double F[3] = {0.0, 0.0, 0.0};
 #pragma unroll 1
     for (int x = max(cx - reach, 0); x <= min(cx + reach, s.cs.x - 1); ++x)
@@ -1658,8 +1693,9 @@ k_bodies_react(const DevScene s, const float* __restrict__ massF, const float4* 
                 const float3 d = xyz(lo) - xk;
                 const float r2 = dot3(d, d);
                 if (r2 > s.k.r2cut) continue;
-                const float3 t = (mk * lo.w) * (d * grad_w_factor(sqrtf(r2), s.k));
-                const double f = -cc * static_cast<double>(massF[j]);
+                float3 t;
+                if (!pair.term(d, r2, mk, lo, s.k, t)) continue;
+                const double f = pair.gather(cc, massF[j]);
                 F[0] += f * t.x; F[1] += f * t.y; F[2] += f * t.z;
             }
         }
@@ -1679,7 +1715,7 @@ extern "C" int sphk_bodies_react(sphk_ctx* c, const sphk_scene* s, float coef) {
     // positions moved since the search (PBD corrections): a fluid particle within R of x_k may be listed two cells away
     const int reach = c->posDirty ? 2 : 1;
     k_bodies_react<<<sphk_blocks(c->nB), SPHK_BLOCK, 0, c->stream>>>(dev_scene(c, s), s->fluid.mass, B->local, B->decl, B->pose,
-                                                                    c->nB, B->nStatic, reach, coef, B->acc);
+                                                                    c->nB, B->nStatic, reach, ReactGradW{coef}, B->acc);
     c->launches++;
     SPHK_CUDA_TRY(cudaGetLastError());
     return SPHK_OK;
@@ -2511,6 +2547,142 @@ extern "C" int sphk_thermal_viscosity_eval(sphk_ctx* c, const sphk_viscosity_law
     k_thermal_nu<<<sphk_blocks(n), SPHK_BLOCK, 0, c->stream>>>(*law, T, nu_out, n);
     c->launches++;
     SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+// ---- fluid-solid adhesion (DESIGN.md section 2.11) ------------------------------------------------------------------------------
+// the step's group table beta_g (groups past n_groups: 0) from the setting passed by value, and the statistics reset
+__global__ void k_adhesion_begin(sphk_adhesion_setting ad, float* __restrict__ groups, unsigned int* __restrict__ stats, const int* pred) {
+    if (pred && *pred == 0) return;
+    const int g = threadIdx.x;
+    if (g < SPHK_ADHESION_GROUPS) groups[g] = g < ad.n_groups ? ad.beta[g] : 0.f;
+    if (g == 0) { stats[0] = 0u; stats[1] = 0u; }
+}
+// One thread per fluid particle: the 9 rows of boundary cell ranges around the particle's current cell (boundary records do not
+// move between the boundary search and the velocity stage: sphk_bodies_step searches after it places the bodies).  Without
+// bodies every boundary particle is in group 0, whose beta comes by value; with bodies the group is local[b].w and beta_g comes
+// from the table (read only for pairs in the band).  accel: a_i per element (tests); else v += dt a_i where some pair acted.
+__global__ void __launch_bounds__(SPHK_BLOCK)
+k_adhesion(const DevScene s, float* __restrict__ vel, float* __restrict__ accel, const float4* __restrict__ local,
+           const float* __restrict__ groups, float beta0, float psi, float cA, float dt, unsigned int* __restrict__ stats) {
+    if (s.pred && *s.pred == 0) return;
+    const int i = blockIdx.x * SPHK_BLOCK + threadIdx.x;
+    if (i >= s.nF) return;
+    const float3 xi = xyz(rec_lo(s.rec + i));
+    const int cx = cell_coord(xi.x, s.cellLength) - s.org.x, cy = cell_coord(xi.y, s.cellLength) - s.org.y,
+              cz = cell_coord(xi.z, s.cellLength) - s.org.z;
+    float3 a = make_float3(0.f, 0.f, 0.f);
+    bool wet = false;
+    if (cx >= 0 && cx < s.cs.x && cy >= 0 && cy < s.cs.y && cz >= 0 && cz < s.cs.z) {      // off the grid: no interaction
+        const int zlo = max(cz - 1, 0), zhi = min(cz + 1, s.cs.z - 1);
+#pragma unroll 1
+        for (int x = max(cx - 1, 0); x <= min(cx + 1, s.cs.x - 1); ++x)
+#pragma unroll 1
+            for (int y = max(cy - 1, 0); y <= min(cy + 1, s.cs.y - 1); ++y) {
+                const int c0 = (x * s.cs.y + y) * s.cs.z;
+                const int end = s.csB[c0 + zhi + 1];
+                for (int b = s.csB[c0 + zlo]; b < end; ++b) {
+                    const float4 pb = rec_lo(s.rec + s.bOff + b);          // {x_b, m_b}
+                    const float3 d = xi - xyz(pb);
+                    const float r = sqrtf(dot3(d, d));
+                    const float w = adhesion_w(r, s.k.R, cA);
+                    if (w == 0.0f) continue;
+                    const float beta = local ? groups[static_cast<int>(body_group(local[b]))] : beta0;
+                    if (!(beta > 0.0f)) continue;
+                    a -= (beta * psi * pb.w * __fdividef(w, r)) * d;
+                    wet = true;
+                }
+            }
+    }
+    if (accel) store3(accel, i, a);
+    else if (wet) {
+        const float3 v = load3(vel, i) + dt * a;
+        store3(vel, i, v);
+        rec_set_vel(s.rec + i, v);
+    }
+    namespace cg = cooperative_groups;
+    const float am = sqrtf(dot3(a, a));
+    const cg::coalesced_group grp = cg::coalesced_threads();
+    const unsigned int amax = cg::reduce(grp, __float_as_uint(am), cg::greater<unsigned int>());
+    const unsigned int cnt = __popc(grp.ballot(wet));
+    if (grp.thread_rank() == 0) {
+        if (amax) atomicMax(stats + 1, amax);
+        if (cnt) atomicAdd(stats, cnt);
+    }
+}
+
+static int check_adhesion_call(sphk_ctx* c, const sphk_adhesion_setting* ad, float rho0, float rhoB) {
+    if (!ad || ad->n_groups < 1 || ad->n_groups > SPHK_ADHESION_GROUPS || !(rho0 > 0.f) || !(rhoB > 0.f) || !finite_f(rho0) ||
+        !finite_f(rhoB))
+        return SPHK_ERR_INVALID;
+    for (int g = 0; g < ad->n_groups; ++g)
+        if (!finite_nonneg(ad->beta[g])) return SPHK_ERR_INVALID;
+    if (c->actCount >= 0 || c->rangeDev) return SPHK_ERR_STATE;      // slab ranks: not supported
+    if (ad->n_groups > 1 + (c->bodies ? c->bodies->nBodies : 0)) return SPHK_ERR_STATE;
+    return SPHK_OK;
+}
+
+static double adhesion_scale(float R) { return 0.007 / std::pow(static_cast<double>(R), 3.25); }
+
+// the table + statistics reset, then the sweep (accel: per element, else the velocity update)
+static int adhesion_sweep(sphk_ctx* c, const sphk_scene* s, const sphk_adhesion_setting& ad, float* accel, float dt, float rho0, float rhoB) {
+    k_adhesion_begin<<<1, 96, 0, c->stream>>>(ad, c->adhGroups, c->adhStats, c->pred);
+    c->launches++;
+    const DevScene d = dev_scene(c, s);
+    if (c->nF > 0) {
+        k_adhesion<<<sphk_blocks(c->nF), SPHK_BLOCK, 0, c->stream>>>(d, s->fluid.vel, accel, c->bodies ? c->bodies->local : nullptr,
+                                                                     c->adhGroups, ad.beta[0], rho0 / rhoB,
+                                                                     static_cast<float>(adhesion_scale(s->radius)), dt, c->adhStats);
+        c->launches++;
+    }
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+extern "C" int sphk_adhesion(sphk_ctx* c, const sphk_scene* s, const sphk_adhesion_setting* ad, float dt, float rho0, float rho_boundary) {
+    SPHK_CHECK_SCENE(c, s);
+    if (!finite_nonneg(dt)) return SPHK_ERR_INVALID;
+    const int rc0 = check_adhesion_call(c, ad, rho0, rho_boundary);
+    if (rc0 != SPHK_OK) return rc0;
+    const BodyState* B = c->bodies;
+    bool bodyAdheres = false;
+    for (int g = 1; g < ad->n_groups; ++g) bodyAdheres = bodyAdheres || ad->beta[g] > 0.f;
+    const bool react = B && B->acc && bodyAdheres && c->nB > 0;
+    if (react && !s->fluid.mass) return SPHK_ERR_INVALID;         // (before any launch: a refused call changes nothing)
+    const int rc = adhesion_sweep(c, s, *ad, nullptr, dt, rho0, rho_boundary);
+    if (rc != SPHK_OK) return rc;
+    // the reaction on the bodies, into the impulse of the step (sphk_bodies_integrate)
+    if (react) {
+        // positions moved since the search (PBD corrections): a fluid particle within R of x_k may be listed two cells away
+        const int reach = c->posDirty ? 2 : 1;
+        const ReactAdhesion pair{c->adhGroups, static_cast<double>(dt) * rho0 / rho_boundary, static_cast<float>(adhesion_scale(s->radius))};
+        k_bodies_react<<<sphk_blocks(c->nB), SPHK_BLOCK, 0, c->stream>>>(dev_scene(c, s), s->fluid.mass, B->local, B->decl, B->pose,
+                                                                        c->nB, B->nStatic, reach, pair, B->acc);
+        c->launches++;
+        SPHK_CUDA_TRY(cudaGetLastError());
+    }
+    return SPHK_OK;
+}
+
+extern "C" int sphk_adhesion_accel(sphk_ctx* c, const sphk_scene* s, const sphk_adhesion_setting* ad, float* accel, float rho0,
+                                   float rho_boundary) {
+    SPHK_CHECK_SCENE(c, s);
+    if (!accel || aliases(accel, s)) return SPHK_ERR_INVALID;
+    const int rc = check_adhesion_call(c, ad, rho0, rho_boundary);
+    if (rc != SPHK_OK) return rc;
+    if (c->sTag == accel) c->sTag = nullptr;
+    return adhesion_sweep(c, s, *ad, accel, 0.f, rho0, rho_boundary);
+}
+
+extern "C" int sphk_adhesion_stats(sphk_ctx* c, int* wetted, float* max_accel) {
+    if (!c) return SPHK_ERR_INVALID;
+    unsigned int st[2];
+    SPHK_CUDA_TRY(cudaMemcpyAsync(st, c->adhStats, sizeof(st), cudaMemcpyDeviceToHost, c->stream));
+    SPHK_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    float am;
+    memcpy(&am, &st[1], sizeof(am));
+    if (wetted) *wetted = static_cast<int>(st[0]);
+    if (max_accel) *max_accel = am;
     return SPHK_OK;
 }
 

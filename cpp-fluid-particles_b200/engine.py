@@ -87,6 +87,7 @@ class SphkOps:
     _thermal = None
     _thermal_viscosity = None
     _rheology = None
+    _adhesion = None
     heat_substeps = 0                # conduction substeps of the last step
     implicit_nu_boundary = 0.0
     implicit_tol = 1e-4
@@ -524,6 +525,41 @@ class SphkOps:
                                             C.c_float(self.p.rho_boundary), C.c_float(o["tol"]), C.c_int(int(o["max_iter"]))),
               "sphk_thermal_viscosity")
 
+    # ---- fluid-solid adhesion (no reference counterpart; DESIGN.md section 2.11) -------------------------------------------
+    @property
+    def adhesion(self):
+        """fluid-solid adhesion (BasicSPHSolver::setAdhesion): dict(wall=beta, bodies=[beta, ...]) for capi.adhesion; None: off.
+        More body entries than the system has bodies, and values the library refuses, raise ValueError."""
+        return self._adhesion
+
+    @adhesion.setter
+    def adhesion(self, spec):
+        if spec is not None:
+            a = capi.adhesion(spec)
+            if len(spec.get("bodies", ())) > self.n_bodies:
+                raise ValueError(f"{len(spec['bodies'])} body entries, but the system has {self.n_bodies} bodies")
+            if not all(np.isfinite(a.beta[g]) and a.beta[g] >= 0.0 for g in range(a.n_groups)):
+                raise ValueError(f"adhesion setting refused: {spec}")
+            self._adhesion_abi = a
+        self._adhesion = spec
+
+    def adhesion_step(self):
+        """v += dt a_i with the `adhesion` setting (and the reaction on dynamic bodies)"""
+        check(self.L.sphk_adhesion(self.ctx, self._s(), C.byref(self._adhesion_abi), C.c_float(self.dt), C.c_float(self.p.rho0),
+                                   C.c_float(self.p.rho_boundary)), "sphk_adhesion")
+
+    def adhesion_accel(self, out, spec=None):
+        """a_i (n, 3) of the adhesion sweep alone, with `spec` or the current setting"""
+        a = capi.adhesion(spec) if spec is not None else self._adhesion_abi
+        check(self.L.sphk_adhesion_accel(self.ctx, self._s(), C.byref(a), _ptr(out), C.c_float(self.p.rho0),
+                                         C.c_float(self.p.rho_boundary)), "sphk_adhesion_accel")
+
+    def adhesion_stats(self) -> dict:
+        """as capi.SphApp.adhesion_stats; synchronises"""
+        w, am = C.c_int(0), C.c_float(0)
+        check(self.L.sphk_adhesion_stats(self.ctx, C.byref(w), C.byref(am)), "sphk_adhesion_stats")
+        return {"wetted": w.value, "max_accel": am.value}
+
     def thermal_viscosity_eval(self, spec, t_ref, temperature, nu_out):
         law = capi.viscosity_law(spec, t_ref)
         check(self.L.sphk_thermal_viscosity_eval(self.ctx, C.byref(law), _ptr(temperature), _ptr(nu_out), C.c_int(temperature.numel())),
@@ -610,7 +646,7 @@ class SphkOps:
 
     def _velocity_stage(self, xsph: bool = False):
         """The velocity terms of every solver's step, in the class layer's order (BasicSPHSolver::velocityStage): vorticity omega,
-        viscosity (xsph: PBD's XSPH), surface tension, implicit viscosity, vorticity confinement.  With fused sweeps and not xsph
+        viscosity (xsph: PBD's XSPH), surface tension, adhesion, implicit viscosity, vorticity confinement, heat.  With fused sweeps and not xsph
         the colour gradient must be in color_grad_buf already (the density sweep computes it)."""
         surface, vort = self._surface_enabled(), self.vorticity_eps > 0
         if vort:
@@ -639,6 +675,8 @@ class SphkOps:
             if surface:              # handleSurface, BasicSPHSolver.cu:262-275
                 self._run(self.color_grad, "array", self.buffer3)
                 self._run(self.surface, "vel")
+        if self.adhesion is not None:
+            self._run(self.adhesion_step, "vel")
         if self.rheology is not None:       # replaces the constant-nu solve
             self._run(self.non_newtonian_viscosity, "vel")
         elif self.thermal is not None and self.thermal_viscosity is not None:

@@ -635,6 +635,39 @@ extern "C" int sph_app_thermal_stats(sph_app* app, int* substeps, float* max_cou
 #endif
 }
 
+extern "C" int sph_app_set_adhesion(sph_app* app, int on, float wall, int n_bodies, const float* body_beta) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)on; (void)wall; (void)n_bodies; (void)body_beta;
+    return 1;
+#else
+    auto* b = dynamic_cast<BasicSPHSolver*>(app->solver);
+    if (!b) return 1;
+    if (!on) {
+        b->clearAdhesion();
+        return 0;
+    }
+    if (n_bodies < 0 || (n_bodies > 0 && !body_beta)) return 1;
+    sphb200::Adhesion a;
+    a.wall = wall;
+    a.bodies.assign(body_beta, body_beta + n_bodies);
+    return b->setAdhesion(a) ? 0 : 1;        // (refused: the setting is kept)
+#endif
+}
+
+extern "C" int sph_app_adhesion_stats(sph_app* app, int* wetted, float* max_accel) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)wetted; (void)max_accel;
+    return 1;
+#else
+    auto* b = dynamic_cast<BasicSPHSolver*>(app->solver);
+    if (!b) return 1;
+    const sphb200::AdhesionStats s = b->lastAdhesionStats();
+    if (wetted) *wetted = s.wetted;
+    if (max_accel) *max_accel = s.maxAccel;
+    return 0;
+#endif
+}
+
 extern "C" int sph_app_set_adaptive_dt(sph_app* app, float C, float dt_min, float dt_max) {
 #ifdef SPH_APP_REFERENCE_ENGINE
     (void)app; (void)C; (void)dt_min; (void)dt_max;

@@ -163,6 +163,10 @@ void BasicSPHSolver::velocityStage(std::shared_ptr<SPHParticles>& fluids, const 
             handleSurface(fluids, boundaries, cellStartFluid, cellStartBoundary, rho0, rhoB, cellSize, cellLength, radius,
                           dt, surfaceTensionIntensity, airPressure);
     }
+    if (adhesionOn_) {
+        check(sphk_adhesion(current_.ctx, &current_.abi, &adhesionAbi_, dt, rho0, rhoB), "sphk_adhesion");
+        producedVel(fluids);
+    }
     if (rheoOn_) rheology(fluids, rho0, rhoB, dt);        // replaces the constant-nu solve
     else if (thermalOn_ && thermalViscOn_) thermalViscosity(fluids, rho0, rhoB, dt);
     else if (implicitViscosityOn()) implicitViscosity(fluids, rho0, rhoB, dt);
@@ -392,6 +396,39 @@ sphb200::ThermalStats BasicSPHSolver::lastThermalStats() {
         check(sphk_heat_stats(current_.ctx, temperature_->addr(), current_.abi.fluid.mass, current_.abi.fluid.n, &s.maxCourant,
                               &s.violators, &s.Tmin, &s.Tmax, &s.heat),
               "sphk_heat_stats");
+    return s;
+}
+
+// addition (no reference counterpart): fluid-solid adhesion, sphk.h
+bool BasicSPHSolver::setAdhesion(const sphb200::Adhesion& a) {
+    bool ok = finiteNonneg(a.wall) && a.bodies.size() <= SPHK_BODY_LIMIT;
+    for (float b : a.bodies) ok = ok && finiteNonneg(b);
+    if (!ok) {
+        printf("setAdhesion: need finite beta >= 0 and at most %d bodies; the setting is kept\n", SPHK_BODY_LIMIT);
+        return false;
+    }
+    if (bodies_ >= 0 && static_cast<int>(a.bodies.size()) > bodies_) {
+        printf("setAdhesion: %d body entries, but the system has %d bodies; the setting is kept\n", static_cast<int>(a.bodies.size()),
+               bodies_);
+        return false;
+    }
+    sphk_adhesion_setting abi{};
+    abi.n_groups = 1 + static_cast<int>(a.bodies.size());
+    abi.beta[0] = a.wall;
+    for (size_t b = 0; b < a.bodies.size(); ++b) abi.beta[b + 1] = a.bodies[b];
+    if (!adhesionOn_ || std::memcmp(&abi, &adhesionAbi_, sizeof(abi)) != 0) ++configEpoch_;
+    adhesionOn_ = true; adhesionAbi_ = abi;
+    return true;
+}
+
+void BasicSPHSolver::clearAdhesion() {
+    if (adhesionOn_) ++configEpoch_;
+    adhesionOn_ = false;
+}
+
+sphb200::AdhesionStats BasicSPHSolver::lastAdhesionStats() const {
+    sphb200::AdhesionStats s;
+    if (current_.ctx) check(sphk_adhesion_stats(current_.ctx, &s.wetted, &s.maxAccel), "sphk_adhesion_stats");
     return s;
 }
 

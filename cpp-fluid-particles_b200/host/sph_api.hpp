@@ -162,6 +162,15 @@ struct ThermalStats {
     float Tmin = 0.0f, Tmax = 0.0f;  // over the live fluid particles
     double heat = 0.0;               // sum m T
 };
+// addition: fluid-solid adhesion (DESIGN.md section 2.11; sphk_adhesion in sphk.h)
+struct Adhesion {
+    float wall = 0.0f;               // beta >= 0 of the static walls
+    std::vector<float> bodies;       // beta >= 0 of body b (missing entries: the body does not adhere); at most SPHK_BODY_LIMIT
+};
+struct AdhesionStats {
+    int wetted = 0;                  // fluid particles with a boundary particle in the band R/2 < r <= R of a group with beta > 0
+    float maxAccel = 0.0f;           // largest |a_i|
+};
 }  // namespace sphb200
 
 // ---- DArray.h:21-54 ---------------------------------------------------------------------------
@@ -324,6 +333,15 @@ public:
     // wallFactor > 0 with dynamic bodies.  Its iterations are lastViscosityIterations().
     bool setThermalViscosity(const sphb200::ThermalViscosity& v);
     void clearThermalViscosity();
+    // addition: fluid-solid adhesion (DESIGN.md section 2.11).  When set, the velocity stage pulls the fluid towards the walls and
+    // bodies right after its viscosity and surface-tension terms (dynamic bodies receive the reaction).  A negative or non-finite
+    // beta, more than SPHK_BODY_LIMIT bodies and (after the first step) more body entries than the system has bodies are refused
+    // (printed, setting kept; returns false).
+    bool setAdhesion(const sphb200::Adhesion& a);
+    void clearAdhesion();
+    bool adhesionOn() const { return adhesionOn_; }
+    // statistics of the last step's adhesion sweep (zeros before the first); synchronises
+    sphb200::AdhesionStats lastAdhesionStats() const;
     // addition: true when step() enqueues the same kernel sequence every call and never synchronises the host.
     // Only the three shipped solver types can say so: a user-derived solver (the reference API allows subclassing
     // BasicSPHSolver) has per-step host logic of its own, so it is never captured into a step graph.
@@ -369,7 +387,7 @@ protected:
     };
     StepScene current_;
     // the velocity terms of every solver's step, in this order: vorticity omega, viscosity (xsph: PBD's XSPH with coefficient
-    // visc), surface tension, implicit viscosity, vorticity confinement, heat transfer (with buoyancy along G).  With fused sweeps and xsph false the colour gradient
+    // visc), surface tension, adhesion, implicit viscosity, vorticity confinement, heat transfer (with buoyancy along G).  With fused sweeps and xsph false the colour gradient
     // must be in colorGradBuffer() already (the density sweep computes it).
     void velocityStage(std::shared_ptr<SPHParticles>& fluids, const std::shared_ptr<SPHParticles>& boundaries,
                        const DArray<int>& cellStartFluid, const DArray<int>& cellStartBoundary, int3 cellSize, float cellLength,
@@ -428,6 +446,8 @@ private:
     int heatSubsteps_ = 0;
     void heat(const std::shared_ptr<SPHParticles>& fluids, float rho0, float rhoB, float dt, float3 G);
     void thermalViscosity(const std::shared_ptr<SPHParticles>& fluids, float rho0, float rhoB, float dt);
+    bool adhesionOn_ = false;
+    sphk_adhesion_setting adhesionAbi_{};    // the setting as the C-ABI takes it
 };
 
 // ---- DFSPHSolver.h:20-64 ----------------------------------------------------------------------

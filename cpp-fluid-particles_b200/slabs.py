@@ -1000,6 +1000,16 @@ class SlabSystem(SphkOps):
         if spec is not None:
             raise ValueError("non-Newtonian viscosity is not supported on slab ranks (single-GPU engine.SphkSystem only)")
 
+    # adhesion: the boundary walk and the body reaction are single-context only
+    @property
+    def adhesion(self):
+        return None
+
+    @adhesion.setter
+    def adhesion(self, spec):
+        if spec is not None:
+            raise ValueError("adhesion is not supported on slab ranks (single-GPU engine.SphkSystem only)")
+
     # heat transfer: ghosts and strays would need their temperatures carried as a second array
     @property
     def thermal(self):

@@ -114,6 +114,13 @@ int   sph_app_download_temperature(sph_app* app, float* t_host);
 /* conduction substeps, largest dt_k sum c_ij and particle-substeps above 1 of the last step; min, max and sum m T of the current
  * temperatures (any pointer may be NULL); synchronises; 1 on the reference build */
 int   sph_app_thermal_stats(sph_app* app, int* substeps, float* max_courant, int* violators, float* t_min, float* t_max, double* heat);
+/* Fluid-solid adhesion in every following step (BasicSPHSolver::setAdhesion; DESIGN.md section 2.11): beta of the static walls
+ * (wall) and of body b (body_beta[b], b < n_bodies; bodies past n_bodies do not adhere).  on = 0: off.  Returns 1 on the
+ * reference build and for a setting the class layer refuses (the setting is then kept). */
+int   sph_app_set_adhesion(sph_app* app, int on, float wall, int n_bodies, const float* body_beta);
+/* wetted particles and the largest |a_i| of the last step's adhesion sweep (either pointer may be NULL); synchronises; 1 on the
+ * reference build */
+int   sph_app_adhesion_stats(sph_app* app, int* wetted, float* max_accel);
 /* Kinematic rigid bodies (SPHSystem's constructor with a vector of sphb200::KinematicBody; DESIGN.md section 2.3).  No
  * reference counterpart: NULL / 1 on the reference build.  Body b is the points body_xyz[body_begin[b] .. body_begin[b+1])
  * (body coordinates; body_begin[0] = 0), pose[7 b ..] = {cx, cy, cz, qx, qy, qz, qw} (quaternion scalar part last),

@@ -392,6 +392,34 @@ int sphk_thermal_viscosity(sphk_ctx* ctx, const sphk_scene* s, float* work, floa
                            int max_iter);
 int sphk_thermal_viscosity_eval(sphk_ctx* ctx, const sphk_viscosity_law* law, const float* temperature, float* nu_out, int n);
 
+/* ---- fluid-solid adhesion (Akinci et al. 2013; no reference counterpart; DESIGN.md section 2.11) -------------------------------
+ * Every fluid particle i is pulled towards the boundary particles b near it; fluid pairs contribute nothing (the fluid's cohesion is
+ * the surface tension of sphk_surface).  With x_ib = x_i - x_b, r = |x_ib|, g(b) the group of b (0 = the static walls, k + 1 = body
+ * k) and m_b the boundary mass:
+ *   a_i = - sum_b beta_g(b) Psi_b A(r) x_ib / r,   Psi_b = rho0 m_b / rho_boundary
+ *   A(r) = 0.007 / R^3.25 (-4 r^2 / R + 6 r - 2 R)^(1/4)   for R/2 < r <= R, else 0
+ *   v_i += dt a_i   (API velocities and records; a particle without such a pair gets no write)
+ * Groups at or past n_groups do not adhere.  The sweep walks the boundary cell ranges around each particle's current cell (no
+ * neighbour list), so every execution path gives the same bits.  When the context has declared dynamics (sphk_bodies_set_dynamics),
+ * sphk_adhesion also gathers the reaction dt m_i beta_g Psi_k A x_ik / r and its moment into the bodies' impulse of the step
+ * (sphk_bodies_integrate), like sphk_bodies_react.  The sweep counts the "wetted" particles (some pair in the band with beta > 0)
+ * and the largest |a_i|.
+ * SPHK_ERR_INVALID: NULL pointers, a non-finite or negative beta, n_groups outside [1, SPHK_ADHESION_GROUPS], rho0 or
+ * rho_boundary <= 0, dt < 0 or non-finite.  SPHK_ERR_STATE: an active range (slab ranks), or n_groups above 1 + the bodies of the
+ * context. */
+#define SPHK_ADHESION_GROUPS (1 + SPHK_BODY_LIMIT)
+typedef struct sphk_adhesion_setting {
+    int n_groups;                           /* entries of beta[] in use */
+    float beta[SPHK_ADHESION_GROUPS];       /* adhesion strength >= 0 of the static walls [0] and of body k [k + 1] */
+} sphk_adhesion_setting;
+int sphk_adhesion(sphk_ctx* ctx, const sphk_scene* s, const sphk_adhesion_setting* adhesion, float dt, float rho0, float rho_boundary);
+/* per element (tests): a_i into accel (device float[3 n]) and the statistics; no velocity write, no reaction */
+int sphk_adhesion_accel(sphk_ctx* ctx, const sphk_scene* s, const sphk_adhesion_setting* adhesion, float* accel, float rho0,
+                        float rho_boundary);
+/* the wetted count and the largest |a_i| of the last sphk_adhesion / sphk_adhesion_accel (0 before the first); either pointer
+ * may be NULL.  Synchronises. */
+int sphk_adhesion_stats(sphk_ctx* ctx, int* wetted, float* max_accel);
+
 /* ---- kinematic rigid bodies (no reference counterpart; DESIGN.md section 2.3) ---------------------------------------------
  * A body is a rigid set of boundary particles given in body coordinates r_k, with a pose (centre c, unit quaternion q) and
  * a motion (linear velocity V, angular velocity Omega, both in the world frame).  Poses and motions live in device memory.
