@@ -12,7 +12,15 @@
 //                [--bullets K] [--stir OMEGA] [--float REL] [--implicit-viscosity NU] [--tap SPEED] [--drain SIDE] [--capacity N]
 //                [--cfl C [--dt-min X]] [--rheology cross:NU0,NUINF,LAMBDA,M | hb:K,N,TAU[,MREG] [--rheology-max NU_MAX] [--no-slip]]
 //                [--heat ALPHA,BETA[,TREF] [--heater T] [--wall-temp T[,H]] [--tap-temp T] [--thermal-viscosity NUREF,E[,NUMAX]]]
-//                [--adhesion BETA[,BODYBETA]]
+//                [--adhesion BETA[,BODYBETA]] [--obstacle FILE[,S,X,Y,Z]]... [--mesh-body FILE,REL[,S,X,Y,Z]] [--fluid-mesh FILE[,S,X,Y,Z]]
+// --obstacle, --mesh-body and --fluid-mesh build the scene from Wavefront OBJ meshes (sphb200::loadObj, DESIGN.md section 2.12), each
+// mapped by S * v + (X, Y, Z) (default 1 and 0).  --obstacle (repeatable) is a static obstacle: its surface sampled at the boundary
+// spacing (sphb200::sampleSurface) is appended to the boundary set after the tank shell, so it has the walls' adhesion and
+// temperature.  --mesh-body adds one body (sphb200::meshBody) of relative density REL (0: kinematic, at rest), not together with
+// --stir, --float or --heater; with it the result line carries the body's pose, motion and last impulse.  --fluid-mesh fills the
+// mesh at the fluid spacing from --origin (sphb200::fillMesh) instead of the block.  The fluid is cleared of every obstacle and the
+// body at the boundary spacing (sphb200::clearOf), which needs the inside of every mesh: all three options take closed meshes
+// only, and every mesh must lie in [0, 0.99 box].  Single GPU only; with them --emit-scene needs a GPU too.
 // --adhesion turns on fluid-solid adhesion (BasicSPHSolver::setAdhesion, DESIGN.md section 2.11) after the constructor's step 0: the
 // tank walls with BETA, the --stir paddle, the --float cube or the --heater plate with BODYBETA (default BETA).  Every frame prints
 // the wetted particles and the largest adhesion acceleration; with --float the result line also carries the cube's position and its
@@ -120,6 +128,8 @@ struct Options {
     int bullets = 0;                          // test aid: this many top-layer particles start at ~3 cell planes per step
     int ranks = 1, rank = -1;                 // --ranks N: SlabSPHSystem on N GPUs; --rank R: this process is rank R
     std::string rendezvous;
+    std::vector<std::string> obstacles;       // --obstacle FILE[,S,X,Y,Z] (repeatable)
+    std::string meshBody, fluidMesh;          // --mesh-body FILE,REL[,S,X,Y,Z], --fluid-mesh FILE[,S,X,Y,Z]
 };
 
 // --rheology MODEL:a,b,c[,d] -> the model (not yet checked against its ranges: setRheology does that)
@@ -163,6 +173,54 @@ bool floats_of(const std::string& spec, std::vector<float>& v) {
         v.push_back(x);
         at = comma + 1;
     }
+    return true;
+}
+
+// FILE[,REL][,S,X,Y,Z] of a mesh option
+struct MeshSpec {
+    std::string file;
+    float rel = 0.0f, scale = 1.0f;
+    float3 t = {0.0f, 0.0f, 0.0f};
+};
+
+bool mesh_spec_of(const std::string& spec, bool withRel, MeshSpec& m) {
+    const size_t comma = spec.find(',');
+    m = MeshSpec();
+    m.file = spec.substr(0, comma);
+    std::vector<float> v;
+    if (m.file.empty() || (comma != std::string::npos && !floats_of(spec.substr(comma + 1), v))) return false;
+    if (withRel) {
+        if (v.empty() || !(v[0] >= 0.0f)) return false;
+        m.rel = v[0];
+        v.erase(v.begin());
+    }
+    if (!v.empty() && v.size() != 4) return false;
+    if (v.size() == 4) { m.scale = v[0]; m.t = make_float3(v[1], v[2], v[3]); }
+    return true;
+}
+
+// reads and checks one mesh option's mesh before any CUDA call: parsed, closed where required, inside [0, 0.99 box]
+bool load_mesh(const char* option, const std::string& spec, bool withRel, bool needClosed, const float box[3], MeshSpec& s,
+               sphb200::TriangleMesh& m) {
+    if (!mesh_spec_of(spec, withRel, s)) {
+        std::fprintf(stderr, "sph_headless: %s needs FILE%s[,S,X,Y,Z] with finite values\n", option, withRel ? ",REL" : "");
+        return false;
+    }
+    try {
+        m = sphb200::loadObj(s.file, s.scale, s.t);
+        if (needClosed && !sphb200::meshProperties(m).closed) {
+            std::fprintf(stderr, "sph_headless: %s %s: the mesh is not closed\n", option, s.file.c_str());
+            return false;
+        }
+    } catch (const std::exception& e) {
+        std::fprintf(stderr, "sph_headless: %s %s\n", option, e.what());
+        return false;
+    }
+    for (const float3& v : m.vertices)
+        if (!(v.x >= 0.0f && v.y >= 0.0f && v.z >= 0.0f && v.x <= 0.99f * box[0] && v.y <= 0.99f * box[1] && v.z <= 0.99f * box[2])) {
+            std::fprintf(stderr, "sph_headless: %s %s: the mesh leaves the box [0, 0.99 * box]\n", option, s.file.c_str());
+            return false;
+        }
     return true;
 }
 
@@ -236,6 +294,9 @@ bool parse(int argc, char** argv, Options& o) {
         else if (a == "--ranks" && need(i, 1)) o.ranks = std::atoi(argv[++i]);
         else if (a == "--rank" && need(i, 1)) o.rank = std::atoi(argv[++i]);
         else if (a == "--rendezvous" && need(i, 1)) o.rendezvous = argv[++i];
+        else if (a == "--obstacle" && need(i, 1)) o.obstacles.push_back(argv[++i]);
+        else if (a == "--mesh-body" && need(i, 1)) o.meshBody = argv[++i];
+        else if (a == "--fluid-mesh" && need(i, 1)) o.fluidMesh = argv[++i];
         else if (a == "--block" && need(i, 3)) { for (int k = 0; k < 3; ++k) o.block[k] = std::atoi(argv[++i]); }
         else if (a == "--origin" && need(i, 3)) { for (int k = 0; k < 3; ++k) o.origin[k] = static_cast<float>(std::atof(argv[++i])); }
         else if (a == "--box" && need(i, 1)) {
@@ -326,6 +387,14 @@ bool parse(int argc, char** argv, Options& o) {
     }
     if (o.cfl > 0.0f && o.ranks > 1) {
         std::fprintf(stderr, "sph_headless: --cfl runs on one GPU only (adaptive time stepping is not supported with --ranks)\n");
+        return false;
+    }
+    if ((!o.obstacles.empty() || !o.meshBody.empty() || !o.fluidMesh.empty()) && o.ranks > 1) {
+        std::fprintf(stderr, "sph_headless: --obstacle, --mesh-body and --fluid-mesh run on one GPU only (not with --ranks)\n");
+        return false;
+    }
+    if (!o.meshBody.empty() && (o.stir || o.floating || !o.heater.empty())) {
+        std::fprintf(stderr, "sph_headless: --mesh-body not together with --stir, --float or --heater\n");
         return false;
     }
     return o.frames >= 0 && o.vorticity >= 0.0f && o.block[0] > 0 && o.block[1] > 0 && o.block[2] > 0 &&
@@ -509,7 +578,8 @@ int main(int argc, char** argv) {
                              "[--origin X Y Z] [--dt DT] [--iters K] [--vorticity EPS] [--implicit-viscosity NU] [--stir OMEGA | --float REL] "
                              "[--tap SPEED] [--drain SIDE] [--capacity N] [--cfl C [--dt-min X]] [--rheology cross:NU0,NUINF,LAMBDA,M | hb:K,N,TAU[,MREG] "
                              "[--rheology-max NU_MAX] [--no-slip]] [--heat ALPHA,BETA[,TREF] [--heater T] [--wall-temp T[,H]] "
-                             "[--tap-temp T] [--thermal-viscosity NUREF,E[,NUMAX]]] [--adhesion BETA[,BODYBETA]] [--dump PREFIX] [--quiet] "
+                             "[--tap-temp T] [--thermal-viscosity NUREF,E[,NUMAX]]] [--adhesion BETA[,BODYBETA]] [--obstacle FILE[,S,X,Y,Z]]... "
+                             "[--mesh-body FILE,REL[,S,X,Y,Z]] [--fluid-mesh FILE[,S,X,Y,Z]] [--dump PREFIX] [--quiet] "
                              "[--emit-scene PREFIX] "
                              "[--ranks N [--rank R --rendezvous DIR]]\n");
         return 2;
@@ -523,18 +593,48 @@ int main(int argc, char** argv) {
                                     static_cast<int>(std::ceil(spaceSize.z / sphCellLength)));
     // the boundary shell's lattice spacing along x (boundary_shell: 0.99 * space / (2 * cells - 1))
     const float boundarySpacing = 0.99f * spaceSize.x / float(2 * cellSize.x - 1);
+    // ---- meshes: read and checked before any CUDA call ----
+    std::vector<sphb200::TriangleMesh> carve;               // the obstacles, then the body: the fluid is cleared of them
+    sphb200::TriangleMesh bodyMesh, fluidMesh;
+    MeshSpec spec;
+    for (const std::string& ob : o.obstacles) {
+        carve.emplace_back();
+        if (!load_mesh("--obstacle", ob, false, true, o.box, spec, carve.back())) return 2;
+    }
+    const size_t nObstacles = carve.size();
+    float meshRel = 0.0f;
+    if (!o.meshBody.empty()) {
+        if (!load_mesh("--mesh-body", o.meshBody, true, true, o.box, spec, bodyMesh)) return 2;
+        meshRel = spec.rel;
+        carve.push_back(bodyMesh);
+    }
+    if (!o.fluidMesh.empty() && !load_mesh("--fluid-mesh", o.fluidMesh, false, true, o.box, spec, fluidMesh)) return 2;
     std::vector<sphb200::KinematicBody> bodies;
-    std::vector<float3> fluidPoints = fluid_block(o, sphSpacing);
+    std::vector<float3> fluidPoints, boundaryPoints = boundary_shell(cellSize, spaceSize);
+    try {
+        fluidPoints = o.fluidMesh.empty() ? fluid_block(o, sphSpacing)
+                                          : sphb200::fillMesh(fluidMesh, sphSpacing, make_float3(o.origin[0], o.origin[1], o.origin[2]), 0.0f);
+        for (size_t k = 0; k < nObstacles; ++k) {
+            const std::vector<float3> s = sphb200::sampleSurface(carve[k], boundarySpacing);
+            boundaryPoints.insert(boundaryPoints.end(), s.begin(), s.end());
+        }
+        if (!o.meshBody.empty())
+            bodies.push_back(sphb200::meshBody(bodyMesh, boundarySpacing, meshRel, kSphM0 / (sphSpacing * sphSpacing * sphSpacing)));
+        if (!carve.empty()) fluidPoints = sphb200::clearOf(fluidPoints, carve, boundarySpacing);
+    } catch (const std::exception& e) {
+        std::fprintf(stderr, "sph_headless: building the mesh scene failed: %s\n", e.what());
+        return 4;
+    }
     if (o.stir) bodies.push_back(paddle(o, sphSpacing, boundarySpacing));
     if (o.floating) bodies.push_back(floating_cube(o, sphSpacing, boundarySpacing));
     if (!o.heater.empty()) bodies.push_back(heater_plate(o, sphSpacing, boundarySpacing));
-    if (!bodies.empty()) fluidPoints = clear_of(fluidPoints, bodies[0], boundarySpacing);
+    if (!bodies.empty() && o.meshBody.empty()) fluidPoints = clear_of(fluidPoints, bodies[0], boundarySpacing);
     const sphb200::OpenBoundaries openB = open_boundaries(o, sphSpacing);
     const bool open = !openB.emitters.empty() || !openB.sinks.empty();
     if (!o.emitScene.empty()) {
         const int3 cells = cellSize;
         bool ok = write_floats(o.emitScene + ".fluid.f32", flat(fluidPoints)) &&
-                  write_floats(o.emitScene + ".boundary.f32", flat(boundary_shell(cells, spaceSize)));
+                  write_floats(o.emitScene + ".boundary.f32", flat(boundaryPoints));
         if (ok && !bodies.empty()) {
             const auto& b = bodies[0];
             ok = write_floats(o.emitScene + ".body.f32", flat(b.points)) &&
@@ -542,7 +642,7 @@ int main(int argc, char** argv) {
                               {b.position.x, b.position.y, b.position.z, b.orientation.x, b.orientation.y, b.orientation.z, b.orientation.w,
                                b.linearVelocity.x, b.linearVelocity.y, b.linearVelocity.z, b.angularVelocity.x, b.angularVelocity.y,
                                b.angularVelocity.z});
-            if (ok && o.floating)
+            if (ok && (o.floating || !o.meshBody.empty()))
                 ok = write_floats(o.emitScene + ".body_dyn.f32", {b.mass, b.inertia.x, b.inertia.y, b.inertia.z});
         }
         for (const auto& e : openB.emitters)
@@ -612,7 +712,7 @@ int main(int argc, char** argv) {
     const unsigned int capacity = open ? static_cast<unsigned int>(o.capacity > 0 ? o.capacity : 2LL * static_cast<long long>(fluidPoints.size()))
                                        : static_cast<unsigned int>(fluidPoints.size());
     auto fluidParticles = open ? std::make_shared<SPHParticles>(fluidPoints, capacity) : std::make_shared<SPHParticles>(fluidPoints);
-    auto boundaryParticles = std::make_shared<SPHParticles>(boundary_shell(cellSize, spaceSize));
+    auto boundaryParticles = std::make_shared<SPHParticles>(boundaryPoints);
     const int nFluid = static_cast<int>(fluidParticles->size()), nBoundary = static_cast<int>(boundaryParticles->size());
     const int nSlots = static_cast<int>(fluidParticles->capacity());   // the solver's buffers hold every slot
     std::shared_ptr<BaseSolver> pSolver;
@@ -798,6 +898,18 @@ int main(int argc, char** argv) {
                           J.x, J.y, J.z);
             openJson += bb;
         }
+    }
+    if (!o.meshBody.empty()) {
+        float3 c, V, W, J, H;
+        float4 q;
+        pSystem->getBodyPose(0, c, q);
+        pSystem->getBodyMotion(0, V, W);
+        pSystem->getBodyImpulse(0, J, H);
+        char bb[512];
+        std::snprintf(bb, sizeof bb, ", \"body_pose\": [%.9g, %.9g, %.9g, %.9g, %.9g, %.9g, %.9g], \"body_motion\": [%.9g, %.9g, %.9g, %.9g, %.9g, "
+                      "%.9g], \"body_impulse\": [%.9g, %.9g, %.9g, %.9g, %.9g, %.9g]", c.x, c.y, c.z, q.x, q.y, q.z, q.w, V.x, V.y, V.z, W.x, W.y,
+                      W.z, J.x, J.y, J.z, H.x, H.y, H.z);
+        openJson += bb;
     }
     if (open) {
         const sphb200::OpenBoundaryStats st = pSystem->openBoundaryStats();

@@ -41,6 +41,8 @@ SPHK_FUNCTIONS = [
     "sphk_visc_field_setup", "sphk_visc_field_matvec",
     "sphk_heat_substeps", "sphk_heat_step", "sphk_heat_conduction", "sphk_heat_stats", "sphk_thermal_viscosity",
     "sphk_thermal_viscosity_eval", "sphk_adhesion", "sphk_adhesion_accel", "sphk_adhesion_stats",
+    "sphk_mesh_transform", "sphk_mesh_properties", "sphk_mesh_create", "sphk_mesh_destroy", "sphk_mesh_classify", "sphk_mesh_fill",
+    "sphk_mesh_sample_surface",
 ]
 SPH_APP_FUNCTIONS = [
     "sph_app_create", "sph_app_destroy", "sph_app_step", "sph_app_fluid_size", "sph_app_boundary_size",
@@ -51,7 +53,7 @@ SPH_APP_FUNCTIONS = [
     "sph_app_viscosity_stats", "sph_app_create_open", "sph_app_open_boundary_stats", "sph_app_set_adaptive_dt", "sph_app_advance",
     "sph_app_adaptive_stats", "sph_app_set_rheology", "sph_app_rheology_stats", "sph_app_download_viscosity",
     "sph_app_set_thermal", "sph_app_set_thermal_viscosity", "sph_app_upload_temperature", "sph_app_download_temperature",
-    "sph_app_thermal_stats", "sph_app_set_adhesion", "sph_app_adhesion_stats",
+    "sph_app_thermal_stats", "sph_app_set_adhesion", "sph_app_adhesion_stats", "sph_app_load_obj", "sph_app_load_obj_error",
 ]
 
 BODY_LIMIT = 64                      # SPHK_BODY_LIMIT
@@ -253,6 +255,7 @@ def sphk():
         L.sphk_rheology_work_floats.restype = C.c_longlong
         L.sphk_destroy.restype = None
         L.sphk_mg_destroy.restype = None
+        L.sphk_mesh_destroy.restype = None
         _sphk = L
     return _sphk
 
@@ -270,6 +273,7 @@ def app_lib(path: str = LIBHOST):
         L.sph_app_step.restype = C.c_float
         L.sph_app_engine.restype = C.c_char_p
         L.sph_app_destroy.restype = None
+        L.sph_app_load_obj_error.restype = C.c_char_p
         _apps[path] = L
     return _apps[path]
 

@@ -10,6 +10,7 @@
 #include <iostream>
 #include <vector>
 #include <memory>
+#include <string>
 #include <cuda_runtime.h>
 #ifdef SPH_APP_REFERENCE_ENGINE
 #include <helper_math.h>
@@ -712,5 +713,43 @@ extern "C" const char* sph_app_engine(void) {
     return "reference-cuda";
 #else
     return "b200-native";
+#endif
+}
+
+#ifndef SPH_APP_REFERENCE_ENGINE
+static thread_local std::string g_load_obj_error;
+#endif
+
+extern "C" int sph_app_load_obj(const char* path, float scale, const float* t, float* v, int v_cap, int* tri, int t_cap, int* nv, int* nt) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)path; (void)scale; (void)t; (void)v; (void)v_cap; (void)tri; (void)t_cap; (void)nv; (void)nt;
+    return 1;
+#else
+    g_load_obj_error.clear();
+    if (!path || !t || !nv || !nt || v_cap < 0 || t_cap < 0 || (v_cap > 0 && !v) || (t_cap > 0 && !tri)) {
+        g_load_obj_error = "sph_app_load_obj: invalid argument";
+        return 1;
+    }
+    sphb200::TriangleMesh m;
+    try {
+        m = sphb200::loadObj(path, scale, make_float3(t[0], t[1], t[2]));
+    } catch (const std::exception& e) {
+        g_load_obj_error = e.what();
+        return 1;
+    }
+    *nv = static_cast<int>(m.vertices.size());
+    *nt = static_cast<int>(m.triangles.size());
+    if (*nv > v_cap || *nt > t_cap) return 2;
+    std::copy(m.vertices.begin(), m.vertices.end(), reinterpret_cast<float3*>(v));
+    std::copy(m.triangles.begin(), m.triangles.end(), reinterpret_cast<int3*>(tri));
+    return 0;
+#endif
+}
+
+extern "C" const char* sph_app_load_obj_error(void) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    return "";
+#else
+    return g_load_obj_error.c_str();
 #endif
 }

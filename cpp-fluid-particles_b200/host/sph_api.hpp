@@ -13,6 +13,7 @@
 #include <functional>
 #include <iostream>
 #include <memory>
+#include <string>
 #include <type_traits>
 #include <typeinfo>
 #include <vector>
@@ -171,6 +172,37 @@ struct AdhesionStats {
     int wetted = 0;                  // fluid particles with a boundary particle in the band R/2 < r <= R of a group with beta > 0
     float maxAccel = 0.0f;           // largest |a_i|
 };
+
+// addition: scenes from triangle meshes (DESIGN.md section 2.12; sphk_mesh_* in sphk.h).  The functions below run on the legacy
+// default stream, need no SPHSystem, and throw std::runtime_error when the library refuses a mesh or a call fails.
+struct TriangleMesh {
+    std::vector<float3> vertices;
+    std::vector<int3> triangles;     // vertex indices, counter-clockwise seen from outside on a closed mesh
+};
+// sphk_mesh_properties as named fields; closed = false leaves everything but the area 0
+struct MeshProperties {
+    bool closed = false;
+    double area = 0.0, volume = 0.0;
+    double centroid[3] = {0, 0, 0};
+    double inertia[6] = {0, 0, 0, 0, 0, 0};      // per unit density about the centroid: xx, yy, zz, xy, xz, yz
+    double principal[3] = {0, 0, 0};             // ascending
+    double orientation[4] = {0, 0, 0, 1};        // body (principal) axes -> world, (x, y, z, w)
+};
+// Wavefront OBJ: `v x y z [w]` and `f` with i, i/j, i//k or i/j/k items (1-based, negative = from the end), polygons fan-
+// triangulated; every other line is ignored.  Vertices are mapped by scale * v + translate (sphk_mesh_transform).  Throws
+// std::runtime_error naming the file and line of a malformed number or index.
+TriangleMesh loadObj(const std::string& path, float scale = 1.0f, float3 translate = float3{0.0f, 0.0f, 0.0f});
+MeshProperties meshProperties(const TriangleMesh& mesh);
+std::vector<float3> sampleSurface(const TriangleMesh& mesh, float r);                       // sphk_mesh_sample_surface
+std::vector<float3> fillMesh(const TriangleMesh& mesh, float spacing, float3 origin, float clearance);   // sphk_mesh_fill
+// the points that are neither inside nor within `clearance` of any of the (closed) meshes, in their order
+std::vector<float3> clearOf(const std::vector<float3>& points, const std::vector<TriangleMesh>& meshes, float clearance);
+// The fluid's mass per unit volume in the reference's scenes, m0 / spacing^3 (see KinematicBody)
+constexpr float kSceneFluidMassPerVolume = 76.596750762082e-6f / (0.02f * 0.02f * 0.02f);
+// A body of a closed mesh: surface samples at r in its principal frame, position = centroid, orientation = principal axes,
+// mass = relDensity * fluidMassPerVolume * V and inertia = the principal moments times that density (relDensity = 0: kinematic),
+// at rest.
+KinematicBody meshBody(const TriangleMesh& mesh, float r, float relDensity, float fluidMassPerVolume = kSceneFluidMassPerVolume);
 }  // namespace sphb200
 
 // ---- DArray.h:21-54 ---------------------------------------------------------------------------

@@ -183,6 +183,13 @@ int   sph_app_advance(sph_app* app, double frame_seconds, int* substeps, float* 
  * set the bound (0 fluid, 1 body, 2 emitter), counts2 = {steps held at dt_min, steps with non-finite velocities or bound},
  * *simulated_time = the double sum of the float dt of every step.  Any pointer may be NULL; 1 on the reference build. */
 int   sph_app_adaptive_stats(sph_app* app, float* speed_dt3, int* source, long long* counts2, double* simulated_time);
+/* Scenes from triangle meshes (DESIGN.md section 2.12): the class layer's Wavefront OBJ reader (sphb200::loadObj: v, and f with
+ * i, i/j, i//k, i/j/k items, negative indices and fan-triangulated polygons), vertices mapped by scale * v + t (sphk_mesh_transform).
+ * Host only, no device.  v: float[3 v_cap], tri: int[3 t_cap] (0-based).  0: read, *nv / *nt set; 2: read, but *nv > v_cap or
+ * *nt > t_cap -- the counts are set and nothing is written; 1: refused (an unreadable file, a malformed number or index; the
+ * message, naming the line, is sph_app_load_obj_error(): valid until the thread's next call) or the reference build. */
+int   sph_app_load_obj(const char* path, float scale, const float* t, float* v, int v_cap, int* tri, int t_cap, int* nv, int* nt);
+const char* sph_app_load_obj_error(void);
 /* Name of the engine underneath: "reference-cuda" or "b200-native". */
 const char* sph_app_engine(void);
 

@@ -599,6 +599,47 @@ int sphk_scene_fluid_block(float* pos_out, int nx, int ny, int nz, const float o
 long long sphk_scene_boundary_count(const int cell_size[3]);
 int sphk_scene_boundary_shell(float* pos_out, const int cell_size[3], const float space[3], void* stream);
 
+/* ---- scenes from triangle meshes (no reference counterpart; DESIGN.md section 2.12) -----------------------------------------
+ * A mesh is float3 vertices and int3 triangles (counter-clockwise seen from outside on a closed mesh).  None of these entries
+ * needs an sphk_ctx; all are safe before sphk_create.  Every entry checks all of its arguments before anything is launched or
+ * allocated: NULL or overlapping buffers, counts <= 0, a triangle index outside [0, nv) and a non-finite vertex or parameter give
+ * SPHK_ERR_INVALID.
+ * sphk_mesh_transform: host only, v_out = scale * v_in + t per coordinate in float (multiply, then add; no contraction) -- the one
+ *   place a mesh transform is computed, so every layer gets the same bits.
+ * sphk_mesh_properties: host only, in double.  flags bit SPHK_MESH_CLOSED: every edge is shared by exactly two triangles that
+ *   run it in opposite directions (and nt >= 4).  out = {area, V, centroid xyz, inertia tensor per unit density about the centroid
+ *   {xx, yy, zz, xy, xz, yz}, principal moments ascending (3), the rotation from the principal (body) axes to the world as a unit
+ *   quaternion (x, y, z, w)} by the divergence theorem; the body axes have det +1, each of the first two has its largest component
+ *   positive, and w >= 0.  A closed mesh with reversed winding gives the same outputs (|V|, the tensor's sign flipped with V).  An
+ *   open mesh reports the area only (the rest 0). */
+#define SPHK_MESH_PROPS 18
+#define SPHK_MESH_CLOSED 1
+#define SPHK_MESH_INSIDE 1        /* sphk_mesh_classify flag bits */
+#define SPHK_MESH_NEAR 2
+typedef struct sphk_mesh sphk_mesh;
+int sphk_mesh_transform(const float* v_in, int nv, float scale, const float t[3], float* v_out);
+int sphk_mesh_properties(const float* v, int nv, const int* tri, int nt, double out[SPHK_MESH_PROPS], int* flags);
+/* Uploads the mesh (host arrays) and bins its triangles, in triangle-index order, into a 3D uniform grid (distance queries) and a
+ * 2D (x, z) column grid (ray parity).  Every later call on the mesh runs on `stream`. */
+int sphk_mesh_create(sphk_mesh** m, const float* v_host, int nv, const int* tri_host, int nt, void* stream);
+void sphk_mesh_destroy(sphk_mesh* m);
+/* Device arrays pos float3[n] -> flags_out int[n]: SPHK_MESH_INSIDE = odd number of crossings of the +y ray from the point
+ * (watertight: exact orientation predicates in (x, z) and one fixed tie rule, so a ray through a shared edge or vertex counts
+ * once); SPHK_MESH_NEAR = distance to the surface <= clearance (>= 0).  Asynchronous.  SPHK_ERR_INVALID also for an open mesh. */
+int sphk_mesh_classify(const sphk_mesh* m, const float* pos, int n, float clearance, int* flags_out);
+/* The lattice points origin + spacing * (j, i, k) (float multiply then add, as sphk_scene_fluid_block) over the mesh's bounding box
+ * that are inside and not near (clearance), in the fluid block's order (i = y outermost, then j = x, k = z innermost).  pos_out:
+ * device float3[capacity]; *count_host = the number of such points; when it exceeds capacity nothing is written.  Synchronises.
+ * SPHK_ERR_INVALID also for an open mesh, spacing <= 0 and a lattice of more than 2^31 - 1 points over the box. */
+int sphk_mesh_fill(const sphk_mesh* m, float spacing, const float origin[3], float clearance, float* pos_out, int capacity,
+                   int* count_host);
+/* A maximal Poisson-disk sampling of the surface (open meshes too) with minimum distance r: candidates on a barycentric lattice of
+ * spacing <= r/4 per triangle (edges and vertices included), accepted in (cell, candidate) order in 27 colour phases of cells of
+ * side >= r.  Every sample lies on a triangle, no two are closer than r, every surface point is within r + r/4 of a sample, and
+ * the output (ordered by cell, then candidate) is the same on every call.  pos_out: device float3[capacity]; *count_host and
+ * capacity as sphk_mesh_fill.  Synchronises.  SPHK_ERR_INVALID also for r <= 0 and more than 2^31 - 1 candidates. */
+int sphk_mesh_sample_surface(const sphk_mesh* m, float r, float* pos_out, int capacity, int* count_host);
+
 /* ---- render export: generate_dots_CUDA, vbo.cu:26-44 (SURVEY 8f-2) -----------------------------------------------
  * dot[i] = pos[i]; colour[i] from density[i] (blue below 0.75, blend to white at 1.0, blend to pink above).  Plain
  * device buffers instead of a mapped GL vertex buffer; synchronises like the reference (vbo.cu:49). */
