@@ -151,6 +151,85 @@ def test_mesh_cube_matches_the_float_cube_formula(pkg, built):
     assert np.allclose(np.asarray(p["principal"]) * rho, float(I), rtol=1e-5)
 
 
+def _bin_sides(v, f):
+    """sphk_mesh_create's 3D cell side candidates: the mean bounding-box side of a triangle and 1/128 of the largest extent"""
+    v = np.asarray(v, np.float32).astype(np.float64)
+    t = v[np.asarray(f)]
+    side = ((t.max(1) - t.min(1)).sum(1) / 3.0).mean()
+    return side, (v.max(0) - v.min(0)).max() / 128.0
+
+
+def test_edge_case_reference_meshes(pkg, built):
+    """the meshes of test_gpu_mesh_edges.py: closed by the library's edge criterion, with the volumes their construction gives,
+    a heightfield whose closed-form top matches its vertices, bins in the regime each mesh is meant for, and lattice() equal to
+    scene.fluid_lattice bit for bit"""
+    meshes = _meshes(pkg)
+    v, f, h = R.heightfield()
+    m = _mesh(meshes, (v, f))
+    assert np.array_equal(m.vertices.astype(np.float64), v)                  # dyadic: exact in float32
+    assert np.array_equal(h(v[:, 0], v[:, 2])[:len(v) // 2], v[:len(v) // 2, 1])
+    tri = v[f]
+    top = np.all(tri[:, :, 1] > 0.25, axis=1)                                # the top's prisms down to y = 0.25, exactly
+    xz = np.cross(tri[top, 1] - tri[top, 0], tri[top, 2] - tri[top, 0])[:, 1]
+    vol = (0.5 * xz * (tri[top, :, 1].mean(1) - 0.25)).sum()
+    p = m.properties()
+    assert p["closed"] and p["volume"] == pytest.approx(vol, rel=1e-12) and R.mass_properties(v, f)[0] == pytest.approx(vol, rel=1e-12)
+    for vf, vol in ((R.needle_fan(), 0.2 * 0.15 * 0.2), (R.tjunction_box(), 0.2 * 0.15 * 0.15)):
+        m = _mesh(meshes, vf)
+        p = m.properties()
+        assert p["closed"] and p["volume"] == pytest.approx(vol, rel=1e-6)
+        assert R.mass_properties(m.vertices, m.triangles)[0] == pytest.approx(p["volume"], rel=1e-12)
+    v, f = R.needle_fan()
+    a, b, c = (v[f[:, k]] for k in range(3))
+    edge = np.maximum(np.linalg.norm(b - a, axis=1), np.maximum(np.linalg.norm(c - b, axis=1), np.linalg.norm(a - c, axis=1)))
+    aspect = edge ** 2 / np.linalg.norm(np.cross(b - a, c - a), axis=1)     # longest edge over the height onto it
+    assert aspect.min() < 10 and 5e2 < np.sort(aspect)[-50] and aspect.max() > 1e5
+    v, f = R.tjunction_box()
+    a, b, c = (v[f[:, k]] for k in range(3))
+    assert np.count_nonzero(np.linalg.norm(np.cross(b - a, c - a), axis=1) == 0) == 1
+    for subdiv in (3, 4):
+        vf = R.box_and_sphere(subdiv)
+        m = _mesh(meshes, vf)
+        p = m.properties()
+        V = R.mass_properties(m.vertices, m.triangles)[0]
+        vs, fs = R.icosphere(subdiv, 0.03, (0.4, 0.3, 0.44))
+        band = R.sphere_band(vs, fs, 0.03, np.array([0.4, 0.3, 0.44])) * R.area(vs, fs)
+        assert p["closed"] and p["volume"] == pytest.approx(V, rel=1e-12)
+        assert abs(V - (0.3 * 0.2 * 0.15 + 4 / 3 * np.pi * 0.03 ** 3)) <= band
+        side, cap = _bin_sides(*vf)
+        assert side > cap if subdiv == 3 else side < cap          # the mean triangle sets the cell / the 128-cell cap binds
+    # the flat plate: closed, a zero y extent, and no volume (properties refuses it, but still reports closed)
+    v, f = R.flat_plate()
+    pm = _mesh(meshes, (v, f))
+    from cpp_fluid_particles_b200 import capi
+    out, fl = np.zeros(18), C.c_int(0)
+    P = lambda a: a.ctypes.data_as(C.c_void_p)           # noqa: E731
+    assert capi.sphk().sphk_mesh_properties(P(pm.vertices), len(v), P(pm.triangles), len(f), P(out), C.byref(fl)) == -1
+    assert fl.value & meshes.CLOSED and np.ptp(pm.vertices[:, 1]) == 0.0
+    # the large curved meshes: closed, and the polyhedral volume within band x area of the ideal solid's
+    for vf, ideal, band in (
+            (R.icosphere(5, 0.3, (0.5, 0.45, 0.5)), 4 / 3 * np.pi * 0.3 ** 3,
+             lambda v, f: R.sphere_band(v, f, 0.3, np.array([0.5, 0.45, 0.5]))),
+            (R.torus(0.25, 0.08, 256, 128, (0.5, 0.45, 0.5)), 2 * np.pi ** 2 * 0.25 * 0.08 ** 2,
+             lambda v, f: R.torus_band(v, f, 0.25, 0.08, np.array([0.5, 0.45, 0.5])))):
+        m = _mesh(meshes, vf)
+        p = m.properties()
+        vv = m.vertices.astype(np.float64)
+        V = R.mass_properties(vv, m.triangles)[0]
+        assert p["closed"] and p["volume"] == pytest.approx(V, rel=1e-12)
+        assert abs(V - ideal) <= band(vv, m.triangles) * R.area(vv, m.triangles)
+    # lattice() is scene.fluid_lattice over its own ranges, and fill_ranges() is the box fill's
+    o, s = (0.135, 0.055, 0.135), float(pkg.scene.SPACING)
+    assert np.array_equal(R.lattice(o, s, ((0, 9), (0, 13), (0, 9))).view(np.uint32), pkg.scene.fluid_lattice(10, 14, 10, o).view(np.uint32))
+    lo = np.array(o) - s / 2
+    hi = np.array(o) + s * np.array([9, 13, 9]) + s / 2
+    v, _ = R.box(lo, hi)
+    pts = R.lattice(o, s, R.fill_ranges(v, o, s))
+    v32 = np.float32(v)
+    inside = np.all((pts > v32.min(0)) & (pts < v32.max(0)), axis=1)
+    assert np.array_equal(pts[inside].view(np.uint32), pkg.scene.fluid_lattice(10, 14, 10, o).view(np.uint32))
+
+
 # ---- exports and refusals ------------------------------------------------------------------------------------------------------
 def test_exports(pkg, built):
     from cpp_fluid_particles_b200 import capi
