@@ -128,6 +128,22 @@ struct sphk_ctx {
     bool fluidSearched = false, boundarySearched = false, permValid = false;
     const int* lastCsB = nullptr;
     long long launches = 0;
+    // Pressure-solve activity (DFSPH; sphk_sweeps.cu, "Chunk activity"): a chunk is the 32 particles [32k, 32k + 32) of the
+    // sorted fluid set, i.e. one warp of a list sweep.
+    unsigned int* chunkAct = nullptr;          // device [capF / 32 + 1]: ballot of the chunk's particles whose rec.s may be non-zero
+    unsigned long long* chunkStamp = nullptr;  // device [capF / 32 + 1]: corrSeq of the last correct sweep that gathered in the chunk
+    bool listSpans = false;                    // tileWin[tile * 18 + 0..8] hold the fluid windows of the current list's tiles
+    long long credited = 0;                    // launches that write neither rec.s nor anything an error sweep reads, except
+                                               // velocities under chunk stamps (the correct sweeps) -- see act_mark()
+    long long actMark = -1;                    // act_mark() when chunkAct last described rec.s of every chunk
+    unsigned long long corrSeq = 0;            // correct sweeps launched (their stamp)
+    struct ErrTok {                            // the last DFSPH error sweep, reused while act_mark() == mark (kind 0: none)
+        int kind = 0;                          // 1 divergence (sphk_dfsph_div_error or the fused sweep), 2 density
+        const void *density = nullptr, *alpha = nullptr, *error = nullptr, *stiff = nullptr;
+        float dt = 0.f, rho0 = 0.f;
+        long long mark = -1;
+        unsigned long long seq = 0;            // corrSeq at that sweep: chunks stamped later have moved
+    } tok;
     BodyState* bodies = nullptr;     // non-null after sphk_bodies_init
     float* viscStats = nullptr;      // [2] device: {iterations (int bits), |r|_M / |b|_M} of the last sphk_implicit_viscosity
     float* rheoStats = nullptr;      // [6] device: {iterations, |r|_M / |b|_M, max gamma_dot, min nu, max nu, count at nu_max} of the
@@ -165,6 +181,10 @@ struct DevScene {
     int iBegin, iEnd;                // sweeps compute particles [iBegin, iEnd)
     const int* rangeDev;             // non-null: ... intersected with the device-resident range {begin, count}
     int patch;                       // > 0: the warps of a block take their 32-particle chunks from 4 runs `patch` chunks apart
+    unsigned int* act;               // non-null: this list sweep keeps (error sweeps) or reads (correct sweeps) chunk activity
+    unsigned long long* stamp;       // non-null: correct sweeps stamp the chunks they gathered in with `seq`
+    unsigned long long seq;          // correct sweeps: their stamp; error sweeps with `reuse`: the token's
+    int reuse;                       // error sweeps: the previous error sweep's outputs stand for chunks quiet since `seq`
     int3 cs, org;
     float cellLength;
     float r2list;                    // candidate cut-off of the cell walk: r2cut, or (R + skin)^2 when building a skin list

@@ -154,7 +154,7 @@ template <bool kDensity> struct OpDfsphError {
     Rec rec; const float* density; const float* alpha; float* error; float* stiff; float* warm;
     float dt, rho0;
     static constexpr bool kFluidOnly = false, kHi = true;
-    struct Acc { float e; float3 vi; template <class F> __device__ void sums(F f) { f(e); } };
+    struct Acc { float e; float3 vi; bool quiet; template <class F> __device__ void sums(F f) { f(e); } };
     __device__ void begin(Acc& a, int, float4, float4 hi, const DevScene&) const { a.e = 0.f; a.vi = xyz(hi); }
     __device__ void pair(Acc& a, int, int, bool, float3 d, float r2, float mj, float4 lo, float4 hi, const DevScene& s) const {
         a.e += mj * dot3(a.vi - xyz(hi), d * grad_w_factor(sqrtf(r2), s.k));
@@ -173,6 +173,11 @@ template <bool kDensity> struct OpDfsphError {
         stiff[i] = k;
         rec_set_s(rec + i, k);
         if (kDensity && warm) warm[i] += k;
+        // Quiet (chunk activity): e = +0 and kappa = -0, the state of every particle whose density and divergence errors are
+        // clamped to zero.  fmaxf(0, x) compiles to FMNMX.FTZ against RZ: +0 for every x <= 0 and for NaN; alpha = -1 / max(eps, .)
+        // is negative and finite, so kappa = (+0) * alpha = -0.  Then:  warm += kappa  leaves warm unchanged bit for bit
+        // (x + -0 = x for every x), and the particle adds an exact zero to every correct-sweep pair term it takes part in.
+        a.quiet = __float_as_uint(e) == 0u && __float_as_uint(k) == 0x80000000u;
     }
 };
 
@@ -294,6 +299,22 @@ template <bool kColorGrad> struct OpDensityAlphaDivError {
         p.b.finish(c.b, i, da->den, OpDensityAlpha::alpha_of(*da));
     }
 };
+
+// Roles in chunk activity (k_sweep_list): the DFSPH error sweeps produce the record scalar kappa and report whether each
+// particle left it quiet; the DFSPH correct sweeps consume it.  PBD's lambda sweeps (OpScalarGradient<2>) take no part.
+enum { kActNone = 0, kActError = 1, kActCorrect = 2 };
+struct act_never_quiet { template <class Acc> __device__ static bool quiet(const Acc&) { return false; } };
+template <class Op> struct act_of : act_never_quiet { static constexpr int role = kActNone; };
+template <bool kD> struct act_of<OpDfsphError<kD>> {
+    static constexpr int role = kActError;
+    __device__ static bool quiet(const typename OpDfsphError<kD>::Acc& a) { return a.quiet; }
+};
+template <bool kCG> struct act_of<OpDensityAlphaDivError<kCG>> {
+    static constexpr int role = kActError;
+    __device__ static bool quiet(const typename OpDensityAlphaDivError<kCG>::Acc& a) { return a.b.quiet; }
+};
+template <> struct act_of<OpScalarGradient<0>> : act_never_quiet { static constexpr int role = kActCorrect; };
+template <> struct act_of<OpScalarGradient<1>> : act_never_quiet { static constexpr int role = kActCorrect; };
 
 // viscosity + surface tension / air pressure in one sweep (BasicSPHSolver.cu:183-225 then :332-381): the
 // viscosity term reads the neighbours' velocity BEFORE either update (as both reference kernels do), the surface
@@ -743,9 +764,9 @@ __device__ __forceinline__ void walk_list(const DevScene& s, const Op& op, typen
     }
 }
 
-// one particle's walk of its neighbour list (thread per particle)
+// one particle's walk of its neighbour list (thread per particle); returns whether an error sweep left the particle quiet
 template <class Op>
-__device__ __forceinline__ void sweep_list_particle(const DevScene& s, const Op& op, int i) {
+__device__ __forceinline__ bool sweep_list_particle(const DevScene& s, const Op& op, int i) {
     float4 lo, hi;
     rec_full(s.rec + i, lo, hi);
     const float3 xi = xyz(lo);
@@ -766,20 +787,96 @@ __device__ __forceinline__ void sweep_list_particle(const DevScene& s, const Op&
         walk_cells(s, op, acc, i, lo, m0);  // more neighbours than the list keeps: exact fallback
     }
     op.end(acc, i, lo, hi, s);
+    return act_of<Op>::quiet(acc);
 }
 
+// ---- chunk activity: the DFSPH sweeps skip what they would recompute unchanged ----------------------------------------------
+// A chunk is the 32 particles [32k, 32k + 32) of the sorted fluid set: warp k of a list sweep launched over all nF (iBegin = 0),
+// with the default or the patch mapping alike.  chunkAct[k] is the ballot of the chunk's particles whose record scalar may be
+// non-zero: a lane counts as quiet only when it is in the sweep's range and its error sweep left e = +0, kappa = -0
+// (OpDfsphError::finish), or k_s_copy wrote exactly -0 -- ghosts of a slab rank and lanes past nF are always active.
+// Reach: every list entry of a particle of tile T (and every cell of its exact cell-walk fallback) is a boundary record, whose
+// scalar is 0, or lies in one of T's nine fluid windows (tile_window: the cells [cA + off - 1, cB + off + 1] around the tile's
+// cells [cA, cB]).  The list builder keeps those windows in tileWin; a tile with a particle outside the grid is unbounded.
+// true when every chunk the fluid windows of `tile` touch has chunkAct == 0 (kStamp false) / a stamp <= s.seq (kStamp true)
+template <bool kStamp>
+__device__ __forceinline__ bool reach_quiet(const DevScene& s, int tile) {
+    const int lane = threadIdx.x & 31;
+    const int2* w = s.tileWin + static_cast<size_t>(tile) * SPHK_TILE_WINS;
+    bool ok = true;
+#pragma unroll 1
+    for (int r = 0; r < 9; ++r) {
+        const int2 wr = w[r];
+        if (wr.y < 0) return false;                   // warp-uniform: one tile per warp
+        if (wr.y == 0) continue;
+        for (int k = (wr.x >> 5) + lane; k <= (wr.x + wr.y - 1) >> 5; k += 32)
+            ok = ok && (kStamp ? s.stamp[k] <= s.seq : s.act[k] == 0u);
+    }
+    return __all_sync(0xffffffffu, ok);
+}
+
+// one warp = one chunk of a DFSPH error or correct sweep that keeps chunk activity
 template <class Op>
-__global__ void __launch_bounds__(SPHK_BLOCK) k_sweep_list(const DevScene s, const Op op) {
-    if (s.pred && *s.pred == 0) return;
+__device__ __forceinline__ void sweep_list_warp(const DevScene& s, const Op& op, int i) {
+    const int lane = threadIdx.x & 31, chunk = i >> 5;
+    if (i - lane >= s.nF) return;                     // a whole warp past the set (patch mapping rounds the grid up)
+    const bool in = in_range(s, i);
+    if (act_of<Op>::role == kActError) {
+        // Reuse (s.reuse: the host's token -- the previous error sweep was of this kind with the same arrays, dt and rho0, and
+        // since then no launch changed positions, densities, alpha, rec.s or these outputs, only correct sweeps moved velocities).
+        // The outputs of this chunk's particles depend on their own velocity and those of their reach, nothing else that moved:
+        // when no chunk of the reach was stamped since that sweep, they are what it wrote.  Own kappa quiet is required as well:
+        // the density error's warm accumulate (warm += kappa) must be a no-op for a skip to be exact -- a particle with
+        // kappa != 0 whose velocities did not change still accumulates.
+        if (s.reuse && s.act[chunk] == 0u && reach_quiet<true>(s, i / SPHK_BLOCK)) return;
+        bool quiet = false;
+        if (in) quiet = sweep_list_particle(s, op, i);
+        const unsigned int act = __ballot_sync(0xffffffffu, !quiet);
+        if ((threadIdx.x & 31) == 0) s.act[i >> 5] = act;
+    } else {
+        // Every kappa in reach is -0 (boundary records: +0 after feed_pair), so every pair term is mj * (+-0) * (d * f) with a
+        // finite d * f (listed pairs have r^2 <= r2list at unchanged positions): +-0, and the accumulator, starting at +0, stays
+        // +0.  The walk is skipped; the epilogue still runs on the +0 sum, so vel and rec.b get exactly what the walk would
+        // write (v + 0: -0 components become +0).  That write is not stamped: an error sweep cannot tell a +0 velocity
+        // component from a -0 one (its sum starts at +0 and only ever adds terms; a zero term of either sign leaves it unchanged).
+        if (s.act && s.act[chunk] == 0u && reach_quiet<false>(s, i / SPHK_BLOCK)) {
+            if (in) {
+                float4 lo, hi;
+                rec_full(s.rec + i, lo, hi);
+                typename Op::Acc acc;
+                op.begin(acc, i, lo, hi, s);
+                op.end(acc, i, lo, hi, s);
+            }
+            return;
+        }
+        if (lane == 0) s.stamp[chunk] = s.seq;          // (before the walk: nothing of this stays live across it)
+        if (in) sweep_list_particle(s, op, i);
+    }
+}
+
+// the particle (default mapping) or the chunk (patch mapping) of thread t of a list sweep
+__device__ __forceinline__ int list_thread(const DevScene& s) {
     int t = blockIdx.x * SPHK_BLOCK + threadIdx.x;
     if (s.patch > 0) {               // groups of 4 runs of `patch` chunks; block bb of a group: chunk bb of each run, one per warp
         static_assert(SPHK_BLOCK == 128, "four warps per block");
         const int chunk = t >> 5, per = 4 * s.patch, g = chunk / per, r = chunk - g * per;
         t = ((g * per + (r & 3) * s.patch + (r >> 2)) << 5) | (t & 31);
     }
-    const int i = s.iBegin + t;
+    return s.iBegin + t;
+}
+
+template <class Op>
+__global__ void __launch_bounds__(SPHK_BLOCK) k_sweep_list(const DevScene s, const Op op) {
+    if (s.pred && *s.pred == 0) return;
+    const int i = list_thread(s);
     if (!in_range(s, i)) return;
     sweep_list_particle(s, op, i);
+}
+// the DFSPH error and correct sweeps when they keep chunk activity (a kernel of its own: the plain walk keeps its registers)
+template <class Op>
+__global__ void __launch_bounds__(SPHK_BLOCK) k_sweep_list_act(const DevScene s, const Op op) {
+    if (s.pred && *s.pred == 0) return;
+    sweep_list_warp(s, op, list_thread(s));
 }
 
 // =================================================================================================
@@ -992,17 +1089,17 @@ __device__ __forceinline__ void build_range_staged(const float4* smA, int slotOf
 }
 
 __global__ void __launch_bounds__(SPHK_BLOCK)
-k_build_list_staged(const DevScene s, int* __restrict__ nbr, int* __restrict__ cnt, float4* __restrict__ posBuild) {
+k_build_list_staged(const DevScene s, int* __restrict__ nbr, int* __restrict__ cnt, float4* __restrict__ posBuild, int2* __restrict__ tileWin) {
     extern __shared__ float4 smA[];                 // [SPHK_BUILD_CAP + 1 + SPHK_BUILD_OVERREAD]
     __shared__ unsigned long long bar;
-    __shared__ int sMin, sMax;
+    __shared__ int sMin, sMax, sOut;
     __shared__ int2 sWin[SPHK_TILE_WINS];
     __shared__ int sPre[SPHK_TILE_WINS + 1];
     const int tile = s.iBegin / SPHK_BLOCK + blockIdx.x;
     const int i = tile * SPHK_BLOCK + threadIdx.x;
     const bool have = i < s.nF;
     const int ncells = s.cs.x * s.cs.y * s.cs.z;
-    if (threadIdx.x == 0) { sMin = 0x7fffffff; sMax = -1; }
+    if (threadIdx.x == 0) { sMin = 0x7fffffff; sMax = -1; sOut = 0; }
     __syncthreads();
     float4 lo = make_float4(0.f, 0.f, 0.f, 0.f);
     int cx = 0, cy = 0, cz = 0, c = ncells;
@@ -1011,9 +1108,16 @@ k_build_list_staged(const DevScene s, int* __restrict__ nbr, int* __restrict__ c
         cx = cell_coord(lo.x, s.cellLength) - s.org.x; cy = cell_coord(lo.y, s.cellLength) - s.org.y; cz = cell_coord(lo.z, s.cellLength) - s.org.z;
         c = cell_index(cx, cy, cz, s.cs);
         if (c < ncells) { atomicMin(&sMin, c); atomicMax(&sMax, c); }
+        else sOut = 1;
     }
     __syncthreads();
-    if (threadIdx.x < SPHK_TILE_WINS) sWin[threadIdx.x] = tile_window(s, threadIdx.x, sMin, sMax, ncells);
+    if (threadIdx.x < SPHK_TILE_WINS) {
+        const int2 w = tile_window(s, threadIdx.x, sMin, sMax, ncells);
+        sWin[threadIdx.x] = w;
+        // the fluid windows are the reach of the tile's sweeps (chunk activity, sweep_list_warp); a particle outside the grid
+        // may reach past them: count -1 marks such a tile as unbounded
+        if (threadIdx.x < 9) tileWin[static_cast<size_t>(tile) * SPHK_TILE_WINS + threadIdx.x] = (sOut && threadIdx.x == 0) ? make_int2(0, -1) : w;
+    }
     __syncthreads();
     if (threadIdx.x == 0) tile_stage(s, sWin, sPre, smA, nullptr, false, &bar, SPHK_BUILD_CAP);
     __syncthreads();
@@ -1249,9 +1353,13 @@ __global__ void __launch_bounds__(SPHK_BLOCK) k_s_cg2(const float* __restrict__ 
     const float3 c = load3(cg, i);
     rec_set_s(rec + i, dot3(c, c));
 }
-__global__ void __launch_bounds__(SPHK_BLOCK) k_s_copy(const float* __restrict__ a, Rec rec, int n) {
+// (+ the chunk activity of the copied scalar: -0 is quiet, sweep_list_warp)
+__global__ void __launch_bounds__(SPHK_BLOCK) k_s_copy(const float* __restrict__ a, Rec rec, int n, unsigned int* __restrict__ act) {
     const int i = blockIdx.x * SPHK_BLOCK + threadIdx.x;
-    if (i < n) rec_set_s(rec + i, a[i]);
+    float v = 0.f;
+    if (i < n) { v = a[i]; rec_set_s(rec + i, v); }
+    const unsigned int b = __ballot_sync(0xffffffffu, !(i < n && __float_as_uint(v) == 0x80000000u));
+    if ((threadIdx.x & 31) == 0 && i < n) act[i >> 5] = b;
 }
 
 // Particles::advect (Particles.cu:28-36) + enforceBoundary_CUDA(pos, vel) (BasicSPHSolver.cu:85-96)
@@ -1359,8 +1467,17 @@ static DevScene dev_scene(const sphk_ctx* c, const sphk_scene* s) {
     d.k = kernel_constants(s->radius);
     d.r2list = d.k.r2cut;
     d.cellFlag = nullptr;
+    d.act = nullptr; d.stamp = nullptr; d.seq = 0; d.reuse = 0;
     return d;
 }
+
+// Chunk activity on the host (sweep_list_warp).  Every launch counts in c->launches; the launches known to leave rec.s and all
+// an error sweep reads alone -- except velocities moved under chunk stamps by the correct sweeps -- also count in c->credited
+// (correct sweeps, loop control, reductions).  So act_mark() stays put across exactly those: the chunk bits stay valid, and the
+// last error sweep's outputs stay reusable, until anything else is launched.  Host-side only: a captured step repeats the order
+// of its calls and with it these decisions; what depends on data (which chunks are quiet) is decided on the device.
+static long long act_mark(const sphk_ctx* c) { return c->launches - c->credited; }
+static bool same_bits(float a, float b) { unsigned int x, y; std::memcpy(&x, &a, 4); std::memcpy(&y, &b, 4); return x == y; }
 
 SkinTrack sphk_skin_track(const sphk_ctx* c, float radius, bool on) {
     SkinTrack t;
@@ -1384,6 +1501,7 @@ static int ensure_list(sphk_ctx* c, const DevScene& d) {
     b.nbr = c->nbr;
     b.rangeDev = nullptr;
     c->listBegin = d.iBegin; c->listEnd = d.iEnd;
+    c->listSpans = false;
     c->listHasSkin = c->skin > 0.f;
     if (c->listHasSkin) {
         const float rs = d.k.R * (1.0f + c->skin);
@@ -1409,7 +1527,8 @@ static int ensure_list(sphk_ctx* c, const DevScene& d) {
         const int smem = (SPHK_BUILD_CAP + 1 + SPHK_BUILD_OVERREAD) * 16;
         if (!attr) { cudaFuncSetAttribute(k_build_list_staged, cudaFuncAttributeMaxDynamicSharedMemorySize, smem); attr = true; }
         const int tiles = (b.iEnd + SPHK_BLOCK - 1) / SPHK_BLOCK - b.iBegin / SPHK_BLOCK;
-        k_build_list_staged<<<tiles, SPHK_BLOCK, smem, c->stream>>>(b, c->nbr, c->cnt, nullptr);
+        k_build_list_staged<<<tiles, SPHK_BLOCK, smem, c->stream>>>(b, c->nbr, c->cnt, nullptr, c->tileWin);
+        c->listSpans = b.iBegin == 0 && b.iEnd == c->nF;
     } else {
         k_build_list<<<sphk_blocks(b.iEnd - b.iBegin), SPHK_BLOCK, 0, c->stream>>>(b, c->nbr, c->cnt, nullptr);
     }
@@ -1418,8 +1537,12 @@ static int ensure_list(sphk_ctx* c, const DevScene& d) {
     return SPHK_OK;
 }
 
-template <class Op> static int run_sweep(sphk_ctx* c, const sphk_scene* s, const Op& op) {
+// kept (DFSPH error and correct sweeps): the launch kept chunk activity -- a list sweep over every chunk whose list builder recorded
+// the tiles' windows.  reuse (error sweeps): the token matches, chunks quiet since it may keep their outputs.
+template <class Op> static int run_sweep(sphk_ctx* c, const sphk_scene* s, const Op& op, bool* kept = nullptr, bool reuse = false) {
+    constexpr int role = act_of<Op>::role;
     DevScene d = dev_scene(c, s);
+    if (kept) *kept = false;
     if (d.iEnd <= d.iBegin) return SPHK_OK;
     // the list is usable while positions are those of the search, or -- skin lists -- while the particles have
     // only been moved by sphk_pbd_delta_pos_apply (displacement tracked on the device against skin/2)
@@ -1437,23 +1560,57 @@ template <class Op> static int run_sweep(sphk_ctx* c, const sphk_scene* s, const
             k_sweep_tile<Op><<<tiles, SPHK_BLOCK, smem, c->stream>>>(d, op);
         }
         else {
+            if (role != kActNone && c->listSpans && d.iBegin == 0 && d.iEnd == c->nF) {
+                if (kept) *kept = true;
+                if (role == kActError) {
+                    d.act = c->chunkAct;
+                    if (reuse) { d.reuse = 1; d.stamp = c->chunkStamp; d.seq = c->tok.seq; }
+                } else {
+                    d.stamp = c->chunkStamp;
+                    d.seq = ++c->corrSeq;
+                    if (c->actMark == act_mark(c)) d.act = c->chunkAct;
+                }
+            }
             int blocks = sphk_blocks(d.iEnd - d.iBegin);
             if (d.patch > 0) blocks = (blocks + d.patch - 1) / d.patch * d.patch;      // whole groups (4 * patch chunks = patch blocks)
-            k_sweep_list<Op><<<blocks, SPHK_BLOCK, 0, c->stream>>>(d, op);
+            if (d.act || d.stamp) {
+                if constexpr (role != kActNone) k_sweep_list_act<Op><<<blocks, SPHK_BLOCK, 0, c->stream>>>(d, op);
+            } else {
+                k_sweep_list<Op><<<blocks, SPHK_BLOCK, 0, c->stream>>>(d, op);
+            }
         }
     } else {
         k_sweep_cells<Op><<<sphk_blocks(d.iEnd - d.iBegin), SPHK_BLOCK, 0, c->stream>>>(d, op);
     }
     c->launches++;
+    if (role == kActCorrect) c->credited++;           // velocities only; stamped, or the caller drops the token
     SPHK_CUDA_TRY(cudaGetLastError());
     return SPHK_OK;
+}
+
+// after a DFSPH error sweep (kind 1 divergence -- also the fused sweep --, 2 density): its chunk bits and reuse token
+static void error_swept(sphk_ctx* c, bool kept, int kind, const sphk_scene* s, const float* alpha, const float* error, const float* stiff,
+                        float dt, float rho0) {
+    c->actMark = kept ? act_mark(c) : -1;
+    c->tok.kind = kept ? kind : 0;
+    c->tok.density = s->fluid.density; c->tok.alpha = alpha; c->tok.error = error; c->tok.stiff = stiff;
+    c->tok.dt = dt; c->tok.rho0 = rho0;
+    c->tok.mark = act_mark(c);
+    c->tok.seq = c->corrSeq;
+}
+static bool error_reusable(const sphk_ctx* c, int kind, const sphk_scene* s, const float* alpha, const float* error, const float* stiff,
+                           float dt, float rho0) {
+    const auto& k = c->tok;
+    return k.kind == kind && k.mark == act_mark(c) && c->actMark == k.mark && c->sTag == stiff && k.density == s->fluid.density &&
+           k.alpha == alpha && k.error == error && k.stiff == stiff && same_bits(k.dt, dt) && same_bits(k.rho0, rho0);
 }
 
 // rec.s must mirror `array` before a sweep that gathers it; skipped when the previous sweep wrote both
 static void ensure_scalar(sphk_ctx* c, const float* array) {
     if (c->sTag == array) return;
-    k_s_copy<<<sphk_blocks(c->nF), SPHK_BLOCK, 0, c->stream>>>(array, c->rec, c->nF);
+    k_s_copy<<<sphk_blocks(c->nF), SPHK_BLOCK, 0, c->stream>>>(array, c->rec, c->nF, c->chunkAct);
     c->launches++;
+    c->actMark = act_mark(c);
     c->sTag = array;
 }
 
@@ -1566,7 +1723,9 @@ extern "C" int sphk_dfsph_div_error(sphk_ctx* c, const sphk_scene* s, const floa
     SPHK_CHECK_SCENE(c, s);
     if (!alpha || !error || !stiff || !s->fluid.density) return SPHK_ERR_INVALID;
     OpDfsphError<false> op{c->rec, s->fluid.density, alpha, error, stiff, nullptr, dt, rho0};
-    const int rc = run_sweep(c, s, op);
+    bool kept;
+    const int rc = run_sweep(c, s, op, &kept, error_reusable(c, 1, s, alpha, error, stiff, dt, rho0));
+    error_swept(c, kept, 1, s, alpha, error, stiff, dt, rho0);
     c->sTag = stiff;
     return rc;
 }
@@ -1577,7 +1736,9 @@ extern "C" int sphk_dfsph_den_error(sphk_ctx* c, const sphk_scene* s, const floa
     if (!alpha || !error || !stiff || !s->fluid.density) return SPHK_ERR_INVALID;
     if (warm == c->sTag) c->sTag = nullptr;
     OpDfsphError<true> op{c->rec, s->fluid.density, alpha, error, stiff, warm, dt, rho0};
-    const int rc = run_sweep(c, s, op);
+    bool kept;
+    const int rc = run_sweep(c, s, op, &kept, error_reusable(c, 2, s, alpha, error, stiff, dt, rho0));
+    error_swept(c, kept, 2, s, alpha, error, stiff, dt, rho0);
     c->sTag = stiff;
     return rc;
 }
@@ -1587,7 +1748,10 @@ extern "C" int sphk_dfsph_div_correct(sphk_ctx* c, const sphk_scene* s, const fl
     if (!stiff) return SPHK_ERR_INVALID;
     ensure_scalar(c, stiff);
     OpScalarGradient<0> op{c->rec, s->fluid.vel, nullptr, 1.0f};
-    return run_sweep(c, s, op);
+    bool kept;
+    const int rc = run_sweep(c, s, op, &kept);
+    if (!kept) c->tok.kind = 0;                       // velocities moved without stamps
+    return rc;
 }
 
 extern "C" int sphk_dfsph_den_correct(sphk_ctx* c, const sphk_scene* s, const float* stiff, float dt) {
@@ -1595,7 +1759,10 @@ extern "C" int sphk_dfsph_den_correct(sphk_ctx* c, const sphk_scene* s, const fl
     if (!stiff) return SPHK_ERR_INVALID;
     ensure_scalar(c, stiff);
     OpScalarGradient<1> op{c->rec, s->fluid.vel, nullptr, dt};
-    return run_sweep(c, s, op);
+    bool kept;
+    const int rc = run_sweep(c, s, op, &kept);
+    if (!kept) c->tok.kind = 0;                       // velocities moved without stamps
+    return rc;
 }
 
 extern "C" int sphk_pbd_density_lambda(sphk_ctx* c, const sphk_scene* s, float* lambda, float rho0, float relaxation) {
@@ -1832,14 +1999,18 @@ extern "C" int sphk_fused_dfsph_density_alpha_div_error(sphk_ctx* c, const sphk_
     if (!alpha || !error || !stiff || !s->fluid.density) return SPHK_ERR_INVALID;
     const OpDfsphError<false> err{c->rec, s->fluid.density, alpha, error, stiff, nullptr, dt, rho0};
     int rc;
+    bool kept;
     if (color_grad_or_null) {
         OpDensityAlphaDivError<true> op{{OpPair<OpDensityAlpha, OpColorGrad>{OpDensityAlpha{s->fluid.density, alpha},
                                                                              OpColorGrad{color_grad_or_null, rho0, rhoB}}, err}};
-        rc = run_sweep(c, s, op);
+        rc = run_sweep(c, s, op, &kept);
     } else {
         OpDensityAlphaDivError<false> op{{OpDensityAlpha{s->fluid.density, alpha}, err}};
-        rc = run_sweep(c, s, op);
+        rc = run_sweep(c, s, op, &kept);
     }
+    // never reused (it forms density and alpha), but a divergence error for the sweeps after it: the same pair terms in the same
+    // order, and the epilogue takes the density and alpha it stores
+    error_swept(c, kept, 1, s, alpha, error, stiff, dt, rho0);
     c->sTag = stiff;
     return rc;
 }
