@@ -13,6 +13,13 @@
 //                [--cfl C [--dt-min X]] [--rheology cross:NU0,NUINF,LAMBDA,M | hb:K,N,TAU[,MREG] [--rheology-max NU_MAX] [--no-slip]]
 //                [--heat ALPHA,BETA[,TREF] [--heater T] [--wall-temp T[,H]] [--tap-temp T] [--thermal-viscosity NUREF,E[,NUMAX]]]
 //                [--adhesion BETA[,BODYBETA]] [--obstacle FILE[,S,X,Y,Z]]... [--mesh-body FILE,REL[,S,X,Y,Z]] [--fluid-mesh FILE[,S,X,Y,Z]]
+//                [--probe X,Y,Z]... [--gauge AX,AY,AZ,BX,BY,BZ[,K]]... [--gauge-threshold THETA] [--probe-out FILE]
+// --probe and --gauge (repeatable; DESIGN.md section 2.13) record SPH-interpolated fields at points and water levels along segments
+// every step after the constructor's step 0 (SPHSystem::setProbes): a gauge runs from A to B with K samples (default 64), its
+// level is its height above A (orient it upwards, along -G, from the floor), wet where the Shepard sum reaches THETA (default 0.5).
+// --probe-out FILE (required with them) gets a CSV row per step: step,t, then each probe's S,rho,vx,vy,vz,p,T,n, then each gauge's
+// level (-1: dry).  The device ring is drained after every frame (sized for a frame's largest substep count with --cfl).  At most
+// 4096 probes and 64 gauges; single GPU only.
 // --obstacle, --mesh-body and --fluid-mesh build the scene from Wavefront OBJ meshes (sphb200::loadObj, DESIGN.md section 2.12), each
 // mapped by S * v + (X, Y, Z) (default 1 and 0).  --obstacle (repeatable) is a static obstacle: its surface sampled at the boundary
 // spacing (sphb200::sampleSurface) is appended to the boundary set after the tank shell, so it has the walls' adhesion and
@@ -130,6 +137,8 @@ struct Options {
     std::string rendezvous;
     std::vector<std::string> obstacles;       // --obstacle FILE[,S,X,Y,Z] (repeatable)
     std::string meshBody, fluidMesh;          // --mesh-body FILE,REL[,S,X,Y,Z], --fluid-mesh FILE[,S,X,Y,Z]
+    std::vector<std::string> probes, gauges;  // --probe X,Y,Z and --gauge AX,AY,AZ,BX,BY,BZ[,K] (repeatable)
+    std::string gaugeThreshold, probeOut;     // --gauge-threshold THETA, --probe-out FILE
 };
 
 // --rheology MODEL:a,b,c[,d] -> the model (not yet checked against its ranges: setRheology does that)
@@ -234,6 +243,37 @@ bool adhesion_of(const Options& o, bool hasBody, sphb200::Adhesion& a) {
     return true;
 }
 
+// --probe, --gauge and --gauge-threshold -> the setting (capacity: the caller's); false for malformed or out-of-range values
+bool probes_of(const Options& o, sphb200::Probes& p) {
+    p = sphb200::Probes();
+    for (const auto& spec : o.probes) {
+        std::vector<float> v;
+        if (!floats_of(spec, v) || v.size() != 3) return false;
+        for (float x : v) if (!std::isfinite(x)) return false;
+        p.points.push_back(make_float3(v[0], v[1], v[2]));
+    }
+    for (const auto& spec : o.gauges) {
+        std::vector<float> v;
+        if (!floats_of(spec, v) || (v.size() != 6 && v.size() != 7)) return false;
+        for (float x : v) if (!std::isfinite(x)) return false;
+        sphb200::Gauge g;
+        g.a = make_float3(v[0], v[1], v[2]);
+        g.b = make_float3(v[3], v[4], v[5]);
+        if (v.size() == 7) {
+            if (v[6] != std::floor(v[6]) || v[6] < 2.0f || v[6] > SPHK_GAUGE_MAX_SAMPLES) return false;
+            g.samples = static_cast<int>(v[6]);
+        }
+        if (g.a.x == g.b.x && g.a.y == g.b.y && g.a.z == g.b.z) return false;
+        p.gauges.push_back(g);
+    }
+    if (!o.gaugeThreshold.empty()) {
+        std::vector<float> v;
+        if (!floats_of(o.gaugeThreshold, v) || v.size() != 1 || !std::isfinite(v[0]) || !(v[0] > 0.0f)) return false;
+        p.threshold = v[0];
+    }
+    return p.points.size() <= SPHK_PROBE_LIMIT && p.gauges.size() <= SPHK_GAUGE_LIMIT;
+}
+
 // --heat and its companions -> the thermal setting and the viscosity law (ranges are checked by the setters)
 bool thermal_of(const Options& o, sphb200::Thermal& t, sphb200::ThermalViscosity& tv) {
     std::vector<float> v;
@@ -297,6 +337,10 @@ bool parse(int argc, char** argv, Options& o) {
         else if (a == "--obstacle" && need(i, 1)) o.obstacles.push_back(argv[++i]);
         else if (a == "--mesh-body" && need(i, 1)) o.meshBody = argv[++i];
         else if (a == "--fluid-mesh" && need(i, 1)) o.fluidMesh = argv[++i];
+        else if (a == "--probe" && need(i, 1)) o.probes.push_back(argv[++i]);
+        else if (a == "--gauge" && need(i, 1)) o.gauges.push_back(argv[++i]);
+        else if (a == "--gauge-threshold" && need(i, 1)) o.gaugeThreshold = argv[++i];
+        else if (a == "--probe-out" && need(i, 1)) o.probeOut = argv[++i];
         else if (a == "--block" && need(i, 3)) { for (int k = 0; k < 3; ++k) o.block[k] = std::atoi(argv[++i]); }
         else if (a == "--origin" && need(i, 3)) { for (int k = 0; k < 3; ++k) o.origin[k] = static_cast<float>(std::atof(argv[++i])); }
         else if (a == "--box" && need(i, 1)) {
@@ -392,6 +436,17 @@ bool parse(int argc, char** argv, Options& o) {
     if ((!o.obstacles.empty() || !o.meshBody.empty() || !o.fluidMesh.empty()) && o.ranks > 1) {
         std::fprintf(stderr, "sph_headless: --obstacle, --mesh-body and --fluid-mesh run on one GPU only (not with --ranks)\n");
         return false;
+    }
+    if (!o.probes.empty() || !o.gauges.empty() || !o.gaugeThreshold.empty() || !o.probeOut.empty()) {
+        sphb200::Probes p;
+        if (!probes_of(o, p) || o.ranks > 1 || o.probeOut.empty() || (p.points.empty() && p.gauges.empty()) ||
+            (!o.gaugeThreshold.empty() && p.gauges.empty())) {
+            std::fprintf(stderr, "sph_headless: --probe X,Y,Z and --gauge AX,AY,AZ,BX,BY,BZ[,K] need finite values, a != b and K in [2, %d] "
+                                 "(at most %d probes and %d gauges), --gauge-threshold a finite value > 0 and gauges, --probe-out a file "
+                                 "and at least one probe or gauge; single GPU only (not with --ranks)\n",
+                         SPHK_GAUGE_MAX_SAMPLES, SPHK_PROBE_LIMIT, SPHK_GAUGE_LIMIT);
+            return false;
+        }
     }
     if (!o.meshBody.empty() && (o.stir || o.floating || !o.heater.empty())) {
         std::fprintf(stderr, "sph_headless: --mesh-body not together with --stir, --float or --heater\n");
@@ -782,6 +837,38 @@ int main(int argc, char** argv) {
         std::fprintf(stderr, "sph_headless: --cfl %g --dt-min %g was refused\n", o.cfl, o.dtMin);
         return 4;
     }
+    std::FILE* probeCsv = nullptr;
+    long long probeLastStep = 0;              // the last step written (the constructor's step 0 is not recorded)
+    if (!o.probeOut.empty()) {
+        sphb200::Probes p;
+        probes_of(o, p);
+        // one frame is one step, or with --cfl at most ceil(dt / dt_min) substeps plus the two shortened ones at its end
+        const double dtMin = o.dtMin > 0.0f ? o.dtMin : dt / 64.0;
+        p.capacity = o.cfl > 0.0f ? static_cast<int>(std::min(65536.0, std::ceil(dt / dtMin) + 2.0)) : 1;
+        if (!pSystem->setProbes(p)) { std::fprintf(stderr, "sph_headless: --probe / --gauge were refused\n"); return 4; }
+        probeCsv = std::fopen(o.probeOut.c_str(), "w");
+        if (!probeCsv) { std::fprintf(stderr, "sph_headless: cannot write --probe-out %s\n", o.probeOut.c_str()); return 5; }
+        static const char* kFields[SPHK_PROBE_FIELDS] = {"S", "rho", "vx", "vy", "vz", "p", "T", "n"};
+        std::fprintf(probeCsv, "step,t");
+        for (size_t k = 0; k < p.points.size(); ++k)
+            for (const char* f : kFields) std::fprintf(probeCsv, ",p%zu_%s", k, f);
+        for (size_t k = 0; k < p.gauges.size(); ++k) std::fprintf(probeCsv, ",g%zu_level", k);
+        std::fprintf(probeCsv, "\n");
+    }
+    // the rows recorded since the last drain, one CSV line per step (floats with 9 significant digits: the float32 bits round-trip)
+    auto drainProbes = [&]() {
+        if (!probeCsv) return;
+        const sphb200::ProbeSeries ps = pSystem->probeSeries();
+        const size_t nr = static_cast<size_t>(ps.probes) * SPHK_PROBE_FIELDS, ng = static_cast<size_t>(ps.gauges);
+        for (size_t r = 0; r < ps.steps.size(); ++r) {
+            if (ps.steps[r] <= probeLastStep) continue;
+            std::fprintf(probeCsv, "%lld,%.17g", ps.steps[r], ps.times[r]);
+            for (size_t k = 0; k < nr; ++k) std::fprintf(probeCsv, ",%.9g", ps.records[r * nr + k]);
+            for (size_t k = 0; k < ng; ++k) std::fprintf(probeCsv, ",%.9g", ps.levels[r * ng + k]);
+            std::fprintf(probeCsv, "\n");
+            probeLastStep = ps.steps[r];
+        }
+    };
 
     if (o.bullets > 0) {
         const int hit = slab ? shoot(o, sphSpacing, dt, pSlab->getFluids(), static_cast<size_t>(pSlab->ownedBegin()), static_cast<size_t>(pSlab->size()))
@@ -817,6 +904,7 @@ int main(int argc, char** argv) {
             _exit(4);
         }
         if (slab && o.bullets > 0) straysRouted += pSlab->straysRouted();
+        drainProbes();
         totalTime += milliseconds;
         worst = milliseconds > worst ? milliseconds : worst;
         if (!o.quiet && !o.heat.empty()) {
@@ -839,6 +927,7 @@ int main(int argc, char** argv) {
                         totalTime / float(frameId), float(frameId) * 1000.0f / totalTime);
     }
     if (!o.quiet) std::printf("\n");
+    if (probeCsv && std::fclose(probeCsv) != 0) { std::fprintf(stderr, "sph_headless: writing --probe-out %s failed\n", o.probeOut.c_str()); return 5; }
 
     // ---- optional dump through the public accessors + the render hook (vbo.cu:46-51) ----
     if (!o.dump.empty() && slab) {

@@ -42,7 +42,8 @@ SPHK_FUNCTIONS = [
     "sphk_heat_substeps", "sphk_heat_step", "sphk_heat_conduction", "sphk_heat_stats", "sphk_thermal_viscosity",
     "sphk_thermal_viscosity_eval", "sphk_adhesion", "sphk_adhesion_accel", "sphk_adhesion_stats",
     "sphk_mesh_transform", "sphk_mesh_properties", "sphk_mesh_create", "sphk_mesh_destroy", "sphk_mesh_classify", "sphk_mesh_fill",
-    "sphk_mesh_sample_surface",
+    "sphk_mesh_sample_surface", "sphk_probe_sample", "sphk_probe_lattice", "sphk_gauge_levels", "sphk_probe_series_create",
+    "sphk_probe_series_destroy", "sphk_probes_record", "sphk_probe_series_read",
 ]
 SPH_APP_FUNCTIONS = [
     "sph_app_create", "sph_app_destroy", "sph_app_step", "sph_app_fluid_size", "sph_app_boundary_size",
@@ -54,9 +55,15 @@ SPH_APP_FUNCTIONS = [
     "sph_app_adaptive_stats", "sph_app_set_rheology", "sph_app_rheology_stats", "sph_app_download_viscosity",
     "sph_app_set_thermal", "sph_app_set_thermal_viscosity", "sph_app_upload_temperature", "sph_app_download_temperature",
     "sph_app_thermal_stats", "sph_app_set_adhesion", "sph_app_adhesion_stats", "sph_app_load_obj", "sph_app_load_obj_error",
+    "sph_app_set_probes", "sph_app_probe_series", "sph_app_sample_probes", "sph_app_sample_lattice",
 ]
 
 BODY_LIMIT = 64                      # SPHK_BODY_LIMIT
+PROBE_FIELDS = 8                     # SPHK_PROBE_FIELDS: S, rho, vx, vy, vz, p, T, n
+PROBE_LIMIT = 4096                   # SPHK_PROBE_LIMIT
+GAUGE_LIMIT = 64                     # SPHK_GAUGE_LIMIT
+GAUGE_MAX_SAMPLES = 1024             # SPHK_GAUGE_MAX_SAMPLES
+PROBE_CAPACITY_LIMIT = 65536         # SPHK_PROBE_CAPACITY_LIMIT
 THERMAL_GROUPS = 1 + BODY_LIMIT      # SPHK_THERMAL_GROUPS
 
 
@@ -207,6 +214,35 @@ class SphkTimeStepRule(C.Structure):
     _fields_ = [("cfl", C.c_double), ("dt_min", C.c_double), ("dt_max", C.c_double), ("radius", C.c_double), ("gravity", C.c_double)]
 
 
+class SphkGauge(C.Structure):
+    """sphk_gauge of sphk.h"""
+    _fields_ = [("a", C.c_float * 3), ("b", C.c_float * 3), ("samples", C.c_int)]
+
+
+def probe_points(points) -> np.ndarray:
+    """(P, 3) float32 probe points; ValueError for a wrong shape, non-finite values or more than PROBE_LIMIT"""
+    p = np.ascontiguousarray(np.asarray(points, np.float32).reshape(-1, 3))
+    if p.shape[0] > PROBE_LIMIT or not np.isfinite(p).all():
+        raise ValueError(f"probes need finite (x, y, z) points, at most {PROBE_LIMIT}")
+    return p
+
+
+def gauge_structs(specs, threshold: float):
+    """sphk_gauge[] from (a, b) or (a, b, k) tuples (k default 64); ValueError for a == b, k outside [2, GAUGE_MAX_SAMPLES],
+    non-finite values, more than GAUGE_LIMIT gauges or a threshold that is not finite and > 0"""
+    specs = list(specs)
+    if len(specs) > GAUGE_LIMIT or not (np.isfinite(threshold) and threshold > 0):
+        raise ValueError(f"at most {GAUGE_LIMIT} gauges and a finite threshold > 0")
+    out = (SphkGauge * max(1, len(specs)))()
+    for g, spec in zip(out, specs):
+        a, b = np.asarray(spec[0], np.float32).reshape(3), np.asarray(spec[1], np.float32).reshape(3)
+        k = int(spec[2]) if len(spec) > 2 else 64
+        if not (np.isfinite(a).all() and np.isfinite(b).all()) or (a == b).all() or not 2 <= k <= GAUGE_MAX_SAMPLES:
+            raise ValueError(f"a gauge needs finite a != b and 2 <= k <= {GAUGE_MAX_SAMPLES}: {spec}")
+        g.a[:], g.b[:], g.samples = [float(x) for x in a], [float(x) for x in b], k
+    return out, len(specs)
+
+
 class SphkGrid(C.Structure):
     _fields_ = [("cell_size", C.c_int * 3), ("cell_length", C.c_float), ("origin", C.c_int * 3)]
 
@@ -256,6 +292,7 @@ def sphk():
         L.sphk_destroy.restype = None
         L.sphk_mg_destroy.restype = None
         L.sphk_mesh_destroy.restype = None
+        L.sphk_probe_series_destroy.restype = None
         _sphk = L
     return _sphk
 
@@ -523,6 +560,48 @@ class SphApp:
         if self.L.sph_app_adhesion_stats(self.h, C.byref(w), C.byref(am)):
             raise RuntimeError("sph_app_adhesion_stats failed (reference engine)")
         return {"wetted": w.value, "max_accel": am.value}
+
+    def set_probes(self, points=(), gauges=(), threshold: float = 0.5, capacity: int = 1024):
+        """Probes and water-level gauges recorded every following step (SPHSystem::setProbes; DESIGN.md section 2.13).  points: (P, 3);
+        gauges: (a, b) or (a, b, k) tuples; no points and no gauges: off.  Not on the reference engine."""
+        pts = probe_points(points)
+        gs, ng = gauge_structs(gauges, threshold)
+        ab = np.ascontiguousarray([[*g.a, *g.b] for g in gs[:ng]], np.float32).reshape(-1)
+        k = np.ascontiguousarray([g.samples for g in gs[:ng]], np.int32)
+        if self.L.sph_app_set_probes(self.h, C.c_int(pts.shape[0]), pts.ctypes.data_as(C.c_void_p), C.c_int(ng),
+                                     ab.ctypes.data_as(C.c_void_p), k.ctypes.data_as(C.c_void_p), C.c_float(threshold), C.c_int(capacity)):
+            raise RuntimeError("sph_app_set_probes failed (reference engine or a refused setting)")
+
+    def probe_series(self) -> dict:
+        """the recorded rows still in the ring, oldest first: steps (T,), times (T,), records (T, P, 8), levels (T, G), overwritten"""
+        rows, npt, ng, over = C.c_int(0), C.c_int(0), C.c_int(0), C.c_longlong(0)
+        if self.L.sph_app_probe_series(self.h, C.byref(rows), C.byref(npt), C.byref(ng), C.byref(over), None, None, None, None):
+            raise RuntimeError("sph_app_probe_series failed (reference engine)")
+        T, P, G = rows.value, npt.value, ng.value
+        out = {"steps": np.zeros(T, np.int64), "times": np.zeros(T, np.float64), "records": np.zeros((T, P, PROBE_FIELDS), np.float32),
+               "levels": np.zeros((T, G), np.float32), "overwritten": int(over.value)}
+        if self.L.sph_app_probe_series(self.h, None, None, None, None, *[out[k].ctypes.data_as(C.c_void_p)
+                                                                         for k in ("steps", "times", "records", "levels")]):
+            raise RuntimeError("sph_app_probe_series failed")
+        return out
+
+    def sample_probes(self, points) -> np.ndarray:
+        """records (P, 8) of the given points in the current state"""
+        pts = np.ascontiguousarray(np.asarray(points, np.float32).reshape(-1, 3))
+        out = np.zeros((pts.shape[0], PROBE_FIELDS), np.float32)
+        if self.L.sph_app_sample_probes(self.h, C.c_int(pts.shape[0]), pts.ctypes.data_as(C.c_void_p), out.ctypes.data_as(C.c_void_p)):
+            raise RuntimeError("sph_app_sample_probes failed (reference engine or a refused call)")
+        return out
+
+    def sample_lattice(self, origin, spacing: float, dims) -> np.ndarray:
+        """records (nx, ny, nz, 8) of the lattice origin + spacing (i, j, k) in the current state"""
+        o = np.ascontiguousarray(origin, np.float32)
+        d = np.ascontiguousarray([int(x) for x in dims], np.int32)
+        out = np.zeros((*[int(x) for x in d], PROBE_FIELDS), np.float32)
+        if self.L.sph_app_sample_lattice(self.h, o.ctypes.data_as(C.c_void_p), C.c_float(spacing), d.ctypes.data_as(C.c_void_p),
+                                         out.ctypes.data_as(C.c_void_p)):
+            raise RuntimeError("sph_app_sample_lattice failed (reference engine or a refused call)")
+        return out
 
     def thermal_stats(self) -> dict:
         """substeps, max_courant, violators of the last step; t_min, t_max, heat (sum m T) now"""

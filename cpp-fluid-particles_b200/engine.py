@@ -94,6 +94,9 @@ class SphkOps:
     implicit_max_iter = 20
     _step_dt = None                  # the dt of the step in flight (None: the scene's dt); CFL-adaptive systems set it per step
     pbd_last_dt = None               # PBD: the dt of the last predict (the interval the next projection acts on)
+    _probe_series = None             # sphk_probe_series of set_probes (None: off)
+    _probe_recorded = False          # the step in flight recorded a row
+    steps_run = 0                    # steps run so far (the constructor's step is step 0)
 
     @property
     def dt(self) -> float:
@@ -560,6 +563,37 @@ class SphkOps:
         check(self.L.sphk_adhesion_stats(self.ctx, C.byref(w), C.byref(am)), "sphk_adhesion_stats")
         return {"wetted": w.value, "max_accel": am.value}
 
+    # ---- probes and water-level gauges (no reference counterpart; DESIGN.md section 2.13) ----------------------------------
+    def _probe_sources(self):
+        """the pressure of a WCSPH step (DFSPH and PBD keep none) and the temperatures while heat transfer is on, as pointers"""
+        p = _ptr(self.fluid.pressure) if self.solver not in ("dfsph", "pbd") else None
+        t = _ptr(self.temperature) if self._thermal is not None else None
+        return p, t
+
+    def probe_sample(self, points: torch.Tensor, out: torch.Tensor | None = None) -> torch.Tensor:
+        """records (P, 8) {S, rho, vx, vy, vz, p, T, n} of the device points (P, 3) in the current state (sphk_probe_sample)"""
+        points = points.contiguous()
+        out = torch.empty((points.shape[0], capi.PROBE_FIELDS), dtype=torch.float32, device=self.device) if out is None else out
+        check(self.L.sphk_probe_sample(self.ctx, self._s(), _ptr(points), C.c_int(points.shape[0]), *self._probe_sources(), _ptr(out)),
+              "sphk_probe_sample")
+        return out
+
+    def probe_lattice(self, origin, spacing: float, dims, out: torch.Tensor | None = None) -> torch.Tensor:
+        """records (nx, ny, nz, 8) of the lattice origin + spacing (i, j, k), z fastest (sphk_probe_lattice)"""
+        d = [int(x) for x in dims]
+        out = torch.empty((*d, capi.PROBE_FIELDS), dtype=torch.float32, device=self.device) if out is None else out
+        o = (C.c_float * 3)(*[float(x) for x in origin])
+        check(self.L.sphk_probe_lattice(self.ctx, self._s(), o, C.c_float(spacing), (C.c_int * 3)(*d), *self._probe_sources(), _ptr(out)),
+              "sphk_probe_lattice")
+        return out
+
+    def gauge_levels(self, gauges, threshold: float = 0.5, out: torch.Tensor | None = None) -> torch.Tensor:
+        """levels (G,) of (a, b[, k]) gauges in the current state (sphk_gauge_levels)"""
+        gs, ng = capi.gauge_structs(gauges, threshold)
+        out = torch.empty(ng, dtype=torch.float32, device=self.device) if out is None else out
+        check(self.L.sphk_gauge_levels(self.ctx, self._s(), gs, C.c_int(ng), C.c_float(threshold), _ptr(out)), "sphk_gauge_levels")
+        return out
+
     def thermal_viscosity_eval(self, spec, t_ref, temperature, nu_out):
         law = capi.viscosity_law(spec, t_ref)
         check(self.L.sphk_thermal_viscosity_eval(self.ctx, C.byref(law), _ptr(temperature), _ptr(nu_out), C.c_int(temperature.numel())),
@@ -932,10 +966,51 @@ class SphkOps:
 
     def _run_step(self, dt: float):
         self._step_dt = dt if self.adaptive else None
+        self._probe_recorded = False
         if self._step_body() is not False and self.adaptive:
             self.measure_speed()     # after the step's last velocity write
         self.last_dt = dt
         self.simulated_time += dt
+        if self._probe_recorded:     # the row's step index and simulated time, kept on the host beside the device ring
+            self._probe_meta[self._probe_rows % len(self._probe_meta)] = (self.steps_run, self.simulated_time)
+            self._probe_rows += 1
+        self.steps_run += 1
+
+    def set_probes(self, points=(), gauges=(), threshold: float = 0.5, capacity: int = 1024):
+        """probes (P, 3) and (a, b[, k]) gauges recorded into a device ring of `capacity` rows at the end of every following step
+        (SPHSystem::setProbes); no points and no gauges: off.  ValueError for a setting the library refuses (the setting is kept)."""
+        pts = capi.probe_points(points)
+        gs, ng = capi.gauge_structs(gauges, threshold)
+        if pts.shape[0] == 0 and ng == 0:
+            self._close_probes()
+            return
+        series = C.c_void_p()
+        rc = self.L.sphk_probe_series_create(C.byref(series), pts.ctypes.data_as(C.c_void_p), C.c_int(pts.shape[0]), gs, C.c_int(ng),
+                                             C.c_float(threshold), C.c_int(int(capacity)), C.c_void_p(self.stream.cuda_stream))
+        if rc:
+            raise ValueError(f"probe setting refused: {capi.sphk().sphk_error_string(C.c_int(rc)).decode()}")
+        self._close_probes()
+        self._probe_series, self._probe_shape = series, (pts.shape[0], ng, int(capacity))
+        self._probe_meta, self._probe_rows = [(0, 0.0)] * int(capacity), 0
+
+    def _close_probes(self):
+        if self._probe_series:
+            self.L.sphk_probe_series_destroy(self._probe_series)
+            self._probe_series = None
+
+    def probe_series(self) -> dict:
+        """as capi.SphApp.probe_series; synchronises"""
+        if not self._probe_series:
+            return None
+        P, G, cap = self._probe_shape
+        rec, lev = np.zeros((cap, P, capi.PROBE_FIELDS), np.float32), np.zeros((cap, G), np.float32)
+        count, rows = C.c_longlong(0), C.c_int(0)
+        check(self.L.sphk_probe_series_read(self._probe_series, C.byref(count), C.c_int(cap), rec.ctypes.data_as(C.c_void_p),
+                                            lev.ctypes.data_as(C.c_void_p), C.byref(rows)), "sphk_probe_series_read")
+        T, n = rows.value, count.value
+        meta = [self._probe_meta[r % cap] for r in range(n - T, n)]
+        return {"steps": np.array([m[0] for m in meta], np.int64), "times": np.array([m[1] for m in meta], np.float64),
+                "records": rec[:T], "levels": lev[:T], "overwritten": n - T}
 
     def _step_body(self):
         e = self.open_emit() if self.open else 0
@@ -954,6 +1029,9 @@ class SphkOps:
         if not self._step_solver():
             return False             # the "throwing" first call: no sweep ran, nothing to integrate (as in SPHSystem::step)
         self.bodies_integrate()
+        if self._probe_series:       # as SPHSystem::recordProbes, after the bodies' integration
+            check(self.L.sphk_probes_record(self.ctx, self._s(), self._probe_series, *self._probe_sources()), "sphk_probes_record")
+            self._probe_recorded = True
 
     def _step_solver(self) -> bool:
         """the solver's part of a step; False for PBD's "throwing" first call"""
@@ -976,6 +1054,7 @@ class SphkOps:
                 "p2cB": g(self.boundary.p2c), "cell_startB": g(self.cs_boundary)}
 
     def close(self):
+        self._close_probes()
         if self.ctx:
             self.L.sphk_synchronize(self.ctx)
             self.L.sphk_destroy(self.ctx)

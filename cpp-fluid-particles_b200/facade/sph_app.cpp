@@ -669,6 +669,75 @@ extern "C" int sph_app_adhesion_stats(sph_app* app, int* wetted, float* max_acce
 #endif
 }
 
+extern "C" int sph_app_set_probes(sph_app* app, int n_points, const float* points_xyz, int n_gauges, const float* gauge_ab,
+                                  const int* gauge_samples, float threshold, int capacity) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)n_points; (void)points_xyz; (void)n_gauges; (void)gauge_ab; (void)gauge_samples; (void)threshold; (void)capacity;
+    return 1;
+#else
+    if (!app || n_points < 0 || n_gauges < 0 || (n_points > 0 && !points_xyz) || (n_gauges > 0 && (!gauge_ab || !gauge_samples))) return 1;
+    if (n_points == 0 && n_gauges == 0) { app->system->clearProbes(); return 0; }
+    sphb200::Probes p;
+    for (int k = 0; k < n_points; ++k) p.points.push_back(make_float3(points_xyz[3 * k], points_xyz[3 * k + 1], points_xyz[3 * k + 2]));
+    for (int k = 0; k < n_gauges; ++k) {
+        const float* g = gauge_ab + 6 * k;
+        p.gauges.push_back(sphb200::Gauge{make_float3(g[0], g[1], g[2]), make_float3(g[3], g[4], g[5]), gauge_samples[k]});
+    }
+    p.threshold = threshold;
+    p.capacity = capacity;
+    return app->system->setProbes(p) ? 0 : 1;
+#endif
+}
+
+extern "C" int sph_app_probe_series(sph_app* app, int* rows, int* n_points, int* n_gauges, long long* overwritten, long long* steps,
+                                    double* times, float* records, float* levels) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)rows; (void)n_points; (void)n_gauges; (void)overwritten; (void)steps; (void)times; (void)records; (void)levels;
+    return 1;
+#else
+    if (!app) return 1;
+    const sphb200::ProbeSeries ps = app->system->probeSeries();
+    if (rows) *rows = static_cast<int>(ps.steps.size());
+    if (n_points) *n_points = ps.probes;
+    if (n_gauges) *n_gauges = ps.gauges;
+    if (overwritten) *overwritten = ps.overwritten;
+    if (steps) std::copy(ps.steps.begin(), ps.steps.end(), steps);
+    if (times) std::copy(ps.times.begin(), ps.times.end(), times);
+    if (records) std::copy(ps.records.begin(), ps.records.end(), records);
+    if (levels) std::copy(ps.levels.begin(), ps.levels.end(), levels);
+    return 0;
+#endif
+}
+
+extern "C" int sph_app_sample_probes(sph_app* app, int n, const float* points_xyz, float* out) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)n; (void)points_xyz; (void)out;
+    return 1;
+#else
+    if (!app || n < 1 || !points_xyz || !out) return 1;
+    std::vector<float3> pts;
+    for (int k = 0; k < n; ++k) pts.push_back(make_float3(points_xyz[3 * k], points_xyz[3 * k + 1], points_xyz[3 * k + 2]));
+    const std::vector<float> r = app->system->sampleProbes(pts);
+    if (r.size() != 8 * static_cast<size_t>(n)) return 1;
+    std::copy(r.begin(), r.end(), out);
+    return 0;
+#endif
+}
+
+extern "C" int sph_app_sample_lattice(sph_app* app, const float* origin, float spacing, const int* dims, float* out) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)origin; (void)spacing; (void)dims; (void)out;
+    return 1;
+#else
+    if (!app || !origin || !dims || !out) return 1;
+    const std::vector<float> r = app->system->sampleLattice(make_float3(origin[0], origin[1], origin[2]), spacing,
+                                                            make_int3(dims[0], dims[1], dims[2]));
+    if (r.empty()) return 1;
+    std::copy(r.begin(), r.end(), out);
+    return 0;
+#endif
+}
+
 extern "C" int sph_app_set_adaptive_dt(sph_app* app, float C, float dt_min, float dt_max) {
 #ifdef SPH_APP_REFERENCE_ENGINE
     (void)app; (void)C; (void)dt_min; (void)dt_max;

@@ -800,6 +800,7 @@ SPHSystem::SPHSystem(std::shared_ptr<SPHParticles>& fluidParticles, std::shared_
 SPHSystem::~SPHSystem() noexcept {
     if (_engine && _engine->ok()) sphk_synchronize(_engine->ctx());
     if (_graphExec) cudaGraphExecDestroy(_graphExec);
+    sphk_probe_series_destroy(_probeSeries);
     if (_evStart) cudaEventDestroy(_evStart);
     if (_evStop) cudaEventDestroy(_evStop);
 }
@@ -1094,8 +1095,10 @@ float SPHSystem::runStep() {
     // replayable.  (Particles moved behind the engine's back need nothing special: the replayed step begins with the
     // fluid neighbour search, which re-packs the records from the API arrays.)
     if (_graphExec && (_graphConfigEpoch != solverConfigEpoch() || !solverIsGraphSafe())) dropStepGraph();
+    _probeRecorded = false;
     if (_graphExec) {
         _engine->shadowsStale = false;
+        _probeRecorded = _probeSeries != nullptr;     // (a series set or cleared drops the graph: it was captured with this one)
         CUDA_CALL(cudaGraphLaunch(_graphExec, st));
         sphk_add_launches(ctx, _graphLaunches);
         check(sphk_synchronize(ctx), "step");
@@ -1112,6 +1115,7 @@ float SPHSystem::runStep() {
                               _sphSmoothingRadius, _stepDt, _sphRho0, _sphRhoBoundary, _sphStiff, _sphVisc, _sphG,
                               _sphSurfaceTensionIntensity, _sphAirPressure);
             integrateBodies();
+            recordProbes();
             if (_adaptive) measureSpeed();      // after the step's last velocity write; read before the next step
             ok = true;
         } catch (const char* s) {
@@ -1137,6 +1141,7 @@ float SPHSystem::runStep() {
                                   _sphCellLength, _sphSmoothingRadius, _stepDt, _sphRho0, _sphRhoBoundary, _sphStiff, _sphVisc,
                                   _sphG, _sphSurfaceTensionIntensity, _sphAirPressure);
                     integrateBodies();
+                    recordProbes();
                 } catch (const char* s) {
                     std::cout << s << "\n";
                 } catch (...) {
@@ -1150,11 +1155,156 @@ float SPHSystem::runStep() {
     }
     _lastDt = _stepDt;
     _simTime += _stepDt;
+    if (_probeRecorded) {                        // the row recordProbes() enqueued: its step and time
+        const size_t slot = static_cast<size_t>(_probeRows % _probes.capacity);
+        _probeSteps[slot] = _steps;
+        _probeTimes[slot] = _simTime;
+        ++_probeRows;
+    }
+    ++_steps;
     float milliseconds = 0.0f;
     CUDA_CALL(cudaEventRecord(_evStop, st));
     CUDA_CALL(cudaEventSynchronize(_evStop));
     CUDA_CALL(cudaEventElapsedTime(&milliseconds, _evStart, _evStop));
     return milliseconds;
+}
+
+// ---- probes and water-level gauges (DESIGN.md section 2.13) ----
+sphk_scene SPHSystem::probeScene() const {
+    sphk_scene s{};
+    s.fluid = _fluids->abi();
+    s.boundary = _boundaries->abi();
+    s.cell_start_fluid = cellStartFluid.addr();
+    s.cell_start_boundary = cellStartBoundary.addr();
+    s.radius = _sphSmoothingRadius;
+    return s;
+}
+
+// the pressure a WCSPH step computed (DFSPH and PBD keep none), and the temperatures while heat transfer is on
+void SPHSystem::probeSources(const float*& pressure, const float*& temperature) const {
+    auto* basic = dynamic_cast<BasicSPHSolver*>(_solver.get());
+    pressure = basic && typeid(*basic) == typeid(BasicSPHSolver) ? _fluids->getPressurePtr() : nullptr;
+    temperature = basic && basic->thermalOn() ? basic->temperatureField().addr() : nullptr;
+}
+
+void SPHSystem::recordProbes() {
+    if (!_probeSeries || fluidSize() == 0) return;     // (an open system that runs empty records no row)
+    const sphk_scene s = probeScene();
+    const float *p = nullptr, *t = nullptr;
+    probeSources(p, t);
+    const int rc = sphk_probes_record(_engine->ctx(), &s, _probeSeries, p, t);
+    check(rc, "sphk_probes_record");
+    _probeRecorded = rc == 0;
+}
+
+bool SPHSystem::setProbes(const sphb200::Probes& probes) {
+    std::vector<float> pts;
+    for (const float3& q : probes.points) pts.insert(pts.end(), {q.x, q.y, q.z});
+    std::vector<sphk_gauge> gs;
+    for (const auto& g : probes.gauges) gs.push_back(sphk_gauge{{g.a.x, g.a.y, g.a.z}, {g.b.x, g.b.y, g.b.z}, g.samples});
+    if (probes.points.size() > SPHK_PROBE_LIMIT || probes.gauges.size() > SPHK_GAUGE_LIMIT) {
+        printf("setProbes: at most %d probes and %d gauges (got %zu, %zu); the setting is kept\n", SPHK_PROBE_LIMIT, SPHK_GAUGE_LIMIT,
+               probes.points.size(), probes.gauges.size());
+        return false;
+    }
+    if (!_engine->ok()) return false;
+    sphk_probe_series* series = nullptr;
+    const int rc = sphk_probe_series_create(&series, pts.data(), static_cast<int>(probes.points.size()), gs.data(),
+                                            static_cast<int>(gs.size()), probes.threshold, probes.capacity, _engine->stream());
+    if (rc != 0) {
+        printf("setProbes: refused (%s): need finite points, gauges with a != b and 2..%d samples, a finite threshold > 0, a capacity "
+               "in [1, %d] and at least one probe or gauge; the setting is kept\n", sphk_error_string(rc), SPHK_GAUGE_MAX_SAMPLES,
+               SPHK_PROBE_CAPACITY_LIMIT);
+        return false;
+    }
+    dropStepGraph();
+    sphk_probe_series_destroy(_probeSeries);
+    _probeSeries = series;
+    _probes = probes;
+    _probeSteps.assign(static_cast<size_t>(probes.capacity), 0);
+    _probeTimes.assign(static_cast<size_t>(probes.capacity), 0.0);
+    _probeRows = 0;
+    return true;
+}
+
+void SPHSystem::clearProbes() {
+    if (!_probeSeries) return;
+    dropStepGraph();
+    sphk_probe_series_destroy(_probeSeries);
+    _probeSeries = nullptr;
+}
+
+sphb200::ProbeSeries SPHSystem::probeSeries() const {
+    sphb200::ProbeSeries out;
+    if (!_probeSeries) return out;
+    out.probes = static_cast<int>(_probes.points.size());
+    out.gauges = static_cast<int>(_probes.gauges.size());
+    const int cap = _probes.capacity;
+    out.records.resize(static_cast<size_t>(cap) * out.probes * SPHK_PROBE_FIELDS);
+    out.levels.resize(static_cast<size_t>(cap) * out.gauges);
+    long long count = 0;
+    int rows = 0;
+    const int rc = sphk_probe_series_read(_probeSeries, &count, cap, out.records.data(), out.levels.data(), &rows);
+    check(rc, "sphk_probe_series_read");
+    if (rc != 0) rows = 0;
+    if (rc == 0 && count != _probeRows) printf("probeSeries: the device recorded %lld rows, the host %lld\n", count, _probeRows);
+    out.records.resize(static_cast<size_t>(rows) * out.probes * SPHK_PROBE_FIELDS);
+    out.levels.resize(static_cast<size_t>(rows) * out.gauges);
+    for (long long r = count - rows; r < count; ++r) {
+        out.steps.push_back(_probeSteps[static_cast<size_t>(r % cap)]);
+        out.times.push_back(_probeTimes[static_cast<size_t>(r % cap)]);
+    }
+    out.overwritten = count - rows;
+    return out;
+}
+
+std::vector<float> SPHSystem::sampleProbes(const std::vector<float3>& points) const {
+    std::vector<float> out;
+    if (!_engine->ok() || points.empty() || fluidSize() == 0) return out;
+    const size_t n = points.size();
+    float *dp = nullptr, *dout = nullptr;
+    CUDA_CALL(cudaMalloc(&dp, 12 * n));
+    CUDA_CALL(cudaMalloc(&dout, 32 * n));
+    CUDA_CALL(cudaMemcpyAsync(dp, points.data(), 12 * n, cudaMemcpyHostToDevice, _engine->stream()));
+    const sphk_scene s = probeScene();
+    const float *p = nullptr, *t = nullptr;
+    probeSources(p, t);
+    const int rc = sphk_probe_sample(_engine->ctx(), &s, dp, static_cast<int>(n), p, t, dout);
+    check(rc, "sphk_probe_sample");
+    if (rc == 0) {
+        out.resize(8 * n);
+        CUDA_CALL(cudaMemcpyAsync(out.data(), dout, 32 * n, cudaMemcpyDeviceToHost, _engine->stream()));
+    }
+    check(sphk_synchronize(_engine->ctx()), "sphk_synchronize");
+    cudaFree(dp);
+    cudaFree(dout);
+    return out;
+}
+
+std::vector<float> SPHSystem::sampleLattice(float3 origin, float spacing, int3 dims) const {
+    std::vector<float> out;
+    if (!_engine->ok() || fluidSize() == 0) return out;
+    const long long total = static_cast<long long>(dims.x) * dims.y * dims.z;
+    if (dims.x < 1 || dims.y < 1 || dims.z < 1 || total > (1LL << 27)) {
+        printf("sampleLattice: dims must be >= 1 with at most 2^27 points (got %d x %d x %d)\n", dims.x, dims.y, dims.z);
+        return out;
+    }
+    float* dout = nullptr;
+    CUDA_CALL(cudaMalloc(&dout, 32 * static_cast<size_t>(total)));
+    const sphk_scene s = probeScene();
+    const float *p = nullptr, *t = nullptr;
+    probeSources(p, t);
+    const float o[3] = {origin.x, origin.y, origin.z};
+    const int d[3] = {dims.x, dims.y, dims.z};
+    const int rc = sphk_probe_lattice(_engine->ctx(), &s, o, spacing, d, p, t, dout);
+    check(rc, "sphk_probe_lattice");
+    if (rc == 0) {
+        out.resize(8 * static_cast<size_t>(total));
+        CUDA_CALL(cudaMemcpyAsync(out.data(), dout, 32 * static_cast<size_t>(total), cudaMemcpyDeviceToHost, _engine->stream()));
+    }
+    check(sphk_synchronize(_engine->ctx()), "sphk_synchronize");
+    cudaFree(dout);
+    return out;
 }
 
 // vbo.cu:46-51

@@ -173,6 +173,27 @@ struct AdhesionStats {
     float maxAccel = 0.0f;           // largest |a_i|
 };
 
+// addition: probes and water-level gauges (DESIGN.md section 2.13; sphk_probe_* in sphk.h)
+struct Gauge {
+    float3 a, b;                     // the segment, a != b (orient it along -G for a water level measured from a)
+    int samples = 64;                // in [2, SPHK_GAUGE_MAX_SAMPLES]
+};
+struct Probes {
+    std::vector<float3> points;      // at most SPHK_PROBE_LIMIT
+    std::vector<Gauge> gauges;       // at most SPHK_GAUGE_LIMIT
+    float threshold = 0.5f;          // a gauge sample is wet when its Shepard sum S >= threshold (finite, > 0)
+    int capacity = 1024;             // rows of the device ring, in [1, SPHK_PROBE_CAPACITY_LIMIT]
+};
+// the last min(recorded, capacity) rows of a series, oldest first
+struct ProbeSeries {
+    int probes = 0, gauges = 0;
+    std::vector<long long> steps;    // the system's step index of each row (the constructor's step is 0)
+    std::vector<double> times;       // simulatedTime() after that step
+    std::vector<float> records;      // [rows][probes][SPHK_PROBE_FIELDS]: S, rho, vx, vy, vz, p, T, n
+    std::vector<float> levels;       // [rows][gauges]
+    long long overwritten = 0;       // rows recorded but no longer in the ring
+};
+
 // addition: scenes from triangle meshes (DESIGN.md section 2.12; sphk_mesh_* in sphk.h).  The functions below run on the legacy
 // default stream, need no SPHSystem, and throw std::runtime_error when the library refuses a mesh or a call fails.
 struct TriangleMesh {
@@ -662,6 +683,18 @@ public:
     float lastTimeStep() const { return _lastDt; }            // the dt of the last step
     double simulatedTime() const { return _simTime; }         // the double sum of the float dt of every step
     sphb200::AdaptiveStats adaptiveStats() const { return _adaptiveStats; }
+    // probes and gauges (DESIGN.md section 2.13): from the next step on, every step() records one row -- the probes' records and
+    // the gauges' levels of the state the step leaves -- into a device ring, inside a captured step graph too (no host
+    // synchronisation of its own).  p is recorded for a BasicSPHSolver (WCSPH) only, T while heat transfer is on.  Out-of-range
+    // settings are refused (printed, setting kept, false); setting or clearing drops the step graph.
+    bool setProbes(const sphb200::Probes& probes);
+    void clearProbes();
+    bool probesOn() const { return _probeSeries != nullptr; }
+    sphb200::ProbeSeries probeSeries() const;      // synchronises
+    // on demand, between steps (synchronise): records of the given points, and of the lattice origin + spacing (i, j, k), z fastest
+    // ([nx][ny][nz][8]); an empty vector when refused (printed)
+    std::vector<float> sampleProbes(const std::vector<float3>& points) const;
+    std::vector<float> sampleLattice(float3 origin, float spacing, int3 dims) const;
 
 private:
     std::shared_ptr<SPHParticles> _fluids;
@@ -717,6 +750,16 @@ private:
     float runStep();                      // one step at _stepDt
     float chooseTimeStep(double remaining, bool& frameEnd);   // waits for the last speed bound, applies the rule
     void measureSpeed();                  // enqueues the speed bound of the current state (sphk_step_speed)
+    // probes: the series, and per recorded row (slot row mod capacity) the step index and simulated time the host saw
+    sphk_probe_series* _probeSeries = nullptr;
+    sphb200::Probes _probes;
+    std::vector<long long> _probeSteps;
+    std::vector<double> _probeTimes;
+    long long _probeRows = 0, _steps = 0;
+    bool _probeRecorded = false;          // the step in flight enqueued a row
+    sphk_scene probeScene() const;
+    void probeSources(const float*& pressure, const float*& temperature) const;
+    void recordProbes();                  // sphk_probes_record at the end of a step (inside a captured step graph)
 };
 
 // ---- vbo.cu:46-51 --------------------------------------------------------------------------------

@@ -42,6 +42,11 @@ public:
     float step();
 
     bool ok() const { return ok_; }
+    // probes and gauges are single-context only (a probe near a cut would miss the other rank's fluid): refused, printed
+    bool setProbes(const sphb200::Probes&) {
+        printf("SlabSPHSystem: probes and gauges are not supported on slab ranks (single-GPU SPHSystem only)\n");
+        return false;
+    }
     int size() const { return nOwn_; }                  // particles this rank owns
     int ownedBegin() const { return ownBegin_; }        // ... stored at [ownedBegin, ownedBegin + size) of the local set
     int globalSize() const { return nGlobal_; }

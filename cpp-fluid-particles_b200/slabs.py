@@ -1010,6 +1010,10 @@ class SlabSystem(SphkOps):
         if spec is not None:
             raise ValueError("adhesion is not supported on slab ranks (single-GPU engine.SphkSystem only)")
 
+    # probes and gauges: a probe near a cut would miss the other rank's fluid
+    def set_probes(self, points=(), gauges=(), threshold=0.5, capacity=1024):
+        raise ValueError("probes and gauges are not supported on slab ranks (single-GPU engine.SphkSystem only)")
+
     # heat transfer: ghosts and strays would need their temperatures carried as a second array
     @property
     def thermal(self):

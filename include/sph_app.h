@@ -121,6 +121,22 @@ int   sph_app_set_adhesion(sph_app* app, int on, float wall, int n_bodies, const
 /* wetted particles and the largest |a_i| of the last step's adhesion sweep (either pointer may be NULL); synchronises; 1 on the
  * reference build */
 int   sph_app_adhesion_stats(sph_app* app, int* wetted, float* max_accel);
+/* Probes and water-level gauges (SPHSystem::setProbes; DESIGN.md section 2.13): from the next step on every step records the
+ * records {S, rho, vx, vy, vz, p, T, n} of n_points points (points_xyz: float[3 n_points]) and the levels of n_gauges gauges
+ * (gauge_ab: float[6 n_gauges] = {a.xyz, b.xyz}, gauge_samples: int[n_gauges]) into a ring of `capacity` rows.  n_points = n_gauges
+ * = 0: off.  Returns 1 on the reference build and for a setting the class layer refuses (the setting is then kept). */
+int   sph_app_set_probes(sph_app* app, int n_points, const float* points_xyz, int n_gauges, const float* gauge_ab,
+                         const int* gauge_samples, float threshold, int capacity);
+/* The recorded rows still in the ring, oldest first (synchronises).  With steps, times, records and levels all NULL: only the counts
+ * (*rows, *n_points, *n_gauges, *overwritten); otherwise also steps[rows] (the step index), times[rows] (simulated time after the
+ * step), records[rows][n_points][8] and levels[rows][n_gauges] -- arrays sized from a count query made since the last step.  Any
+ * count pointer may be NULL.  1 on the reference build. */
+int   sph_app_probe_series(sph_app* app, int* rows, int* n_points, int* n_gauges, long long* overwritten, long long* steps,
+                           double* times, float* records, float* levels);
+/* On demand, between steps (synchronise): records of n points (float[3 n]) into out (float[8 n]); records of the lattice origin +
+ * spacing (i, j, k), z fastest, into out (float[8 nx ny nz]).  1 for a refused call and on the reference build. */
+int   sph_app_sample_probes(sph_app* app, int n, const float* points_xyz, float* out);
+int   sph_app_sample_lattice(sph_app* app, const float* origin, float spacing, const int* dims, float* out);
 /* Kinematic rigid bodies (SPHSystem's constructor with a vector of sphb200::KinematicBody; DESIGN.md section 2.3).  No
  * reference counterpart: NULL / 1 on the reference build.  Body b is the points body_xyz[body_begin[b] .. body_begin[b+1])
  * (body coordinates; body_begin[0] = 0), pose[7 b ..] = {cx, cy, cz, qx, qy, qz, qw} (quaternion scalar part last),

@@ -640,6 +640,58 @@ int sphk_mesh_fill(const sphk_mesh* m, float spacing, const float origin[3], flo
  * capacity as sphk_mesh_fill.  Synchronises.  SPHK_ERR_INVALID also for r <= 0 and more than 2^31 - 1 candidates. */
 int sphk_mesh_sample_surface(const sphk_mesh* m, float r, float* pos_out, int capacity, int* count_host);
 
+/* ---- probes and water-level gauges (no reference counterpart; DESIGN.md section 2.13) ------------------------------------------
+ * SPH-interpolated fluid fields at points.  For a point x, over the fluid particles j with |x - x_j| <= R and rho_j > 0, with
+ * V_j = m_j / rho_j and W the continuous cubic spline of radius R (W(0) > 0: no quirk Q1, so the interpolant does not jump when x
+ * sits on a particle; boundary particles take no part):
+ *   S(x) = sum_j V_j W (the Shepard sum),  n(x) = the count of those particles,
+ *   A(x) = sum_j V_j A_j W / S  for A in {rho, v, p, T}   (so rho(x) = sum_j m_j W / S)
+ * A record is 8 floats {S, rho, vx, vy, vz, p, T, n} (32 bytes, 16-byte aligned).  A point with no such particle, or outside the
+ * grid, is dry: n = 0 and zeros (S = 0 with n > 0 -- every particle exactly at R -- also gives zero fields).  p is NaN when
+ * pressure_or_null is NULL (only WCSPH keeps a pressure field), T is NaN when temperature_or_null is NULL.
+ * A gauge is the segment a -> b with k samples a + (b - a) (i / (k - 1)), i = 0..k-1 (each operation rounded once).  With i* the
+ * highest sample with S >= threshold, its level is the linear crossing of the threshold between i* and i* + 1, measured from a
+ * along the segment; |b - a| when i* = k - 1 (overtopped); -1 when no sample is wet.  A gauge has no notion of up: orient it along
+ * -G for a water level.
+ * Every entry reads the API arrays pos, vel, mass, density (and the optional pressure and temperature arrays, in the fluid's
+ * current order) as the caller left them and the fluid cell ranges of the last search -- not the packed records.  Reach: the cells
+ * within 1 of the point's (2 when positions have moved since the search), so no particle may have moved more than one cell since
+ * the search (the sphk_bodies_react / sphk_adhesion contract).  Particles outside the grid do not count; live particles only.
+ * Refused before anything is enqueued: NULL pointers, a non-finite value, an output overlapping a scene array or an input
+ * (SPHK_ERR_INVALID); the set not searched or sized otherwise, and an active range (slab ranks) (SPHK_ERR_STATE). */
+#define SPHK_PROBE_FIELDS 8
+#define SPHK_PROBE_LIMIT 4096                 /* probes of one series */
+#define SPHK_GAUGE_LIMIT 64                   /* gauges of one series or call */
+#define SPHK_GAUGE_MAX_SAMPLES 1024           /* samples per gauge (at least 2) */
+#define SPHK_PROBE_CAPACITY_LIMIT 65536       /* rows of a series ring */
+typedef struct sphk_gauge {
+    float a[3], b[3];        /* the segment, a != b */
+    int samples;             /* k in [2, SPHK_GAUGE_MAX_SAMPLES] */
+} sphk_gauge;
+/* records of n points (device float3[n]) into out (device float[8 n]).  The points are checked for finite values on the device
+ * first, which synchronises. */
+int sphk_probe_sample(sphk_ctx* ctx, const sphk_scene* s, const float* points, int n, const float* pressure_or_null,
+                      const float* temperature_or_null, float* out);
+/* records of the lattice origin + spacing (ix, iy, iz) (multiply then add, per axis), z fastest -- the cell hash's order -- into
+ * out[nx][ny][nz][8].  spacing > 0 and finite, dims >= 1, at most 2^31 - 1 points. */
+int sphk_probe_lattice(sphk_ctx* ctx, const sphk_scene* s, const float origin[3], float spacing, const int dims[3],
+                       const float* pressure_or_null, const float* temperature_or_null, float* out);
+/* levels of n_gauges (1..SPHK_GAUGE_LIMIT) gauges (host array) into out (device float[n_gauges]); threshold finite and > 0 */
+int sphk_gauge_levels(sphk_ctx* ctx, const sphk_scene* s, const sphk_gauge* gauges, int n_gauges, float threshold, float* out);
+/* A series: fixed probes (host float3[n_points], up to SPHK_PROBE_LIMIT) and gauges (host, up to SPHK_GAUGE_LIMIT; at least one of
+ * the two) recorded into a device ring of `capacity` rows.  sphk_probes_record writes the row into slot (counter mod capacity) and
+ * then advances the counter, both on the device: no argument changes from step to step, so the two launches can sit inside a
+ * captured step graph.  sphk_probe_series_read (synchronises on the series' stream) gives the counter and copies the last
+ * min(counter, capacity, max_rows) rows, oldest first: records [rows][n_points][8] and levels [rows][n_gauges]. */
+typedef struct sphk_probe_series sphk_probe_series;
+int sphk_probe_series_create(sphk_probe_series** series, const float* points_host, int n_points, const sphk_gauge* gauges_host,
+                             int n_gauges, float threshold, int capacity, void* stream);
+void sphk_probe_series_destroy(sphk_probe_series* series);
+int sphk_probes_record(sphk_ctx* ctx, const sphk_scene* s, sphk_probe_series* series, const float* pressure_or_null,
+                       const float* temperature_or_null);
+int sphk_probe_series_read(sphk_probe_series* series, long long* counter, int max_rows, float* records_host, float* levels_host,
+                           int* rows);
+
 /* ---- render export: generate_dots_CUDA, vbo.cu:26-44 (SURVEY 8f-2) -----------------------------------------------
  * dot[i] = pos[i]; colour[i] from density[i] (blue below 0.75, blend to white at 1.0, blend to pink above).  Plain
  * device buffers instead of a mapped GL vertex buffer; synchronises like the reference (vbo.cu:49). */
