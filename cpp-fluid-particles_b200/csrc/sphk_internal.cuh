@@ -144,6 +144,13 @@ struct sphk_ctx {
         long long mark = -1;
         unsigned long long seq = 0;            // corrSeq at that sweep: chunks stamped later have moved
     } tok;
+    // Velocity fixed points (sphk_sweeps.cu, "Velocity epochs"): a correct sweep's quiet epilogue leaves a chunk it has been
+    // through once untouched until anything else writes velocities.
+    unsigned char* chunkMark = nullptr;        // device [capF / 32 + 1]: 1 = the chunk's vel and rec.b hold a fixed point of the
+                                               // quiet epilogue (written by every correct sweep that keeps the marks)
+    long long velCredited = 0;                 // launches that write neither vel nor rec.b, or keep the marks -- see vel_mark()
+    long long velMark = -1;                    // vel_mark() after the last correct sweep that kept the marks ...
+    const float* velArr = nullptr;             // ... and its fluid velocities
     BodyState* bodies = nullptr;     // non-null after sphk_bodies_init
     float* viscStats = nullptr;      // [2] device: {iterations (int bits), |r|_M / |b|_M} of the last sphk_implicit_viscosity
     float* rheoStats = nullptr;      // [6] device: {iterations, |r|_M / |b|_M, max gamma_dot, min nu, max nu, count at nu_max} of the
@@ -185,6 +192,8 @@ struct DevScene {
     unsigned long long* stamp;       // non-null: correct sweeps stamp the chunks they gathered in with `seq`
     unsigned long long seq;          // correct sweeps: their stamp; error sweeps with `reuse`: the token's
     int reuse;                       // error sweeps: the previous error sweep's outputs stand for chunks quiet since `seq`
+    unsigned char* mark;             // non-null: this correct sweep writes every chunk's velocity fixed-point mark ...
+    int trust;                       // ... and may skip a quiet chunk whose mark is set (not the first sweep of its epoch)
     int3 cs, org;
     float cellLength;
     float r2list;                    // candidate cut-off of the cell walk: r2cut, or (R + skin)^2 when building a skin list
@@ -208,6 +217,10 @@ __device__ __forceinline__ float3 operator/(float3 a, float s) { return f3(a.x /
 __device__ __forceinline__ void operator+=(float3& a, float3 b) { a.x += b.x; a.y += b.y; a.z += b.z; }
 __device__ __forceinline__ void operator-=(float3& a, float3 b) { a.x -= b.x; a.y -= b.y; a.z -= b.z; }
 __device__ __forceinline__ float dot3(float3 a, float3 b) { return a.x * b.x + a.y * b.y + a.z * b.z; }
+__device__ __forceinline__ bool same_bits3(float3 a, float3 b) {
+    return __float_as_uint(a.x) == __float_as_uint(b.x) && __float_as_uint(a.y) == __float_as_uint(b.y) &&
+           __float_as_uint(a.z) == __float_as_uint(b.z);
+}
 
 __device__ __forceinline__ float3 load3(const float* __restrict__ p, int i) {
     return f3(p[3 * i], p[3 * i + 1], p[3 * i + 2]);

@@ -222,6 +222,7 @@ extern "C" int sphk_create(sphk_ctx** out, int max_fluid, int max_boundary, cons
     if (e == cudaSuccess) e = dalloc(&c->tileWin, (static_cast<size_t>(max_fluid) / SPHK_BLOCK + 1) * SPHK_TILE_WINS);
     if (e == cudaSuccess) e = dalloc(&c->chunkAct, static_cast<size_t>(max_fluid) / 32 + 1);
     if (e == cudaSuccess) e = dalloc(&c->chunkStamp, static_cast<size_t>(max_fluid) / 32 + 1);
+    if (e == cudaSuccess) e = dalloc(&c->chunkMark, static_cast<size_t>(max_fluid) / 32 + 1);
     if (e == cudaSuccess) {
         int dev = 0;
         cudaGetDevice(&dev);
@@ -251,7 +252,7 @@ extern "C" void sphk_destroy(sphk_ctx* c) {
     if (!c) return;
     cudaFree(c->keys); cudaFree(c->keysSorted); cudaFree(c->idx); cudaFree(c->idxSorted);
     cudaFree(c->snapA); cudaFree(c->snapB); cudaFree(c->rec.a); cudaFree(c->rec.b); cudaFree(c->massRange); cudaFree(c->dispMax); cudaFree(c->cellFlag);
-    cudaFree(c->tmpF); cudaFree(c->partial); cudaFree(c->loops); cudaFree(c->viscStats); cudaFree(c->rheoStats); cudaFree(c->heatGroups); cudaFree(c->heatStats); cudaFree(c->heatRed); cudaFree(c->adhGroups); cudaFree(c->adhStats); cudaFree(c->cnt); cudaFree(c->nbr); cudaFree(c->cubTemp); cudaFree(c->tileWin); cudaFree(c->chunkAct); cudaFree(c->chunkStamp);
+    cudaFree(c->tmpF); cudaFree(c->partial); cudaFree(c->loops); cudaFree(c->viscStats); cudaFree(c->rheoStats); cudaFree(c->heatGroups); cudaFree(c->heatStats); cudaFree(c->heatRed); cudaFree(c->adhGroups); cudaFree(c->adhStats); cudaFree(c->cnt); cudaFree(c->nbr); cudaFree(c->cubTemp); cudaFree(c->tileWin); cudaFree(c->chunkAct); cudaFree(c->chunkStamp); cudaFree(c->chunkMark);
     if (c->pinned) cudaFreeHost(c->pinned);
     cudaFree(c->openDev);
     if (c->openPinned) cudaFreeHost(c->openPinned);
@@ -435,6 +436,8 @@ extern "C" int sphk_copy(sphk_ctx* c, float* dst, const float* src, int n_floats
     if (dst == c->sTag) c->sTag = nullptr;
     // a copy is no launch (act_mark() does not see it): one into an array of the DFSPH error sweeps ends their reuse
     if (dst == c->tok.density || dst == c->tok.alpha || dst == c->tok.error || dst == c->tok.stiff) c->tok.kind = 0;
+    // ... and one over the velocities of the last correct sweep ends their epoch
+    if (c->velArr && dst < c->velArr + 3 * static_cast<size_t>(c->capF) && dst + n_floats > c->velArr) c->velMark = -1;
     SPHK_CUDA_TRY(cudaMemcpyAsync(dst, src, sizeof(float) * static_cast<size_t>(n_floats), cudaMemcpyDeviceToDevice, c->stream));
     return SPHK_OK;
 }
@@ -446,7 +449,7 @@ extern "C" int sphk_reduce_abs_sum(sphk_ctx* c, const float* x, int n, float* ho
     if (blocks > 1024) blocks = 1024;
     k_abs_sum_partial<<<blocks, 256, 0, c->stream>>>(x, n, c->partial);
     k_abs_sum_final<<<1, 256, 0, c->stream>>>(c->partial, blocks, c->partial);
-    c->launches += 2; c->credited += 2;   // writes only the partials
+    c->launches += 2; c->credited += 2; c->velCredited += 2;   // writes only the partials
     SPHK_CUDA_TRY(cudaMemcpyAsync(c->pinned, c->partial, sizeof(float), cudaMemcpyDeviceToHost, c->stream));
     SPHK_CUDA_TRY(cudaStreamSynchronize(c->stream));
     *host_out = *c->pinned;
@@ -582,7 +585,7 @@ __global__ void __launch_bounds__(256) k_loop_finish(LoopState* st, const float*
 extern "C" int sphk_loop_begin(sphk_ctx* c, int slot, int min_iter, int max_iter, float threshold, int reduce_from_iter) {
     if (!c || slot < 0 || slot > 1 || max_iter < 0) return SPHK_ERR_INVALID;
     k_loop_begin<<<1, 1, 0, c->stream>>>(c->loops + slot, min_iter, max_iter, threshold, reduce_from_iter);
-    c->launches++; c->credited++;      // loop control writes only its LoopState (chunk activity stays valid)
+    c->launches++; c->credited++; c->velCredited++;   // loop control writes only its LoopState (chunk activity stays valid)
     c->pred = &c->loops[slot].active;
     SPHK_CUDA_TRY(cudaGetLastError());
     return SPHK_OK;
@@ -595,7 +598,7 @@ extern "C" int sphk_loop_next(sphk_ctx* c, int slot, const float* error, int n) 
     if (blocks > 1024) blocks = 1024;
     k_loop_partial<<<blocks, 256, 0, c->stream>>>(c->loops + slot, error, n, c->partial);
     k_loop_finish<<<1, 256, 0, c->stream>>>(c->loops + slot, c->partial, blocks);
-    c->launches += 2; c->credited += 2;
+    c->launches += 2; c->credited += 2; c->velCredited += 2;
     SPHK_CUDA_TRY(cudaGetLastError());
     return SPHK_OK;
 }

@@ -191,12 +191,26 @@ template <int kMode /*0: vel += a, 1: vel += a/dt, 2: deltaPos = a/rho0*/> struc
     __device__ void pair(Acc& a, int, int, bool, float3 d, float r2, float mj, float4 lo, float4 hi, const DevScene& s) const {
         a.a += mj * (a.ki + lo.w) * (d * grad_w_factor(sqrtf(r2), s.k));
     }
+    __device__ float3 velocity(float3 sum, float4 hi) const {
+        const float3 dv = (kMode == 1) ? sum / dt_or_rho0 : sum;
+        return f3(hi.x + dv.x, hi.y + dv.y, hi.z + dv.z);
+    }
     __device__ void end(Acc& a, int i, float4, float4 hi, const DevScene&) const {
         if (kMode == 2) { store3(deltaPos, i, a.a / dt_or_rho0); return; }
-        const float3 dv = (kMode == 1) ? a.a / dt_or_rho0 : a.a;
-        const float3 v = f3(hi.x + dv.x, hi.y + dv.y, hi.z + dv.z);
+        const float3 v = velocity(a.a, hi);
         rec_set_vel(rec + i, v); store3(vel, i, v);
     }
+    // The epilogue on the +0 sum of a skipped walk (chunk activity), storing only what differs in bits from what is stored --
+    // a -0 component, a NaN payload, a velocity that differs from its record: the arrays end up as after end(), and afterwards
+    // hold a fixed point of it when the +0 sum adds +0 (quiet_adds_zero): x + 0 = x for every x but -0, and a NaN stays one.
+    __device__ void end_quiet(int i) const {
+        const float4 hi = *(rec + i).b;
+        const float3 u = load3(vel, i);
+        const float3 v = velocity(f3(0.f, 0.f, 0.f), hi);
+        if (!same_bits3(v, xyz(hi))) rec_set_vel(rec + i, v);
+        if (!same_bits3(v, u)) store3(vel, i, v);
+    }
+    bool quiet_adds_zero() const { return kMode == 0 || (std::isnormal(dt_or_rho0) && dt_or_rho0 > 0.f); }   // host: +0 / dt = +0
 };
 
 // computeDensityLambda_CUDA, PBDSolver.cu:127-168 (rho0 passed through `bool`, Q4).  Writes lambda to rec.s.
@@ -798,22 +812,53 @@ __device__ __forceinline__ bool sweep_list_particle(const DevScene& s, const Op&
 // Reach: every list entry of a particle of tile T (and every cell of its exact cell-walk fallback) is a boundary record, whose
 // scalar is 0, or lies in one of T's nine fluid windows (tile_window: the cells [cA + off - 1, cB + off + 1] around the tile's
 // cells [cA, cB]).  The list builder keeps those windows in tileWin; a tile with a particle outside the grid is unbounded.
-// true when every chunk the fluid windows of `tile` touch has chunkAct == 0 (kStamp false) / a stamp <= s.seq (kStamp true)
-template <bool kStamp>
-__device__ __forceinline__ bool reach_quiet(const DevScene& s, int tile) {
+// The fluid windows of `tile`, one per lane 0..8, loaded together (one round trip instead of one per window): lane r holds the
+// chunk words [a, b] that window r touches (b < a: empty; a count of -1 marks an unbounded tile, b = -2).
+__device__ __forceinline__ int2 tile_reach(const DevScene& s, int tile) {
     const int lane = threadIdx.x & 31;
-    const int2* w = s.tileWin + static_cast<size_t>(tile) * SPHK_TILE_WINS;
-    bool ok = true;
-#pragma unroll 1
-    for (int r = 0; r < 9; ++r) {
-        const int2 wr = w[r];
-        if (wr.y < 0) return false;                   // warp-uniform: one tile per warp
-        if (wr.y == 0) continue;
-        for (int k = (wr.x >> 5) + lane; k <= (wr.x + wr.y - 1) >> 5; k += 32)
-            ok = ok && (kStamp ? s.stamp[k] <= s.seq : s.act[k] == 0u);
-    }
-    return __all_sync(0xffffffffu, ok);
+    int2 w = make_int2(0, 0);
+    if (lane < 9) w = s.tileWin[static_cast<size_t>(tile) * SPHK_TILE_WINS + lane];
+    if (w.y < 0) return make_int2(0, -2);
+    return make_int2(w.x >> 5, w.y > 0 ? (w.x + w.y - 1) >> 5 : (w.x >> 5) - 1);
 }
+template <bool kStamp> __device__ __forceinline__ bool chunk_quiet(const DevScene& s, int k) {
+    return kStamp ? s.stamp[k] <= s.seq : s.act[k] == 0u;
+}
+// true when every chunk the fluid windows touch has chunkAct == 0 (kStamp false) / a stamp <= s.seq (kStamp true).  Lane l
+// checks chunk a + l of every window, so the nine chunk-word loads of the common case (no window spans more than 32 chunks)
+// are independent and issued together; longer windows finish in a loop.
+template <bool kStamp>
+__device__ __forceinline__ bool reach_quiet(const DevScene& s, int2 t) {
+    const unsigned int full = 0xffffffffu;
+    const int lane = threadIdx.x & 31;
+    if (__any_sync(full, t.y == -2)) return false;    // unbounded tile
+    const bool more = __any_sync(full, t.y - t.x >= 32);
+    bool ok = true;
+#pragma unroll
+    for (int r = 0; r < 9; ++r) {
+        const int a = __shfl_sync(full, t.x, r), b = __shfl_sync(full, t.y, r);
+        if (a + lane <= b) ok &= chunk_quiet<kStamp>(s, a + lane);
+    }
+    if (more) {
+#pragma unroll 1
+        for (int r = 0; r < 9; ++r) {
+            const int a = __shfl_sync(full, t.x, r), b = __shfl_sync(full, t.y, r);
+            for (int k = a + 32 + lane; k <= b; k += 32) ok &= chunk_quiet<kStamp>(s, k);
+        }
+    }
+    return __all_sync(full, ok);
+}
+
+// ---- velocity epochs: a quiet chunk's epilogue runs once per stretch of correct sweeps ----------------------------------------
+// The quiet epilogue adds +0 to every velocity (OpScalarGradient::quiet_adds_zero): after one pass through it a chunk's vel and
+// rec.b hold a fixed point, and every later pass is a no-op -- until anything else writes velocities.  The host counts in
+// velCredited the launches known to write neither vel nor rec.b (error sweeps, the scalar copy, loop control, reductions) and
+// the correct sweeps that keep the marks; an epoch is a run of marked correct sweeps over one vel array with only those in
+// between (vel_mark() unchanged).  Every marked sweep writes the mark of every chunk of its grid: a warp that walks clears it,
+// a quiet warp sets it after its pass -- also when the loop predicate skips the sweep (cleared, nothing is known of what came
+// before).  The first sweep of an epoch (trust 0) ignores the marks it finds and takes every quiet chunk through end_quiet;
+// later ones skip a quiet chunk whose mark is set.  So a mark is only trusted after the same epoch has written it: marks left
+// by an earlier epoch -- or by an earlier replay of a captured step, which repeats the same trust flags -- are never read.
 
 // one warp = one chunk of a DFSPH error or correct sweep that keeps chunk activity
 template <class Op>
@@ -821,14 +866,17 @@ __device__ __forceinline__ void sweep_list_warp(const DevScene& s, const Op& op,
     const int lane = threadIdx.x & 31, chunk = i >> 5;
     if (i - lane >= s.nF) return;                     // a whole warp past the set (patch mapping rounds the grid up)
     const bool in = in_range(s, i);
-    if (act_of<Op>::role == kActError) {
+    if constexpr (act_of<Op>::role == kActError) {
         // Reuse (s.reuse: the host's token -- the previous error sweep was of this kind with the same arrays, dt and rho0, and
         // since then no launch changed positions, densities, alpha, rec.s or these outputs, only correct sweeps moved velocities).
         // The outputs of this chunk's particles depend on their own velocity and those of their reach, nothing else that moved:
         // when no chunk of the reach was stamped since that sweep, they are what it wrote.  Own kappa quiet is required as well:
         // the density error's warm accumulate (warm += kappa) must be a no-op for a skip to be exact -- a particle with
         // kappa != 0 whose velocities did not change still accumulates.
-        if (s.reuse && s.act[chunk] == 0u && reach_quiet<true>(s, i / SPHK_BLOCK)) return;
+        if (s.reuse) {
+            const int2 t = tile_reach(s, i / SPHK_BLOCK);    // (issued with the chunk word: one round trip for both)
+            if (s.act[chunk] == 0u && reach_quiet<true>(s, t)) return;
+        }
         bool quiet = false;
         if (in) quiet = sweep_list_particle(s, op, i);
         const unsigned int act = __ballot_sync(0xffffffffu, !quiet);
@@ -836,20 +884,24 @@ __device__ __forceinline__ void sweep_list_warp(const DevScene& s, const Op& op,
     } else {
         // Every kappa in reach is -0 (boundary records: +0 after feed_pair), so every pair term is mj * (+-0) * (d * f) with a
         // finite d * f (listed pairs have r^2 <= r2list at unchanged positions): +-0, and the accumulator, starting at +0, stays
-        // +0.  The walk is skipped; the epilogue still runs on the +0 sum, so vel and rec.b get exactly what the walk would
-        // write (v + 0: -0 components become +0).  That write is not stamped: an error sweep cannot tell a +0 velocity
-        // component from a -0 one (its sum starts at +0 and only ever adds terms; a zero term of either sign leaves it unchanged).
-        if (s.act && s.act[chunk] == 0u && reach_quiet<false>(s, i / SPHK_BLOCK)) {
-            if (in) {
-                float4 lo, hi;
-                rec_full(s.rec + i, lo, hi);
-                typename Op::Acc acc;
-                op.begin(acc, i, lo, hi, s);
-                op.end(acc, i, lo, hi, s);
+        // +0.  The walk is skipped; the epilogue runs on the +0 sum (end_quiet), so vel and rec.b hold exactly what the walk
+        // would write (v + 0: -0 components become +0), or -- a marked chunk of a trusted sweep -- already hold it.  Neither
+        // is stamped: an error sweep cannot tell a +0 velocity component from a -0 one (its sum starts at +0 and only ever adds
+        // terms; a zero term of either sign leaves it unchanged).
+        if (s.act) {
+            const int2 t = tile_reach(s, i / SPHK_BLOCK);
+            const bool marked = s.mark && s.trust && s.mark[chunk] != 0;
+            if (s.act[chunk] == 0u && reach_quiet<false>(s, t)) {
+                if (marked) return;
+                if (in) op.end_quiet(i);
+                if (lane == 0 && s.mark) s.mark[chunk] = 1;
+                return;
             }
-            return;
         }
-        if (lane == 0) s.stamp[chunk] = s.seq;          // (before the walk: nothing of this stays live across it)
+        if (lane == 0) {                               // (before the walk: nothing of this stays live across it)
+            s.stamp[chunk] = s.seq;
+            if (s.mark) s.mark[chunk] = 0;
+        }
         if (in) sweep_list_particle(s, op, i);
     }
 }
@@ -875,8 +927,13 @@ __global__ void __launch_bounds__(SPHK_BLOCK) k_sweep_list(const DevScene s, con
 // the DFSPH error and correct sweeps when they keep chunk activity (a kernel of its own: the plain walk keeps its registers)
 template <class Op>
 __global__ void __launch_bounds__(SPHK_BLOCK) k_sweep_list_act(const DevScene s, const Op op) {
-    if (s.pred && *s.pred == 0) return;
-    sweep_list_warp(s, op, list_thread(s));
+    const int i = list_thread(s);
+    if (s.pred && *s.pred == 0) {
+        // a skipped correct sweep still writes its marks (velocity epochs): cleared
+        if (act_of<Op>::role == kActCorrect && s.mark && (threadIdx.x & 31) == 0 && i < s.nF) s.mark[i >> 5] = 0;
+        return;
+    }
+    sweep_list_warp(s, op, i);
 }
 
 // =================================================================================================
@@ -1468,6 +1525,7 @@ static DevScene dev_scene(const sphk_ctx* c, const sphk_scene* s) {
     d.r2list = d.k.r2cut;
     d.cellFlag = nullptr;
     d.act = nullptr; d.stamp = nullptr; d.seq = 0; d.reuse = 0;
+    d.mark = nullptr; d.trust = 0;
     return d;
 }
 
@@ -1477,6 +1535,9 @@ static DevScene dev_scene(const sphk_ctx* c, const sphk_scene* s) {
 // last error sweep's outputs stay reusable, until anything else is launched.  Host-side only: a captured step repeats the order
 // of its calls and with it these decisions; what depends on data (which chunks are quiet) is decided on the device.
 static long long act_mark(const sphk_ctx* c) { return c->launches - c->credited; }
+// Velocity epochs (sweep_list_warp) in the same pattern: vel_mark() stays put across the launches that leave vel and rec.b alone
+// and across the correct sweeps that keep the marks; anything else -- a launch, or a copy over the velocities -- ends the epoch.
+static long long vel_mark(const sphk_ctx* c) { return c->launches - c->velCredited; }
 static bool same_bits(float a, float b) { unsigned int x, y; std::memcpy(&x, &a, 4); std::memcpy(&y, &b, 4); return x == y; }
 
 SkinTrack sphk_skin_track(const sphk_ctx* c, float radius, bool on) {
@@ -1569,6 +1630,12 @@ template <class Op> static int run_sweep(sphk_ctx* c, const sphk_scene* s, const
                     d.stamp = c->chunkStamp;
                     d.seq = ++c->corrSeq;
                     if (c->actMark == act_mark(c)) d.act = c->chunkAct;
+                    if constexpr (role == kActCorrect) {
+                        if (op.quiet_adds_zero()) {   // else: a quiet pass is no fixed point of the others -- no marks, the epoch ends
+                            d.mark = c->chunkMark;
+                            d.trust = c->velMark == vel_mark(c) && c->velArr == s->fluid.vel;
+                        }
+                    }
                 }
             }
             int blocks = sphk_blocks(d.iEnd - d.iBegin);
@@ -1584,6 +1651,8 @@ template <class Op> static int run_sweep(sphk_ctx* c, const sphk_scene* s, const
     }
     c->launches++;
     if (role == kActCorrect) c->credited++;           // velocities only; stamped, or the caller drops the token
+    if (role == kActError || d.mark) c->velCredited++;   // the error sweeps write no velocity; a marked correct sweep keeps its marks
+    if (d.mark) { c->velMark = vel_mark(c); c->velArr = s->fluid.vel; }
     SPHK_CUDA_TRY(cudaGetLastError());
     return SPHK_OK;
 }
@@ -1609,7 +1678,7 @@ static bool error_reusable(const sphk_ctx* c, int kind, const sphk_scene* s, con
 static void ensure_scalar(sphk_ctx* c, const float* array) {
     if (c->sTag == array) return;
     k_s_copy<<<sphk_blocks(c->nF), SPHK_BLOCK, 0, c->stream>>>(array, c->rec, c->nF, c->chunkAct);
-    c->launches++;
+    c->launches++; c->velCredited++;
     c->actMark = act_mark(c);
     c->sTag = array;
 }
