@@ -20,6 +20,10 @@
 // --probe-out FILE (required with them) gets a CSV row per step: step,t, then each probe's S,rho,vx,vy,vz,p,T,n, then each gauge's
 // level (-1: dry).  The device ring is drained after every frame (sized for a frame's largest substep count with --cfl).  At most
 // 4096 probes and 64 gauges; single GPU only.
+// --checkpoint FILE [--checkpoint-every K] saves the state (SPHSystem::checkpoint, DESIGN.md section 2.14) after every K-th frame
+// (K = 0, the default: none before the last) and after the last frame; the file is written behind the following frames.
+// --resume FILE restores such a file into the system the same scene and setting flags build and continues from its frame to
+// --frames; with --probe-out the rows of the resumed frames are appended to the CSV.  Single GPU only; not with --bullets.
 // --obstacle, --mesh-body and --fluid-mesh build the scene from Wavefront OBJ meshes (sphb200::loadObj, DESIGN.md section 2.12), each
 // mapped by S * v + (X, Y, Z) (default 1 and 0).  --obstacle (repeatable) is a static obstacle: its surface sampled at the boundary
 // spacing (sphb200::sampleSurface) is appended to the boundary set after the tank shell, so it has the walls' adhesion and
@@ -139,6 +143,8 @@ struct Options {
     std::string meshBody, fluidMesh;          // --mesh-body FILE,REL[,S,X,Y,Z], --fluid-mesh FILE[,S,X,Y,Z]
     std::vector<std::string> probes, gauges;  // --probe X,Y,Z and --gauge AX,AY,AZ,BX,BY,BZ[,K] (repeatable)
     std::string gaugeThreshold, probeOut;     // --gauge-threshold THETA, --probe-out FILE
+    std::string checkpoint, resume;           // --checkpoint FILE, --resume FILE
+    int checkpointEvery = 0;                  // --checkpoint-every K (frames; 0: after the last frame only)
 };
 
 // --rheology MODEL:a,b,c[,d] -> the model (not yet checked against its ranges: setRheology does that)
@@ -341,6 +347,13 @@ bool parse(int argc, char** argv, Options& o) {
         else if (a == "--gauge" && need(i, 1)) o.gauges.push_back(argv[++i]);
         else if (a == "--gauge-threshold" && need(i, 1)) o.gaugeThreshold = argv[++i];
         else if (a == "--probe-out" && need(i, 1)) o.probeOut = argv[++i];
+        else if (a == "--checkpoint" && need(i, 1)) o.checkpoint = argv[++i];
+        else if (a == "--resume" && need(i, 1)) o.resume = argv[++i];
+        else if (a == "--checkpoint-every" && need(i, 1)) {
+            char* end = nullptr;
+            const long k = std::strtol(argv[++i], &end, 10);
+            o.checkpointEvery = (end && *end == 0 && k >= 0 && k <= 1000000000L) ? static_cast<int>(k) : -1;
+        }
         else if (a == "--block" && need(i, 3)) { for (int k = 0; k < 3; ++k) o.block[k] = std::atoi(argv[++i]); }
         else if (a == "--origin" && need(i, 3)) { for (int k = 0; k < 3; ++k) o.origin[k] = static_cast<float>(std::atof(argv[++i])); }
         else if (a == "--box" && need(i, 1)) {
@@ -436,6 +449,13 @@ bool parse(int argc, char** argv, Options& o) {
     if ((!o.obstacles.empty() || !o.meshBody.empty() || !o.fluidMesh.empty()) && o.ranks > 1) {
         std::fprintf(stderr, "sph_headless: --obstacle, --mesh-body and --fluid-mesh run on one GPU only (not with --ranks)\n");
         return false;
+    }
+    if (!o.checkpoint.empty() || !o.resume.empty() || o.checkpointEvery != 0) {
+        if (o.checkpointEvery < 0 || (o.checkpointEvery > 0 && o.checkpoint.empty()) || o.ranks > 1 || o.bullets > 0 || o.frames < 0) {
+            std::fprintf(stderr, "sph_headless: --checkpoint FILE, --checkpoint-every K (an integer >= 0, with --checkpoint) and --resume FILE "
+                                 "run on one GPU only (not with --ranks) and not with --bullets\n");
+            return false;
+        }
     }
     if (!o.probes.empty() || !o.gauges.empty() || !o.gaugeThreshold.empty() || !o.probeOut.empty()) {
         sphb200::Probes p;
@@ -635,7 +655,7 @@ int main(int argc, char** argv) {
                              "[--rheology-max NU_MAX] [--no-slip]] [--heat ALPHA,BETA[,TREF] [--heater T] [--wall-temp T[,H]] "
                              "[--tap-temp T] [--thermal-viscosity NUREF,E[,NUMAX]]] [--adhesion BETA[,BODYBETA]] [--obstacle FILE[,S,X,Y,Z]]... "
                              "[--mesh-body FILE,REL[,S,X,Y,Z]] [--fluid-mesh FILE[,S,X,Y,Z]] [--dump PREFIX] [--quiet] "
-                             "[--emit-scene PREFIX] "
+                             "[--emit-scene PREFIX] [--checkpoint FILE [--checkpoint-every K]] [--resume FILE] "
                              "[--ranks N [--rank R --rendezvous DIR]]\n");
         return 2;
     }
@@ -846,15 +866,42 @@ int main(int argc, char** argv) {
         const double dtMin = o.dtMin > 0.0f ? o.dtMin : dt / 64.0;
         p.capacity = o.cfl > 0.0f ? static_cast<int>(std::min(65536.0, std::ceil(dt / dtMin) + 2.0)) : 1;
         if (!pSystem->setProbes(p)) { std::fprintf(stderr, "sph_headless: --probe / --gauge were refused\n"); return 4; }
-        probeCsv = std::fopen(o.probeOut.c_str(), "w");
+        // a resumed run appends the rows of its frames to the CSV of the run it continues
+        probeCsv = std::fopen(o.probeOut.c_str(), o.resume.empty() ? "w" : "a");
         if (!probeCsv) { std::fprintf(stderr, "sph_headless: cannot write --probe-out %s\n", o.probeOut.c_str()); return 5; }
         static const char* kFields[SPHK_PROBE_FIELDS] = {"S", "rho", "vx", "vy", "vz", "p", "T", "n"};
-        std::fprintf(probeCsv, "step,t");
-        for (size_t k = 0; k < p.points.size(); ++k)
-            for (const char* f : kFields) std::fprintf(probeCsv, ",p%zu_%s", k, f);
-        for (size_t k = 0; k < p.gauges.size(); ++k) std::fprintf(probeCsv, ",g%zu_level", k);
-        std::fprintf(probeCsv, "\n");
+        if (o.resume.empty()) {
+            std::fprintf(probeCsv, "step,t");
+            for (size_t k = 0; k < p.points.size(); ++k)
+                for (const char* f : kFields) std::fprintf(probeCsv, ",p%zu_%s", k, f);
+            for (size_t k = 0; k < p.gauges.size(); ++k) std::fprintf(probeCsv, ",g%zu_level", k);
+            std::fprintf(probeCsv, "\n");
+        }
     }
+    // --resume: the state and the frame index (the user section: a little-endian int64)
+    int resumedFrom = -1, checkpointsWritten = 0;
+    if (!o.resume.empty()) {
+        std::vector<unsigned char> user;
+        long long frame = -1;
+        if (!pSystem->restore(o.resume, &user) || user.size() != sizeof(frame)) {
+            std::fprintf(stderr, "sph_headless: --resume %s was refused\n", o.resume.c_str());
+            return 4;
+        }
+        std::memcpy(&frame, user.data(), sizeof(frame));
+        if (frame < 0 || frame > o.frames) {
+            std::fprintf(stderr, "sph_headless: --resume %s holds frame %lld, outside [0, --frames %d]\n", o.resume.c_str(), frame, o.frames);
+            return 4;
+        }
+        resumedFrom = static_cast<int>(frame);
+    }
+    auto saveCheckpoint = [&](int frame) {
+        const long long f = frame;
+        std::vector<unsigned char> user(sizeof(f));
+        std::memcpy(user.data(), &f, sizeof(f));
+        if (!pSystem->checkpoint(o.checkpoint, user)) return false;
+        ++checkpointsWritten;
+        return true;
+    };
     // the rows recorded since the last drain, one CSV line per step (floats with 9 significant digits: the float32 bits round-trip)
     auto drainProbes = [&]() {
         if (!probeCsv) return;
@@ -878,7 +925,8 @@ int main(int argc, char** argv) {
     }
 
     // ---- oneStep(), main.cpp:300-306 ----
-    int frameId = 0, straysRouted = 0;
+    int frameId = resumedFrom > 0 ? resumedFrom : 0, straysRouted = 0;
+    const int firstFrame = frameId;
     float totalTime = 0.0f, worst = 0.0f;
     std::string substepsJson;
     for (; frameId < o.frames;) {
@@ -905,6 +953,11 @@ int main(int argc, char** argv) {
         }
         if (slab && o.bullets > 0) straysRouted += pSlab->straysRouted();
         drainProbes();
+        if (!o.checkpoint.empty() && ((o.checkpointEvery > 0 && frameId % o.checkpointEvery == 0) || frameId == o.frames) &&
+            !saveCheckpoint(frameId)) {
+            std::fprintf(stderr, "sph_headless: --checkpoint %s was refused\n", o.checkpoint.c_str());
+            return 4;
+        }
         totalTime += milliseconds;
         worst = milliseconds > worst ? milliseconds : worst;
         if (!o.quiet && !o.heat.empty()) {
@@ -924,7 +977,15 @@ int main(int argc, char** argv) {
         }
         if (!o.quiet)
             std::printf("Frame %d - %2.2f ms, avg time - %2.2f ms/frame (%3.2f FPS)\r", frameId % 10000, milliseconds,
-                        totalTime / float(frameId), float(frameId) * 1000.0f / totalTime);
+                        totalTime / float(frameId - firstFrame), float(frameId - firstFrame) * 1000.0f / totalTime);
+    }
+    if (!o.checkpoint.empty() && frameId == firstFrame && !saveCheckpoint(frameId)) {      // (no frame ran: the state as built)
+        std::fprintf(stderr, "sph_headless: --checkpoint %s was refused\n", o.checkpoint.c_str());
+        return 4;
+    }
+    if (!o.checkpoint.empty() && !pSystem->waitCheckpoint()) {
+        std::fprintf(stderr, "sph_headless: writing --checkpoint %s failed\n", o.checkpoint.c_str());
+        return 5;
     }
     if (!o.quiet) std::printf("\n");
     if (probeCsv && std::fclose(probeCsv) != 0) { std::fprintf(stderr, "sph_headless: writing --probe-out %s failed\n", o.probeOut.c_str()); return 5; }
@@ -956,7 +1017,7 @@ int main(int argc, char** argv) {
         ok = ok && write_floats(o.dump + ".pos.f32", pos) && write_floats(o.dump + ".rgb.f32", col) && write_floats(o.dump + ".density.f32", den);
         if (!ok) { std::fprintf(stderr, "sph_headless: dump to '%s.*' failed\n", o.dump.c_str()); return 5; }
     }
-    const float avg = frameId ? totalTime / float(frameId) : 0.0f;
+    const float avg = frameId > firstFrame ? totalTime / float(frameId - firstFrame) : 0.0f;
     if (slab) {
         std::printf("{\"solver\": \"%s\", \"rank\": %d, \"ranks\": %d, \"n_fluid\": %d, \"n_owned\": %d, \"halo\": \"%s\", \"strays_routed\": %d, \"dt\": %g, "
                     "\"frames\": %d, \"avg_ms_per_frame\": %.4f, \"max_ms_per_frame\": %.4f}\n",
@@ -965,6 +1026,8 @@ int main(int argc, char** argv) {
         return 0;
     }
     std::string openJson;
+    if (!o.checkpoint.empty() || !o.resume.empty())
+        openJson += ", \"resumed_from_frame\": " + std::to_string(resumedFrom) + ", \"checkpoints_written\": " + std::to_string(checkpointsWritten);
     if (o.cfl > 0.0f) {
         const sphb200::AdaptiveStats st = pSystem->adaptiveStats();
         char buf[160];

@@ -44,6 +44,9 @@ SPHK_FUNCTIONS = [
     "sphk_mesh_transform", "sphk_mesh_properties", "sphk_mesh_create", "sphk_mesh_destroy", "sphk_mesh_classify", "sphk_mesh_fill",
     "sphk_mesh_sample_surface", "sphk_probe_sample", "sphk_probe_lattice", "sphk_gauge_levels", "sphk_probe_series_create",
     "sphk_probe_series_destroy", "sphk_probes_record", "sphk_probe_series_read",
+    "sphk_state_checksum_host", "sphk_state_crc32_host", "sphk_state_checksum_device", "sphk_checkpoint_save", "sphk_checkpoint_wait",
+    "sphk_checkpoint_release", "sphk_state_open", "sphk_state_close", "sphk_state_section_bytes", "sphk_checkpoint_load",
+    "sphk_checkpoint_invalidate",
 ]
 SPH_APP_FUNCTIONS = [
     "sph_app_create", "sph_app_destroy", "sph_app_step", "sph_app_fluid_size", "sph_app_boundary_size",
@@ -56,6 +59,7 @@ SPH_APP_FUNCTIONS = [
     "sph_app_set_thermal", "sph_app_set_thermal_viscosity", "sph_app_upload_temperature", "sph_app_download_temperature",
     "sph_app_thermal_stats", "sph_app_set_adhesion", "sph_app_adhesion_stats", "sph_app_load_obj", "sph_app_load_obj_error",
     "sph_app_set_probes", "sph_app_probe_series", "sph_app_sample_probes", "sph_app_sample_lattice",
+    "sph_app_checkpoint", "sph_app_checkpoint_wait", "sph_app_restore",
 ]
 
 BODY_LIMIT = 64                      # SPHK_BODY_LIMIT
@@ -293,6 +297,7 @@ def sphk():
         L.sphk_mg_destroy.restype = None
         L.sphk_mesh_destroy.restype = None
         L.sphk_probe_series_destroy.restype = None
+        L.sphk_state_close.restype = None
         _sphk = L
     return _sphk
 
@@ -333,6 +338,41 @@ def app_params(p) -> SphAppParams:
     q.density_error_threshold = p.density_error_threshold
     q.divergence_error_threshold = p.divergence_error_threshold
     return q
+
+
+class SphkStateConfig(C.Structure):
+    """sphk_state_config (include/sphk.h): the configuration fingerprint of a checkpoint file."""
+    _fields_ = [("solver", C.c_char * 16), ("capacity_fluid", C.c_int), ("capacity_boundary", C.c_int), ("n_boundary", C.c_int),
+                ("n_bodies", C.c_int), ("cell_size", C.c_int * 3), ("flags", C.c_int), ("space_size", C.c_float * 3),
+                ("cell_length", C.c_float), ("radius", C.c_float), ("dt", C.c_float), ("m0", C.c_float), ("rho0", C.c_float),
+                ("rho_boundary", C.c_float), ("stiff", C.c_float), ("visc", C.c_float), ("surface_tension", C.c_float),
+                ("air_pressure", C.c_float), ("gravity", C.c_float * 3), ("solver_args", C.c_float * 4),
+                ("bodies_hash", C.c_ulonglong), ("open_hash", C.c_ulonglong), ("settings_hash", C.c_ulonglong)]
+
+
+class SphkStateSection(C.Structure):
+    """sphk_state_section (include/sphk.h): one named range of device (host = 0) or host (host = 1) memory."""
+    _fields_ = [("name", C.c_char * 32), ("ptr", C.c_void_p), ("bytes", C.c_ulonglong), ("elem_size", C.c_uint), ("host", C.c_int)]
+
+
+def state_hash(data: bytes) -> int:
+    """sphk_state_checksum_host of host bytes"""
+    buf = C.create_string_buffer(bytes(data), max(1, len(data)))
+    h = C.c_ulonglong(0)
+    check(sphk().sphk_state_checksum_host(buf, C.c_ulonglong(len(data)), C.byref(h)), "sphk_state_checksum_host")
+    return int(h.value)
+
+
+def state_user_bytes(path: str) -> int:
+    """the size of a checkpoint file's user section (0 when the file cannot be read: the restore itself reports why)"""
+    L = sphk()
+    f, nb = C.c_void_p(), C.c_ulonglong(0)
+    if L.sphk_state_open(os.fsencode(path), C.byref(f), None, C.c_int(0)):
+        return 0
+    try:
+        return int(nb.value) if L.sphk_state_section_bytes(f, b"user", C.byref(nb)) == 0 else 0
+    finally:
+        L.sphk_state_close(f)
 
 
 class SphApp:
@@ -602,6 +642,28 @@ class SphApp:
                                          out.ctypes.data_as(C.c_void_p)):
             raise RuntimeError("sph_app_sample_lattice failed (reference engine or a refused call)")
         return out
+
+    def checkpoint(self, path: str, user: bytes = b""):
+        """Snapshot the state into `path` (SPHSystem::checkpoint; DESIGN.md section 2.14).  Returns once the snapshot is enqueued; the
+        file is written behind the following steps (checkpoint_wait).  Not on the reference engine."""
+        u = bytes(user)
+        if self.L.sph_app_checkpoint(self.h, os.fsencode(path), u if u else None, C.c_int(len(u))):
+            raise RuntimeError("sph_app_checkpoint refused (reference engine or a solver that does not describe its state)")
+
+    def checkpoint_wait(self):
+        """Wait for the last checkpoint's file; raises when it could not be written."""
+        if self.L.sph_app_checkpoint_wait(self.h):
+            raise RuntimeError("sph_app_checkpoint_wait: the checkpoint failed (see the printed message)")
+
+    def restore(self, path: str) -> bytes:
+        """Overwrite the state from a checkpoint of a system with the same configuration; returns the stored user bytes.  A refused
+        restore (printed reason) changes nothing and raises."""
+        nb = C.c_int(0)
+        buf = C.create_string_buffer(max(1, state_user_bytes(path)))
+        if self.L.sph_app_restore(self.h, os.fsencode(path), buf, C.c_int(len(buf)), C.byref(nb)):
+            raise RuntimeError("sph_app_restore refused (see the printed message)")
+        self.nF = self.fluid_count
+        return buf.raw[:nb.value]
 
     def thermal_stats(self) -> dict:
         """substeps, max_courant, violators of the last step; t_min, t_max, heat (sum m T) now"""

@@ -170,6 +170,8 @@ struct sphk_ctx {
     unsigned int* speedDev = nullptr;     // device [3]: {fluid max |v|^2, body max bound (float bits), non-finite count}
     unsigned int* speedPinned = nullptr;  // pinned [3]: their copy
     cudaEvent_t speedEvent = nullptr;     // recorded after that copy
+    // checkpoints (sphk_state.cu; allocated at the first save or load)
+    struct StateStage* state = nullptr;
 };
 
 struct DevScene {

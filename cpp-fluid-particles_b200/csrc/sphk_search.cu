@@ -250,6 +250,7 @@ extern "C" int sphk_create(sphk_ctx** out, int max_fluid, int max_boundary, cons
 
 extern "C" void sphk_destroy(sphk_ctx* c) {
     if (!c) return;
+    sphk_checkpoint_release(c);
     cudaFree(c->keys); cudaFree(c->keysSorted); cudaFree(c->idx); cudaFree(c->idxSorted);
     cudaFree(c->snapA); cudaFree(c->snapB); cudaFree(c->rec.a); cudaFree(c->rec.b); cudaFree(c->massRange); cudaFree(c->dispMax); cudaFree(c->cellFlag);
     cudaFree(c->tmpF); cudaFree(c->partial); cudaFree(c->loops); cudaFree(c->viscStats); cudaFree(c->rheoStats); cudaFree(c->heatGroups); cudaFree(c->heatStats); cudaFree(c->heatRed); cudaFree(c->adhGroups); cudaFree(c->adhStats); cudaFree(c->cnt); cudaFree(c->nbr); cudaFree(c->cubTemp); cudaFree(c->tileWin); cudaFree(c->chunkAct); cudaFree(c->chunkStamp); cudaFree(c->chunkMark);

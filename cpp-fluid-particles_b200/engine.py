@@ -10,6 +10,8 @@ between the C-ABI calls.
 from __future__ import annotations
 
 import ctypes as C
+import os
+import struct
 
 import numpy as np
 import torch
@@ -1145,6 +1147,7 @@ class SphkSystem(SphkOps):
                                           self._body_begin, fp(self._body_local), fp(self._body_pose), fp(self.body_motion)),
                   "sphk_bodies_init")
             mi = capi.body_mass_inertia(bodies)
+            self._body_mi = mi
             if (mi[:, 0] > 0).any():     # as SPHSystem: held bodies (mass 0) then report their reaction too
                 check(self.L.sphk_bodies_set_dynamics(self.ctx, fp(mi), self._space), "sphk_bodies_set_dynamics")
                 self.bodies_dynamic = True
@@ -1157,6 +1160,169 @@ class SphkSystem(SphkOps):
             self.step()
         if adaptive is not None:
             self.set_adaptive(adaptive["C"], adaptive.get("dt_min", 0.0), adaptive.get("dt_max", 0.0))
+
+    # ---- checkpoints (DESIGN.md section 2.14): the class layer's sections, names and config record ---------------------------------
+    _STATE_RECORD = struct.Struct("<6qd4f2i")          # SPHSystem::StateRecord
+
+    def _state_config(self) -> capi.SphkStateConfig:
+        f32 = lambda x: float(np.float32(x))  # noqa: E731
+        c = capi.SphkStateConfig()
+        p = self.p
+        c.solver = {"wcsph": b"wcsph", "dfsph": b"dfsph", "pbd": b"pbd"}[self.solver]
+        c.capacity_fluid, c.capacity_boundary = self.fluid.pos.shape[0], self.boundary.n
+        c.n_boundary, c.n_bodies = self.boundary.n, self.n_bodies
+        c.cell_size[:] = [int(x) for x in p.cell_size]
+        c.flags = (1 if self.fused else 0) | (2 if self.solver == "dfsph" else 0) | (4 if self.open else 0) | \
+            (8 if self.bodies_dynamic else 0) | (16 if getattr(self, "adaptive", False) else 0)
+        c.space_size[:] = [f32(x) for x in p.space]
+        c.cell_length, c.radius, c.dt, c.m0, c.rho0 = p.cell_length, p.radius, p.dt, p.m0, p.rho0
+        c.rho_boundary, c.stiff, c.visc, c.surface_tension, c.air_pressure = p.rho_boundary, p.stiff, p.visc, p.surface_tension, p.air_pressure
+        c.gravity[:] = [f32(x) for x in p.gravity]
+        if self.solver == "dfsph":
+            c.solver_args[:] = [self.den_thr, self.div_thr, float(self.max_iter), 0.0]
+        elif self.solver == "pbd":
+            c.solver_args[:] = [float(self.max_iter), self.xsph_c, self.relaxation, 0.0]
+        M = (1 << 64) - 1
+        if self.n_bodies:
+            local = np.ascontiguousarray(self._body_local, np.float32).tobytes()
+            mi = np.ascontiguousarray(self._body_mi, np.float32).tobytes()
+            c.bodies_hash = (capi.state_hash(local) * 31 + capi.state_hash(mi) + int(self._body_begin[0])) & M
+        if self.open:
+            em = b"".join(bytes(e) for e in self._emitters)
+            c.open_hash = (capi.state_hash(em) * 31 + capi.state_hash(self._sinks.astype(np.float32).tobytes()) + len(self._emitters)) & M
+        f, i, b = (lambda x: struct.pack("<f", x)), (lambda x: struct.pack("<i", int(x))), (lambda x: struct.pack("<?", bool(x)))
+        st = f(self.vorticity_eps)
+        if self.implicit_nu > 0.0:
+            st += f(self.implicit_nu) + f(self.implicit_nu_boundary) + f(self.implicit_tol) + i(self.implicit_max_iter)
+        st += b(self._rheology is not None)
+        if self._rheology is not None:
+            o = dict(capi.RHEOLOGY_SOLVE_DEFAULTS, **{k: self._rheology[k] for k in capi.RHEOLOGY_SOLVE_DEFAULTS if k in self._rheology})
+            st += bytes(capi.rheology(self._rheology)) + f(o["beta"]) + f(o["tol"]) + i(o["max_iter"])
+        st += b(self._thermal is not None)
+        if self._thermal is not None:
+            st += bytes(self._thermal_abi) + b"".join(f(t) for t in self._thermal.get("emitters", ()))
+            st += b(self._thermal_viscosity is not None)
+            if self._thermal_viscosity is not None:
+                v = capi.viscosity_law(self._thermal_viscosity, 0.0)
+                o = dict(capi.THERMAL_VISCOSITY_DEFAULTS, **{k: self._thermal_viscosity[k] for k in capi.THERMAL_VISCOSITY_DEFAULTS
+                                                             if k in self._thermal_viscosity})
+                st += f(v.nu_ref) + f(v.e) + f(v.nu_min) + f(v.nu_max) + f(o["wall_factor"]) + f(o["tol"]) + i(o["max_iter"])
+        st += b(self._adhesion is not None)
+        if self._adhesion is not None:
+            st += bytes(self._adhesion_abi)
+        if getattr(self, "adaptive", False):
+            st += bytes(self._rule)
+        c.settings_hash = (capi.state_hash(st) + len(st)) & M
+        return c
+
+    def _state_sections(self, n: int, rec, carry, motion, user):
+        """the class layer's sections in its order (SPHSystem::stateSections); host sections point at the given ctypes buffers"""
+        out = []
+
+        def add(name, ptr, nbytes, elem, host=False):
+            s = capi.SphkStateSection()
+            s.name, s.ptr, s.bytes, s.elem_size, s.host = name.encode(), ptr, nbytes, elem, int(host)
+            out.append(s)
+        fl, bd = self.fluid, self.boundary
+        add("fluid.pos", _ptr(fl.pos), 12 * n, 12)
+        add("fluid.vel", _ptr(fl.vel), 12 * n, 12)
+        add("fluid.mass", _ptr(fl.mass), 4 * n, 4)
+        add("fluid.density", _ptr(fl.density), 4 * n, 4)
+        add("fluid.pressure", _ptr(fl.pressure), 4 * n, 4)
+        add("fluid.particle2cell", _ptr(fl.p2c), 4 * n, 4)
+        add("boundary.pos", _ptr(bd.pos), 12 * bd.n, 12)
+        add("boundary.mass", _ptr(bd.mass), 4 * bd.n, 4)
+        if self._thermal is not None:
+            add("solver.temperature", _ptr(self.temperature), 4 * n, 4)
+            add("solver.temperature_set", C.addressof(self._state_tset), 1, 1, True)
+        if self.solver == "dfsph":
+            add("solver.dfsph_warm_stiffness", _ptr(self.warm), 4 * n, 4)
+        if self.solver == "pbd":
+            add("solver.pbd_pos_last", _ptr(self.pos_last), 12 * n, 12)
+            add("solver.pbd_last_predict_dt", C.addressof(self._state_pdt), 4, 4, True)
+            add("solver.pbd_pos_last_initialized", C.addressof(self._state_pinit), 1, 1, True)
+        add("system.record", C.addressof(rec), len(rec), 8, True)
+        if self.open:
+            add("system.emitter_carry", C.addressof(carry), C.sizeof(carry), 8, True)
+        if self.n_bodies:
+            add("system.body_motion", C.addressof(motion), C.sizeof(motion), 4, True)
+        add("user", C.addressof(user) if len(user) else None, len(user), 1, True)
+        return (capi.SphkStateSection * max(1, len(out)))(*out), len(out)
+
+    def save_state(self, path: str, user: bytes = b""):
+        """SPHSystem::checkpoint: the same library entries, sections and config record, so the file restores in any layer.  Returns
+        once the snapshot is enqueued; wait_state() waits for the file."""
+        n = self.fluid.n
+        st = getattr(self, "adaptive_stats", None) or {"speed": 0.0, "source": 0, "min_clamps": 0, "nonfinite_steps": 0, "frame_min_dt": 0.0}
+        o = self._open_stats
+        rec = C.create_string_buffer(self._STATE_RECORD.pack(
+            self.steps_run, o["emitted"], o["removed"], o["refused"], st["min_clamps"], st["nonfinite_steps"], self.simulated_time,
+            self.last_dt, self.dt, st["speed"], st["frame_min_dt"], st["source"], n), self._STATE_RECORD.size)
+        carry = (C.c_double * max(1, len(self.emitter_carry)))(*self.emitter_carry)
+        motion = (C.c_float * max(1, 6 * self.n_bodies))(*(np.asarray(self.body_motion, np.float32).reshape(-1) if self.n_bodies else [0.0]))
+        u = C.create_string_buffer(bytes(user), max(1, len(user)))
+        self._state_tset = C.c_bool(self._thermal is not None)
+        self._state_pdt = C.c_float(self.pbd_last_dt or 0.0)
+        self._state_pinit = C.c_bool(bool(getattr(self, "pos_last_init", False)))
+        secs, k = self._state_sections(n, rec, carry, motion, u if len(user) else b"")
+        cfg = self._state_config()
+        check(self.L.sphk_checkpoint_save(self.ctx, os.fsencode(path), C.byref(cfg), secs, C.c_int(k)), "sphk_checkpoint_save")
+
+    def wait_state(self):
+        """SPHSystem::waitCheckpoint: raises RuntimeError with the library's message when the file could not be written"""
+        msg = C.create_string_buffer(512)
+        if self.L.sphk_checkpoint_wait(self.ctx, msg, C.c_int(512)):
+            raise RuntimeError(f"checkpoint failed: {msg.value.decode()}")
+
+    def load_state(self, path: str) -> bytes:
+        """SPHSystem::restore: overwrites the state from a file of any layer (same configuration); returns the user bytes.  A refused
+        load changes nothing and raises RuntimeError naming the field or section at fault."""
+        msg = C.create_string_buffer(512)
+        self.L.sphk_checkpoint_wait(self.ctx, msg, C.c_int(512))
+        f = C.c_void_p()
+        if self.L.sphk_state_open(os.fsencode(path), C.byref(f), msg, C.c_int(512)):
+            raise RuntimeError(f"restore refused: {msg.value.decode()}")
+        try:
+            pos_b, user_b = C.c_ulonglong(0), C.c_ulonglong(0)
+            if self.L.sphk_state_section_bytes(f, b"fluid.pos", C.byref(pos_b)) or self.L.sphk_state_section_bytes(f, b"user", C.byref(user_b)):
+                raise RuntimeError("restore refused: the file has no fluid.pos or user section")
+            n = self.fluid.n
+            if self.open:
+                if pos_b.value % 12 or pos_b.value // 12 > self.fluid.pos.shape[0]:
+                    raise RuntimeError(f"restore refused: section 'fluid.pos' holds {pos_b.value} bytes, more than the capacity")
+                n = pos_b.value // 12
+            rec = C.create_string_buffer(self._STATE_RECORD.size)
+            carry = (C.c_double * max(1, len(self.emitter_carry)))()
+            motion = (C.c_float * max(1, 6 * self.n_bodies))()
+            u = C.create_string_buffer(max(1, user_b.value))
+            self._state_tset, self._state_pdt, self._state_pinit = C.c_bool(False), C.c_float(0.0), C.c_bool(False)
+            secs, k = self._state_sections(n, rec, carry, motion, u if user_b.value else b"")
+            cfg = self._state_config()
+            if self.L.sphk_checkpoint_load(self.ctx, f, C.byref(cfg), secs, C.c_int(k), msg, C.c_int(512)):
+                raise RuntimeError(f"restore refused: {msg.value.decode()}")
+        finally:
+            self.L.sphk_state_close(f)
+        (self.steps_run, e, r, x, mc, nf, self.simulated_time, last_dt, step_dt, speed, fmin, src, _live) = self._STATE_RECORD.unpack(rec.raw)
+        self.last_dt = last_dt
+        if self.open:
+            self._set_live(n)
+            self._open_stats = {"emitted": e, "removed": r, "refused": x}
+            self.emitter_carry = list(carry)[:len(self.emitter_carry)]
+        if getattr(self, "adaptive", False):
+            self.adaptive_stats = {"speed": speed, "source": src, "min_clamps": mc, "nonfinite_steps": nf, "frame_min_dt": fmin}
+        if self.n_bodies:
+            self.body_motion = np.array(motion[:], np.float32).reshape(-1, 6)
+        if self.solver == "pbd":
+            self.pbd_last_dt = self._state_pdt.value if self._state_pdt.value > 0.0 else None
+            self.pos_last_init = bool(self._state_pinit.value)
+        self.heat_substeps = 0
+        self.it_div = self.it_den = 0
+        self._scene = None
+        check(self.L.sphk_checkpoint_invalidate(self.ctx), "sphk_checkpoint_invalidate")
+        if getattr(self, "adaptive", False):
+            self.measure_speed()
+        self.synchronize()
+        return u.raw[:user_b.value]
 
     def owned(self, t):
         """the live slots of a per-particle tensor (the reductions run over the live count, as in the class layer)"""

@@ -738,6 +738,41 @@ extern "C" int sph_app_sample_lattice(sph_app* app, const float* origin, float s
 #endif
 }
 
+extern "C" int sph_app_checkpoint(sph_app* app, const char* path, const void* user, int user_bytes) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)path; (void)user; (void)user_bytes;
+    return 1;
+#else
+    if (!app || !path || user_bytes < 0 || (user_bytes > 0 && !user)) return 1;
+    const auto* u = static_cast<const unsigned char*>(user);
+    return app->system->checkpoint(path, std::vector<unsigned char>(u, u + user_bytes)) ? 0 : 1;
+#endif
+}
+
+extern "C" int sph_app_checkpoint_wait(sph_app* app) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app;
+    return 1;
+#else
+    if (!app) return 1;
+    return app->system->waitCheckpoint() ? 0 : 1;
+#endif
+}
+
+extern "C" int sph_app_restore(sph_app* app, const char* path, void* user_out, int user_cap, int* user_bytes) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)path; (void)user_out; (void)user_cap; (void)user_bytes;
+    return 1;
+#else
+    if (!app || !path || user_cap < 0) return 1;
+    std::vector<unsigned char> user;
+    if (!app->system->restore(path, &user)) return 1;
+    if (user_bytes) *user_bytes = static_cast<int>(user.size());
+    if (user_out) std::copy(user.begin(), user.begin() + std::min<size_t>(user.size(), static_cast<size_t>(user_cap)), static_cast<unsigned char*>(user_out));
+    return 0;
+#endif
+}
+
 extern "C" int sph_app_set_adaptive_dt(sph_app* app, float C, float dt_min, float dt_max) {
 #ifdef SPH_APP_REFERENCE_ENGINE
     (void)app; (void)C; (void)dt_min; (void)dt_max;

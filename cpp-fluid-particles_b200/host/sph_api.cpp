@@ -12,6 +12,13 @@
 
 using sphb200::check;
 
+// the checkpoint checksum of host bytes (the config record's hashes)
+static unsigned long long stateHash(const void* p, unsigned long long bytes) {
+    unsigned long long h = 0;
+    check(sphk_state_checksum_host(p, bytes, &h), "sphk_state_checksum_host");
+    return h;
+}
+
 // ================================================================================================
 // Engine
 // ================================================================================================
@@ -774,6 +781,10 @@ SPHSystem::SPHSystem(std::shared_ptr<SPHParticles>& fluidParticles, std::shared_
             motion.insert(motion.end(), {b.linearVelocity.x, b.linearVelocity.y, b.linearVelocity.z, b.angularVelocity.x,
                                          b.angularVelocity.y, b.angularVelocity.z});
         }
+        std::vector<float> mi;
+        for (const auto& b : bodies) mi.insert(mi.end(), {b.mass, b.inertia.x, b.inertia.y, b.inertia.z});
+        _bodiesHash = stateHash(local.data(), 4ull * local.size()) * 31u + stateHash(mi.data(), 4ull * mi.size()) +
+                      static_cast<unsigned long long>(nStatic);
         const sphk_particles bp = _boundaries->abi();
         const int rc = sphk_bodies_init(_engine->ctx(), &bp, nStatic, static_cast<int>(bodies.size()), begin.data(),
                                         local.data(), pose.data(), motion.data());
@@ -781,8 +792,6 @@ SPHSystem::SPHSystem(std::shared_ptr<SPHParticles>& fluidParticles, std::shared_
         if (rc == 0) { _bodyMotion = motion; _engine->bodies = static_cast<int>(bodies.size()); }
         const bool dynamic = std::any_of(bodies.begin(), bodies.end(), [](const sphb200::KinematicBody& b) { return b.mass > 0.0f; });
         if (rc == 0 && dynamic) {
-            std::vector<float> mi;
-            for (const auto& b : bodies) mi.insert(mi.end(), {b.mass, b.inertia.x, b.inertia.y, b.inertia.z});
             const float sp[3] = {spaceSize.x, spaceSize.y, spaceSize.z};
             const int rd = sphk_bodies_set_dynamics(_engine->ctx(), mi.data(), sp);
             check(rd, "sphk_bodies_set_dynamics");
@@ -1155,6 +1164,7 @@ float SPHSystem::runStep() {
     }
     _lastDt = _stepDt;
     _simTime += _stepDt;
+    _restored = false;
     if (_probeRecorded) {                        // the row recordProbes() enqueued: its step and time
         const size_t slot = static_cast<size_t>(_probeRows % _probes.capacity);
         _probeSteps[slot] = _steps;
@@ -1260,6 +1270,10 @@ sphb200::ProbeSeries SPHSystem::probeSeries() const {
 
 std::vector<float> SPHSystem::sampleProbes(const std::vector<float3>& points) const {
     std::vector<float> out;
+    if (_restored) {
+        printf("%s: refused until the first step after a restore (no search has run for the restored positions)\n", __func__);
+        return out;
+    }
     if (!_engine->ok() || points.empty() || fluidSize() == 0) return out;
     const size_t n = points.size();
     float *dp = nullptr, *dout = nullptr;
@@ -1283,6 +1297,10 @@ std::vector<float> SPHSystem::sampleProbes(const std::vector<float3>& points) co
 
 std::vector<float> SPHSystem::sampleLattice(float3 origin, float spacing, int3 dims) const {
     std::vector<float> out;
+    if (_restored) {
+        printf("%s: refused until the first step after a restore (no search has run for the restored positions)\n", __func__);
+        return out;
+    }
     if (!_engine->ok() || fluidSize() == 0) return out;
     const long long total = static_cast<long long>(dims.x) * dims.y * dims.z;
     if (dims.x < 1 || dims.y < 1 || dims.z < 1 || total > (1LL << 27)) {
@@ -1305,6 +1323,228 @@ std::vector<float> SPHSystem::sampleLattice(float3 origin, float spacing, int3 d
     check(sphk_synchronize(_engine->ctx()), "sphk_synchronize");
     cudaFree(dout);
     return out;
+}
+
+// ---- checkpoints (DESIGN.md section 2.14) ----
+static sphk_state_section stateSection(const char* name, const void* p, unsigned long long bytes, unsigned int elem, bool host) {
+    sphk_state_section s{};
+    std::snprintf(s.name, sizeof(s.name), "%s", name);
+    s.ptr = const_cast<void*>(p); s.bytes = bytes; s.elem_size = elem; s.host = host ? 1 : 0;
+    return s;
+}
+
+template <typename T>
+static void putBytes(std::vector<unsigned char>& v, const T& x) {
+    const auto* p = reinterpret_cast<const unsigned char*>(&x);
+    v.insert(v.end(), p, p + sizeof(T));
+}
+
+bool BasicSPHSolver::stateSections(std::vector<sphk_state_section>& out, int n) {
+    if (typeid(*this) != typeid(BasicSPHSolver)) return false;
+    commonStateSections(out, n);
+    return true;
+}
+
+void BasicSPHSolver::commonStateSections(std::vector<sphk_state_section>& out, int n) {
+    if (!thermalOn_) return;
+    out.push_back(stateSection("solver.temperature", temperatureField().addr(), 4ull * n, 4, false));
+    out.push_back(stateSection("solver.temperature_set", &temperatureSet_, sizeof(temperatureSet_), 1, true));
+}
+
+void BasicSPHSolver::stateConfig(sphk_state_config& c, std::vector<unsigned char>& settings) const {
+    commonStateConfig(c, settings, "wcsph");
+}
+
+void BasicSPHSolver::commonStateConfig(sphk_state_config& c, std::vector<unsigned char>& settings, const char* name) const {
+    std::snprintf(c.solver, sizeof(c.solver), "%s", name);
+    if (fusedSweeps_) c.flags |= 1;
+    putBytes(settings, vortEps_);
+    if (implicitViscosityOn()) { putBytes(settings, implNu_); putBytes(settings, implNuB_); putBytes(settings, implTol_); putBytes(settings, implMaxIter_); }
+    putBytes(settings, rheoOn_);
+    if (rheoOn_) {
+        putBytes(settings, static_cast<const sphk_rheology&>(rheo_));
+        putBytes(settings, rheoBeta_); putBytes(settings, rheoTol_); putBytes(settings, rheoMaxIter_);
+    }
+    putBytes(settings, thermalOn_);
+    if (thermalOn_) {
+        putBytes(settings, thermalAbi_);
+        for (float T : thermal_.emitterT) putBytes(settings, T);
+        putBytes(settings, thermalViscOn_);
+        if (thermalViscOn_) putBytes(settings, thermalVisc_);
+    }
+    putBytes(settings, adhesionOn_);
+    if (adhesionOn_) putBytes(settings, adhesionAbi_);
+}
+
+bool DFSPHSolver::stateSections(std::vector<sphk_state_section>& out, int n) {
+    commonStateSections(out, n);
+    out.push_back(stateSection("solver.dfsph_warm_stiffness", denWarmStiff.addr(), 4ull * n, 4, false));
+    return true;
+}
+
+void DFSPHSolver::stateConfig(sphk_state_config& c, std::vector<unsigned char>& settings) const {
+    commonStateConfig(c, settings, "dfsph");
+    if (deviceLoops_) c.flags |= 2;
+    c.solver_args[0] = densityErrorThreshold; c.solver_args[1] = divergenceErrorThreshold; c.solver_args[2] = static_cast<float>(maxIter);
+}
+
+bool PBDSolver::stateSections(std::vector<sphk_state_section>& out, int n) {
+    commonStateSections(out, n);
+    out.push_back(stateSection("solver.pbd_pos_last", fluidPosLast.addr(), 12ull * n, 12, false));
+    out.push_back(stateSection("solver.pbd_last_predict_dt", &lastPredictDt_, sizeof(lastPredictDt_), 4, true));
+    out.push_back(stateSection("solver.pbd_pos_last_initialized", &posLastInitialized, sizeof(posLastInitialized), 1, true));
+    return true;
+}
+
+void PBDSolver::stateConfig(sphk_state_config& c, std::vector<unsigned char>& settings) const {
+    commonStateConfig(c, settings, "pbd");
+    c.solver_args[0] = static_cast<float>(maxIter); c.solver_args[1] = xSPH_c; c.solver_args[2] = relaxation;
+}
+
+sphk_state_config SPHSystem::stateConfig() const {
+    sphk_state_config c;
+    std::memset(&c, 0, sizeof(c));
+    c.capacity_fluid = static_cast<int>(_fluids->capacity());
+    c.capacity_boundary = static_cast<int>(_boundaries->capacity());
+    c.n_boundary = boundarySize();
+    c.n_bodies = bodyCount();
+    c.cell_size[0] = _cellSize.x; c.cell_size[1] = _cellSize.y; c.cell_size[2] = _cellSize.z;
+    c.space_size[0] = _spaceSize.x; c.space_size[1] = _spaceSize.y; c.space_size[2] = _spaceSize.z;
+    c.cell_length = _sphCellLength; c.radius = _sphSmoothingRadius; c.dt = _dt; c.m0 = _sphM0; c.rho0 = _sphRho0;
+    c.rho_boundary = _sphRhoBoundary; c.stiff = _sphStiff; c.visc = _sphVisc; c.surface_tension = _sphSurfaceTensionIntensity;
+    c.air_pressure = _sphAirPressure; c.gravity[0] = _sphG.x; c.gravity[1] = _sphG.y; c.gravity[2] = _sphG.z;
+    if (_open) c.flags |= 4;
+    if (_bodiesDynamic) c.flags |= 8;
+    if (_adaptive) c.flags |= 16;
+    c.bodies_hash = _bodiesHash;
+    if (_open)
+        c.open_hash = stateHash(_emitters.data(), sizeof(sphk_emitter) * _emitters.size()) * 31u +
+                      stateHash(_sinkBoxes.data(), 4ull * _sinkBoxes.size()) + _emitters.size();
+    std::vector<unsigned char> settings;
+    if (const auto* solver = dynamic_cast<const BasicSPHSolver*>(_solver.get())) solver->stateConfig(c, settings);
+    if (_adaptive) putBytes(settings, _rule);
+    c.settings_hash = stateHash(settings.data(), settings.size()) + settings.size();
+    return c;
+}
+
+// every section of the file in its order: the fluid's n live particles, the boundary, the solver, the host counters, the user's bytes
+// (the library appends the context's body and open-boundary state)
+bool SPHSystem::stateSections(std::vector<sphk_state_section>& out, int n, StateRecord& rec, std::vector<double>& carry,
+                              std::vector<float>& motion, const std::vector<unsigned char>& user) {
+    const sphk_particles f = _fluids->abi(), b = _boundaries->abi();
+    const unsigned long long nn = static_cast<unsigned long long>(n), nb = static_cast<unsigned long long>(boundarySize());
+    out.push_back(stateSection("fluid.pos", f.pos, 12 * nn, 12, false));
+    out.push_back(stateSection("fluid.vel", f.vel, 12 * nn, 12, false));
+    out.push_back(stateSection("fluid.mass", f.mass, 4 * nn, 4, false));
+    out.push_back(stateSection("fluid.density", f.density, 4 * nn, 4, false));
+    out.push_back(stateSection("fluid.pressure", f.pressure, 4 * nn, 4, false));
+    out.push_back(stateSection("fluid.particle2cell", f.particle2cell, 4 * nn, 4, false));
+    out.push_back(stateSection("boundary.pos", b.pos, 12 * nb, 12, false));
+    out.push_back(stateSection("boundary.mass", b.mass, 4 * nb, 4, false));
+    auto* solver = dynamic_cast<BasicSPHSolver*>(_solver.get());
+    if (!solver || !solver->stateSections(out, n)) return false;
+    out.push_back(stateSection("system.record", &rec, sizeof(rec), 8, true));
+    if (_open) out.push_back(stateSection("system.emitter_carry", carry.data(), 8ull * carry.size(), 8, true));
+    if (!_bodyMotion.empty()) out.push_back(stateSection("system.body_motion", motion.data(), 4ull * motion.size(), 4, true));
+    out.push_back(stateSection("user", user.data(), user.size(), 1, true));
+    return true;
+}
+
+bool SPHSystem::checkpoint(const std::string& path, const std::vector<unsigned char>& user) {
+    if (!_engine->ok()) return false;
+    StateRecord rec;
+    std::memset(&rec, 0, sizeof(rec));
+    rec.steps = _steps; rec.emitted = _openStats.emitted; rec.removed = _openStats.removed; rec.refused = _openStats.refused;
+    rec.minClamps = _adaptiveStats.minClamps; rec.nonFiniteSteps = _adaptiveStats.nonFiniteSteps; rec.simTime = _simTime;
+    rec.lastDt = _lastDt; rec.stepDt = _stepDt; rec.speed = _adaptiveStats.speed; rec.frameMinDt = _adaptiveStats.frameMinDt;
+    rec.source = _adaptiveStats.source; rec.live = fluidSize();
+    std::vector<double> carry = _emitterCarry;
+    std::vector<float> motion = _bodyMotion;
+    std::vector<sphk_state_section> sections;
+    if (!stateSections(sections, fluidSize(), rec, carry, motion, user)) {
+        printf("SPHSystem::checkpoint: refused: the solver does not describe its state (only the shipped solvers do)\n");
+        return false;
+    }
+    const sphk_state_config cfg = stateConfig();
+    const int rc = sphk_checkpoint_save(_engine->ctx(), path.c_str(), &cfg, sections.data(), static_cast<int>(sections.size()));
+    if (rc != 0) {
+        printf("SPHSystem::checkpoint: refused (%s)\n", sphk_error_string(rc));
+        return false;
+    }
+    return true;
+}
+
+bool SPHSystem::waitCheckpoint() {
+    if (!_engine->ok()) return false;
+    char msg[512];
+    const int rc = sphk_checkpoint_wait(_engine->ctx(), msg, sizeof(msg));
+    if (rc != 0) printf("SPHSystem::waitCheckpoint: the checkpoint failed: %s\n", msg[0] ? msg : sphk_error_string(rc));
+    return rc == 0;
+}
+
+bool SPHSystem::restore(const std::string& path, std::vector<unsigned char>* user) {
+    if (!_engine->ok()) return false;
+    sphk_ctx* ctx = _engine->ctx();
+    char msg[512] = {0};
+    if (sphk_checkpoint_wait(ctx, msg, sizeof(msg)) != 0) printf("SPHSystem::restore: an earlier checkpoint failed: %s\n", msg);
+    sphk_state_file* file = nullptr;
+    if (sphk_state_open(path.c_str(), &file, msg, sizeof(msg)) != 0) {
+        printf("SPHSystem::restore: refused: %s\n", msg);
+        return false;
+    }
+    int n = fluidSize();
+    unsigned long long posBytes = 0, userBytes = 0;
+    if (sphk_state_section_bytes(file, "fluid.pos", &posBytes) != 0 || sphk_state_section_bytes(file, "user", &userBytes) != 0) {
+        printf("SPHSystem::restore: refused: the file has no fluid.pos or user section\n");
+        sphk_state_close(file);
+        return false;
+    }
+    if (_open) {                           // an open system's live count is part of its state
+        if (posBytes % 12 != 0 || posBytes / 12 > _fluids->capacity()) {
+            printf("SPHSystem::restore: refused: section 'fluid.pos' holds %llu bytes, more than the capacity of %u particles\n", posBytes,
+                   _fluids->capacity());
+            sphk_state_close(file);
+            return false;
+        }
+        n = static_cast<int>(posBytes / 12);
+    }
+    StateRecord rec;
+    std::memset(&rec, 0, sizeof(rec));
+    std::vector<double> carry(_emitterCarry.size());
+    std::vector<float> motion(_bodyMotion.size());
+    std::vector<unsigned char> userIn(static_cast<size_t>(userBytes));
+    std::vector<sphk_state_section> sections;
+    if (!stateSections(sections, n, rec, carry, motion, userIn)) {
+        printf("SPHSystem::restore: refused: the solver does not describe its state (only the shipped solvers do)\n");
+        sphk_state_close(file);
+        return false;
+    }
+    const sphk_state_config cfg = stateConfig();
+    const int rc = sphk_checkpoint_load(ctx, file, &cfg, sections.data(), static_cast<int>(sections.size()), msg, sizeof(msg));
+    sphk_state_close(file);
+    if (rc != 0) {
+        printf("SPHSystem::restore: refused: %s\n", msg[0] ? msg : sphk_error_string(rc));
+        return false;
+    }
+    // (the solver's host fields were written by the load itself)
+    if (_open) _fluids->setActiveCount(n);
+    _steps = rec.steps; _simTime = rec.simTime; _lastDt = rec.lastDt; _stepDt = rec.stepDt;
+    _openStats.emitted = rec.emitted; _openStats.removed = rec.removed; _openStats.refused = rec.refused;
+    _adaptiveStats.speed = rec.speed; _adaptiveStats.source = rec.source; _adaptiveStats.minClamps = rec.minClamps;
+    _adaptiveStats.nonFiniteSteps = rec.nonFiniteSteps; _adaptiveStats.frameMinDt = rec.frameMinDt;
+    _emitterCarry = carry;
+    _bodyMotion = motion;
+    if (user) *user = userIn;
+    // the caches derived from the old state: the next step rebuilds them
+    check(sphk_checkpoint_invalidate(ctx), "sphk_checkpoint_invalidate");
+    dropStepGraph();
+    _plainSteps = 0;
+    dynamic_cast<BasicSPHSolver*>(_solver.get())->stateRestored();
+    // the next adaptive dt: the speed bound of the restored state, measured again (a max over the same bits as the saved run's)
+    if (_adaptive) measureSpeed();
+    check(sphk_synchronize(ctx), "sphk_synchronize");
+    _restored = true;
+    return true;
 }
 
 // vbo.cu:46-51

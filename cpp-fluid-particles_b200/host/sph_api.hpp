@@ -416,6 +416,14 @@ public:
     int capacity() const { return num_; }
     // addition: the dt an emitted particle's history slot is written with when the coming step runs at dt (PBD: its last predict's)
     virtual float historyTimeStep(float dt) const { return dt; }
+    // addition: checkpoints (DESIGN.md section 2.14).  stateSections appends the solver's mutable state over its n live particles
+    // (device arrays and host fields) as checkpoint sections; false for a solver that does not describe its state (a user-derived
+    // solver), which SPHSystem then refuses to checkpoint or restore.  stateConfig writes the solver's part of the config record and
+    // appends the bytes of every setting in effect to `settings` (hashed into the record).  stateRestored runs after a restore: the
+    // last step's statistics read as zero until the next step.
+    virtual bool stateSections(std::vector<sphk_state_section>& out, int n);
+    virtual void stateConfig(sphk_state_config& c, std::vector<unsigned char>& settings) const;
+    virtual void stateRestored() { heatSubsteps_ = 0; }
     virtual ~BasicSPHSolver() noexcept {}
     virtual void step(std::shared_ptr<SPHParticles>& fluids, const std::shared_ptr<SPHParticles>& boundaries,
                       const DArray<int>& cellStartFluid, const DArray<int>& cellStartBoundary, float3 spaceSize,
@@ -471,6 +479,9 @@ protected:
     // two-way coupled bodies: the reaction of the sweep just run, with its c (sphk_bodies_react); nothing without dynamic bodies
     void react(float c) { if (reacting_) sphb200::check(sphk_bodies_react(current_.ctx, &current_.abi, c), "sphk_bodies_react"); }
     bool reacting_ = false;
+    // the sections and config every shipped solver shares (heat transfer's temperatures; the settings)
+    void commonStateSections(std::vector<sphk_state_section>& out, int n);
+    void commonStateConfig(sphk_state_config& c, std::vector<unsigned char>& settings, const char* name) const;
 private:
     DArray<float3> bufferFloat3;   // viscosity deltaV, then colour gradient (BasicSPHSolver.h:43)
     DArray<float3> bufferColorGrad;   // addition: the fused viscosity+surface sweep needs both at once
@@ -522,6 +533,9 @@ public:
         return !fieldHook_ && (deviceLoops_ || (densityErrorThreshold < 0.0f && divergenceErrorThreshold < 0.0f));
     }
     float* historyArray(int& width) override { width = 1; return denWarmStiff.addr(); }
+    bool stateSections(std::vector<sphk_state_section>& out, int n) override;
+    void stateConfig(sphk_state_config& c, std::vector<unsigned char>& settings) const override;
+    void stateRestored() override { BasicSPHSolver::stateRestored(); itDiv_ = itDen_ = 0; }
     // addition: false = the reference's host loop (one error sum read back per iteration, DFSPHSolver.cu:206,360)
     void setDeviceLoops(bool on) { if (on != deviceLoops_) ++configEpoch_; deviceLoops_ = on; }
     int lastDivergenceIterations() const { return loopIterations(0, itDiv_); }   // addition: iteration counts of the last step
@@ -568,6 +582,8 @@ public:
     bool stepIsGraphSafe() const override { return posLastInitialized && !fieldHook_; }
     float* historyArray(int& width) override { width = 3; return reinterpret_cast<float*>(fluidPosLast.addr()); }
     float historyTimeStep(float dt) const override { return lastPredictDt_ > 0.0f ? lastPredictDt_ : dt; }
+    bool stateSections(std::vector<sphk_state_section>& out, int n) override;
+    void stateConfig(sphk_state_config& c, std::vector<unsigned char>& settings) const override;
     void initializePosLast(const DArray<float3>& posFluid) {
         CUDA_CALL(cudaMemcpy(fluidPosLast.addr(), posFluid.addr(), sizeof(float3) * std::min(fluidPosLast.length(), posFluid.length()),
                              cudaMemcpyDeviceToDevice));
@@ -695,6 +711,20 @@ public:
     // ([nx][ny][nz][8]); an empty vector when refused (printed)
     std::vector<float> sampleProbes(const std::vector<float3>& points) const;
     std::vector<float> sampleLattice(float3 origin, float spacing, int3 dims) const;
+    // checkpoints (DESIGN.md section 2.14).  checkpoint(path, user) runs between steps: it enqueues the pack of the complete mutable
+    // state (fluid, boundary, solver history, bodies, open boundaries, counters, time and an opaque user section) on the step stream
+    // and returns; the copy to the host and the file write (path.tmp, fsync, rename) run behind the following steps, and a captured
+    // step graph stays captured.  waitCheckpoint() waits for that write and reports it (false and a printed message on failure).
+    // restore(path, user) overwrites the state of a system built with the same configuration (constructor arguments, solver type and
+    // arguments, bodies, emitters and sinks, settings in effect); the next step() / advance() continues where the saved run would
+    // have.  A refused restore (other configuration, bad file, checksum, a count that does not fit) changes nothing and prints the
+    // field or section at fault; it returns false.  Until the first step after a restore, sampleProbes / sampleLattice are refused
+    // (no search has run for the restored positions) and the last-step statistics read as zero.  Probe rows recorded before the
+    // restore are not in the file (drain them before checkpointing); rows recorded after it carry the saved run's step indices and
+    // times.  A user-derived solver is refused.
+    bool checkpoint(const std::string& path, const std::vector<unsigned char>& user = {});
+    bool waitCheckpoint();
+    bool restore(const std::string& path, std::vector<unsigned char>* user = nullptr);
 
 private:
     std::shared_ptr<SPHParticles> _fluids;
@@ -760,6 +790,18 @@ private:
     sphk_scene probeScene() const;
     void probeSources(const float*& pressure, const float*& temperature) const;
     void recordProbes();                  // sphk_probes_record at the end of a step (inside a captured step graph)
+    // checkpoints
+    struct StateRecord {                  // the host counters of the system (no padding: the file holds its bytes)
+        long long steps, emitted, removed, refused, minClamps, nonFiniteSteps;
+        double simTime;
+        float lastDt, stepDt, speed, frameMinDt;
+        int source, live;
+    };
+    unsigned long long _bodiesHash = 0;   // body-local points, masses and inertias (the config record)
+    bool _restored = false;               // restored, and no step since
+    sphk_state_config stateConfig() const;
+    bool stateSections(std::vector<sphk_state_section>& out, int n, StateRecord& rec, std::vector<double>& carry,
+                       std::vector<float>& motion, const std::vector<unsigned char>& user);
 };
 
 // ---- vbo.cu:46-51 --------------------------------------------------------------------------------

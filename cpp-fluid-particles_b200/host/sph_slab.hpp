@@ -47,6 +47,15 @@ public:
         printf("SlabSPHSystem: probes and gauges are not supported on slab ranks (single-GPU SPHSystem only)\n");
         return false;
     }
+    // checkpoints are single-context only (DESIGN.md section 2.14): refused, printed
+    bool checkpoint(const std::string&, const std::vector<unsigned char>& = {}) {
+        printf("SlabSPHSystem: checkpoints are not supported on slab ranks (single-GPU SPHSystem only)\n");
+        return false;
+    }
+    bool restore(const std::string&, std::vector<unsigned char>* = nullptr) {
+        printf("SlabSPHSystem: checkpoints are not supported on slab ranks (single-GPU SPHSystem only)\n");
+        return false;
+    }
     int size() const { return nOwn_; }                  // particles this rank owns
     int ownedBegin() const { return ownBegin_; }        // ... stored at [ownedBegin, ownedBegin + size) of the local set
     int globalSize() const { return nGlobal_; }

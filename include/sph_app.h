@@ -137,6 +137,15 @@ int   sph_app_probe_series(sph_app* app, int* rows, int* n_points, int* n_gauges
  * spacing (i, j, k), z fastest, into out (float[8 nx ny nz]).  1 for a refused call and on the reference build. */
 int   sph_app_sample_probes(sph_app* app, int n, const float* points_xyz, float* out);
 int   sph_app_sample_lattice(sph_app* app, const float* origin, float spacing, const int* dims, float* out);
+/* Checkpoints (SPHSystem::checkpoint / waitCheckpoint / restore; DESIGN.md section 2.14).  sph_app_checkpoint enqueues the snapshot
+ * of the state and returns; the file (path.tmp, fsync, rename) is written behind the following steps, and sph_app_checkpoint_wait
+ * reports it.  A checkpoint taken while a pipelined sph_app_submit step is in flight holds the state after that step (stream order).
+ * user: user_bytes opaque bytes stored with the state (NULL / 0: none).  sph_app_restore overwrites the state of a system built with
+ * the same configuration; user_out (capacity user_cap, may be NULL) receives the stored user bytes and *user_bytes their count.  1
+ * for a refused call (printed; a refused restore changes nothing) and on the reference build. */
+int   sph_app_checkpoint(sph_app* app, const char* path, const void* user, int user_bytes);
+int   sph_app_checkpoint_wait(sph_app* app);
+int   sph_app_restore(sph_app* app, const char* path, void* user_out, int user_cap, int* user_bytes);
 /* Kinematic rigid bodies (SPHSystem's constructor with a vector of sphb200::KinematicBody; DESIGN.md section 2.3).  No
  * reference counterpart: NULL / 1 on the reference build.  Body b is the points body_xyz[body_begin[b] .. body_begin[b+1])
  * (body coordinates; body_begin[0] = 0), pose[7 b ..] = {cx, cy, cz, qx, qy, qz, qw} (quaternion scalar part last),

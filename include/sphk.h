@@ -692,6 +692,66 @@ int sphk_probes_record(sphk_ctx* ctx, const sphk_scene* s, sphk_probe_series* se
 int sphk_probe_series_read(sphk_probe_series* series, long long* counter, int max_rows, float* records_host, float* levels_host,
                            int* rows);
 
+/* ---- checkpoints (no reference counterpart; DESIGN.md section 2.14) ------------------------------------------------------------
+ * A checkpoint file holds the mutable state of one system as named sections of bytes.  The caller lists the sections (device or
+ * host memory); the library appends the context's own body and open-boundary state ("ctx.*") and owns the format:
+ *   header  "SPHKCKPT" | u32 version | u32 sections | u64 header bytes | u64 file bytes | u64 config hash |
+ *           sphk_state_config (152 bytes) | sections x {char name[32], u64 offset, u64 bytes, u32 element size, u32 host,
+ *           u64 checksum} | u32 CRC-32 (zlib) of every header byte before it | zero padding to 16
+ *   payload every section at its (16-byte aligned) file offset, zero-padded to 16 bytes
+ * Section checksum: the bytes as little-endian u64 words w_i (the last one zero-padded), h = sum_i splitmix64(w_i + (i + 1)
+ * 0x9E3779B97F4A7C15) mod 2^64 (splitmix64's finaliser: z ^= z >> 30, z *= 0xBF58476D1CE4E5B9, z ^= z >> 27, z *= 0x94D049BB133111EB,
+ * z ^= z >> 31).  The config hash is the checksum of the config record's bytes.
+ * sphk_checkpoint_save packs the device sections into a device staging buffer in one launch on the context's stream (with their
+ * checksums), copies the host sections at once, and returns: a copy stream moves the staging buffer to pinned host memory and a host
+ * thread writes path.tmp, fsyncs and renames it to path.  The snapshot is the stream state at the call; later work on the stream
+ * overlaps the copy and the write.  A save waits for the previous one to finish first (one pinned buffer).  sphk_checkpoint_wait
+ * joins it and returns the result of the saves since the last wait (0, or the first error with its message).  The staging buffers are allocated at the first save or load and
+ * freed by sphk_checkpoint_release or sphk_destroy.
+ * Loading: sphk_state_open reads and checks a file on the host (magic, version, sizes, header CRC; no device needed).
+ * sphk_checkpoint_load then compares the config record field by field and the section table (names, order, sizes) with the
+ * system's, verifies the host checksums on the host and the device ones on the device after uploading, and only when everything
+ * passed writes the sections.  A refused call writes nothing and names the field or section at fault in msg.
+ * sphk_checkpoint_invalidate drops what the context derived from the state it had (neighbour list, search, record scalar tags,
+ * DFSPH chunk activity and velocity epochs, last-step statistics): the next step rebuilds them. */
+#define SPHK_STATE_VERSION 1
+#define SPHK_STATE_MAX_SECTIONS 64
+#define SPHK_STATE_NAME 32
+typedef struct sphk_state_config {
+    char solver[16];                 /* "wcsph", "dfsph", "pbd" */
+    int capacity_fluid, capacity_boundary, n_boundary, n_bodies;
+    int cell_size[3];
+    int flags;                       /* 1 fused sweeps, 2 device loops, 4 open boundaries, 8 dynamic bodies, 16 adaptive dt */
+    float space_size[3], cell_length, radius, dt, m0, rho0, rho_boundary, stiff, visc, surface_tension, air_pressure, gravity[3];
+    float solver_args[4];            /* DFSPH: density / divergence thresholds, max iterations; PBD: max iterations, XSPH c, relaxation */
+    unsigned long long bodies_hash;  /* body-local points, masses and inertias */
+    unsigned long long open_hash;    /* emitters and sinks */
+    unsigned long long settings_hash;/* vorticity, implicit viscosity, rheology, thermal, thermal viscosity, adhesion, adaptive rule */
+} sphk_state_config;
+typedef struct sphk_state_section {
+    char name[SPHK_STATE_NAME];
+    void* ptr;                       /* device memory (host = 0) or host memory (host = 1) */
+    unsigned long long bytes;
+    unsigned int elem_size;
+    int host;
+} sphk_state_section;
+typedef struct sphk_state_file sphk_state_file;
+int  sphk_state_checksum_host(const void* data, unsigned long long bytes, unsigned long long* out);
+int  sphk_state_crc32_host(const void* data, unsigned long long bytes, unsigned int* out);
+/* the same checksum of device memory, computed by the pack kernel (synchronises) */
+int  sphk_state_checksum_device(sphk_ctx* ctx, const void* data, unsigned long long bytes, unsigned long long* out_host);
+int  sphk_checkpoint_save(sphk_ctx* ctx, const char* path, const sphk_state_config* config, const sphk_state_section* sections,
+                          int n_sections);
+int  sphk_checkpoint_wait(sphk_ctx* ctx, char* msg, int msg_len);
+int  sphk_checkpoint_release(sphk_ctx* ctx);
+int  sphk_state_open(const char* path, sphk_state_file** file, char* msg, int msg_len);
+void sphk_state_close(sphk_state_file* file);
+/* bytes of a named section of an opened file (SPHK_ERR_INVALID: no such section) */
+int  sphk_state_section_bytes(const sphk_state_file* file, const char* name, unsigned long long* bytes);
+int  sphk_checkpoint_load(sphk_ctx* ctx, const sphk_state_file* file, const sphk_state_config* expect,
+                          const sphk_state_section* sections, int n_sections, char* msg, int msg_len);
+int  sphk_checkpoint_invalidate(sphk_ctx* ctx);
+
 /* ---- render export: generate_dots_CUDA, vbo.cu:26-44 (SURVEY 8f-2) -----------------------------------------------
  * dot[i] = pos[i]; colour[i] from density[i] (blue below 0.75, blend to white at 1.0, blend to pink above).  Plain
  * device buffers instead of a mapped GL vertex buffer; synchronises like the reference (vbo.cu:49). */
