@@ -14,6 +14,15 @@
 //                [--heat ALPHA,BETA[,TREF] [--heater T] [--wall-temp T[,H]] [--tap-temp T] [--thermal-viscosity NUREF,E[,NUMAX]]]
 //                [--adhesion BETA[,BODYBETA]] [--obstacle FILE[,S,X,Y,Z]]... [--mesh-body FILE,REL[,S,X,Y,Z]] [--fluid-mesh FILE[,S,X,Y,Z]]
 //                [--probe X,Y,Z]... [--gauge AX,AY,AZ,BX,BY,BZ[,K]]... [--gauge-threshold THETA] [--probe-out FILE]
+//                [--tank-roll DEG,HZ[,PX,PY,PZ,NX,NY,NZ]] [--tank-shake AX,AY,AZ,HZ] [--tank-accel AX,AY,AZ] [--tank-spin RAD_S]
+//                [--tank-ramp SEC]
+// --tank-roll, --tank-shake, --tank-accel and --tank-spin move the tank (SPHSystem::setTankMotion, DESIGN.md section 2.15) from the
+// step after the constructor's step 0 on; the simulation runs in the tank's frame, so every output (dump, probes, gauges) is in tank
+// coordinates.  --tank-roll rolls it by DEG degrees at HZ about the axis N through the pivot P (default: the z axis through the
+// bottom centre (L/2, 0, L/2)); --tank-spin spins it at RAD_S about the roll's axis, or without --tank-roll about the vertical axis
+// through the bottom centre; --tank-shake shakes it with the world acceleration (AX, AY, AZ) sin(2 pi HZ t) (m/s^2), --tank-accel
+// adds a constant one; --tank-ramp ramps all of it in over SEC seconds.  Every frame prints theta and a_w.  Single GPU only; not
+// with --heat.
 // --probe and --gauge (repeatable; DESIGN.md section 2.13) record SPH-interpolated fields at points and water levels along segments
 // every step after the constructor's step 0 (SPHSystem::setProbes): a gauge runs from A to B with K samples (default 64), its
 // level is its height above A (orient it upwards, along -G, from the floor), wet where the Shepard sum reaches THETA (default 0.5).
@@ -145,6 +154,8 @@ struct Options {
     std::string gaugeThreshold, probeOut;     // --gauge-threshold THETA, --probe-out FILE
     std::string checkpoint, resume;           // --checkpoint FILE, --resume FILE
     int checkpointEvery = 0;                  // --checkpoint-every K (frames; 0: after the last frame only)
+    std::string tankRoll, tankShake, tankAccel, tankSpin, tankRamp;   // --tank-* (empty: not given)
+    bool tank() const { return !(tankRoll.empty() && tankShake.empty() && tankAccel.empty() && tankSpin.empty() && tankRamp.empty()); }
 };
 
 // --rheology MODEL:a,b,c[,d] -> the model (not yet checked against its ranges: setRheology does that)
@@ -249,6 +260,41 @@ bool adhesion_of(const Options& o, bool hasBody, sphb200::Adhesion& a) {
     return true;
 }
 
+// --tank-* -> the motion in a box of size `box`; false for malformed values (the ranges are checked by setTankMotion)
+bool tank_of(const Options& o, const float box[3], sphb200::TankMotion& m) {
+    constexpr double kPi = 3.14159265358979323846;
+    m = sphb200::TankMotion();
+    m.pivot = make_float3(0.5f * box[0], 0.0f, 0.5f * box[2]);
+    m.axis = make_float3(0.0f, o.tankRoll.empty() ? 1.0f : 0.0f, o.tankRoll.empty() ? 0.0f : 1.0f);
+    std::vector<float> v;
+    if (!o.tankRoll.empty()) {
+        if (!floats_of(o.tankRoll, v) || (v.size() != 2 && v.size() != 8) || v[1] < 0.0f) return false;
+        m.rollAmplitude = static_cast<float>(v[0] * kPi / 180.0);
+        m.rollOmega = static_cast<float>(2.0 * kPi * v[1]);
+        if (v.size() == 8) { m.pivot = make_float3(v[2], v[3], v[4]); m.axis = make_float3(v[5], v[6], v[7]); }
+    }
+    if (!o.tankShake.empty()) {
+        if (!floats_of(o.tankShake, v) || v.size() != 4 || v[3] < 0.0f) return false;
+        sphb200::TankHarmonic h;
+        h.amplitude = make_float3(v[0], v[1], v[2]);
+        h.omega = static_cast<float>(2.0 * kPi * v[3]);
+        m.harmonics.push_back(h);
+    }
+    if (!o.tankAccel.empty()) {
+        if (!floats_of(o.tankAccel, v) || v.size() != 3) return false;
+        m.accel = make_float3(v[0], v[1], v[2]);
+    }
+    if (!o.tankSpin.empty()) {
+        if (!floats_of(o.tankSpin, v) || v.size() != 1) return false;
+        m.spin = v[0];
+    }
+    if (!o.tankRamp.empty()) {
+        if (!floats_of(o.tankRamp, v) || v.size() != 1 || v[0] < 0.0f) return false;
+        m.ramp = v[0];
+    }
+    return true;
+}
+
 // --probe, --gauge and --gauge-threshold -> the setting (capacity: the caller's); false for malformed or out-of-range values
 bool probes_of(const Options& o, sphb200::Probes& p) {
     p = sphb200::Probes();
@@ -331,6 +377,11 @@ bool parse(int argc, char** argv, Options& o) {
         else if (a == "--no-slip") o.noSlip = true;
         else if (a == "--heat" && need(i, 1)) o.heat = argv[++i];
         else if (a == "--adhesion" && need(i, 1)) o.adhesion = argv[++i];
+        else if (a == "--tank-roll" && need(i, 1)) o.tankRoll = argv[++i];
+        else if (a == "--tank-shake" && need(i, 1)) o.tankShake = argv[++i];
+        else if (a == "--tank-accel" && need(i, 1)) o.tankAccel = argv[++i];
+        else if (a == "--tank-spin" && need(i, 1)) o.tankSpin = argv[++i];
+        else if (a == "--tank-ramp" && need(i, 1)) o.tankRamp = argv[++i];
         else if (a == "--heater" && need(i, 1)) o.heater = argv[++i];
         else if (a == "--wall-temp" && need(i, 1)) o.wallTemp = argv[++i];
         else if (a == "--tap-temp" && need(i, 1)) o.tapTemp = argv[++i];
@@ -465,6 +516,15 @@ bool parse(int argc, char** argv, Options& o) {
                                  "(at most %d probes and %d gauges), --gauge-threshold a finite value > 0 and gauges, --probe-out a file "
                                  "and at least one probe or gauge; single GPU only (not with --ranks)\n",
                          SPHK_GAUGE_MAX_SAMPLES, SPHK_PROBE_LIMIT, SPHK_GAUGE_LIMIT);
+            return false;
+        }
+    }
+    if (o.tank()) {
+        sphb200::TankMotion m;
+        if (!tank_of(o, o.box, m) || o.ranks > 1 || !o.heat.empty()) {
+            std::fprintf(stderr, "sph_headless: --tank-roll DEG,HZ[,PX,PY,PZ,NX,NY,NZ], --tank-shake AX,AY,AZ,HZ, --tank-accel AX,AY,AZ, "
+                                 "--tank-spin RAD_S and --tank-ramp SEC need finite values (HZ, SEC >= 0); single GPU only (not with "
+                                 "--ranks) and not with --heat\n");
             return false;
         }
     }
@@ -655,6 +715,8 @@ int main(int argc, char** argv) {
                              "[--rheology-max NU_MAX] [--no-slip]] [--heat ALPHA,BETA[,TREF] [--heater T] [--wall-temp T[,H]] "
                              "[--tap-temp T] [--thermal-viscosity NUREF,E[,NUMAX]]] [--adhesion BETA[,BODYBETA]] [--obstacle FILE[,S,X,Y,Z]]... "
                              "[--mesh-body FILE,REL[,S,X,Y,Z]] [--fluid-mesh FILE[,S,X,Y,Z]] [--dump PREFIX] [--quiet] "
+                             "[--tank-roll DEG,HZ[,PX,PY,PZ,NX,NY,NZ]] [--tank-shake AX,AY,AZ,HZ] [--tank-accel AX,AY,AZ] [--tank-spin RAD_S] "
+                             "[--tank-ramp SEC] "
                              "[--emit-scene PREFIX] [--checkpoint FILE [--checkpoint-every K]] [--resume FILE] "
                              "[--ranks N [--rank R --rendezvous DIR]]\n");
         return 2;
@@ -853,6 +915,14 @@ int main(int argc, char** argv) {
             return 4;
         }
     }
+    if (o.tank()) {
+        sphb200::TankMotion m;
+        tank_of(o, o.box, m);
+        if (!pSystem->setTankMotion(m)) {
+            std::fprintf(stderr, "sph_headless: the --tank-* motion was refused\n");
+            return 4;
+        }
+    }
     if (o.cfl > 0.0f && !pSystem->setAdaptiveTimeStep(o.cfl, o.dtMin)) {
         std::fprintf(stderr, "sph_headless: --cfl %g --dt-min %g was refused\n", o.cfl, o.dtMin);
         return 4;
@@ -969,6 +1039,10 @@ int main(int argc, char** argv) {
         if (!o.quiet && !o.adhesion.empty()) {
             const sphb200::AdhesionStats as = basicSolver->lastAdhesionStats();
             std::printf("Frame %d adhesion - %d wetted particles, max acceleration %g m/s^2\n", frameId, as.wetted, as.maxAccel);
+        }
+        if (!o.quiet && o.tank()) {
+            const sphb200::TankState ts = pSystem->tankState();
+            std::printf("Frame %d tank - theta %g rad, a_w (%g, %g, %g) m/s^2\n", frameId, ts.theta, ts.accel.x, ts.accel.y, ts.accel.z);
         }
         if (!o.quiet && !o.rheology.empty()) {
             const sphb200::RheologyStats rs = basicSolver->lastRheologyStats();

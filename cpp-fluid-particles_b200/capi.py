@@ -46,7 +46,8 @@ SPHK_FUNCTIONS = [
     "sphk_probe_series_destroy", "sphk_probes_record", "sphk_probe_series_read",
     "sphk_state_checksum_host", "sphk_state_crc32_host", "sphk_state_checksum_device", "sphk_checkpoint_save", "sphk_checkpoint_wait",
     "sphk_checkpoint_release", "sphk_state_open", "sphk_state_close", "sphk_state_section_bytes", "sphk_checkpoint_load",
-    "sphk_checkpoint_invalidate",
+    "sphk_checkpoint_invalidate", "sphk_tank_eval", "sphk_tank_accel_bound", "sphk_tank_set", "sphk_tank_force", "sphk_tank_time",
+    "sphk_tank_set_time",
 ]
 SPH_APP_FUNCTIONS = [
     "sph_app_create", "sph_app_destroy", "sph_app_step", "sph_app_fluid_size", "sph_app_boundary_size",
@@ -59,7 +60,7 @@ SPH_APP_FUNCTIONS = [
     "sph_app_set_thermal", "sph_app_set_thermal_viscosity", "sph_app_upload_temperature", "sph_app_download_temperature",
     "sph_app_thermal_stats", "sph_app_set_adhesion", "sph_app_adhesion_stats", "sph_app_load_obj", "sph_app_load_obj_error",
     "sph_app_set_probes", "sph_app_probe_series", "sph_app_sample_probes", "sph_app_sample_lattice",
-    "sph_app_checkpoint", "sph_app_checkpoint_wait", "sph_app_restore",
+    "sph_app_checkpoint", "sph_app_checkpoint_wait", "sph_app_restore", "sph_app_set_tank_motion", "sph_app_tank_state",
 ]
 
 BODY_LIMIT = 64                      # SPHK_BODY_LIMIT
@@ -110,6 +111,47 @@ ADHESION_GROUPS = 1 + BODY_LIMIT     # SPHK_ADHESION_GROUPS
 class Adhesion(C.Structure):
     """sphk_adhesion_setting of sphk.h"""
     _fields_ = [("n_groups", C.c_int), ("beta", C.c_float * ADHESION_GROUPS)]
+
+
+TANK_HARMONICS = 4                   # SPHK_TANK_HARMONICS
+TANK_STATE = 9                       # SPHK_TANK_STATE
+
+
+class TankMotion(C.Structure):
+    """sphk_tank_motion of sphk.h (sph_app_tank_motion has the same layout)"""
+    _fields_ = [("axis", C.c_float * 3), ("pivot", C.c_float * 3), ("roll_amplitude", C.c_float), ("roll_omega", C.c_float),
+                ("roll_phase", C.c_float), ("spin", C.c_float), ("accel", C.c_float * 3), ("n_harmonics", C.c_int),
+                ("harmonic_amplitude", (C.c_float * 3) * TANK_HARMONICS), ("harmonic_omega", C.c_float * TANK_HARMONICS),
+                ("harmonic_phase", C.c_float * TANK_HARMONICS), ("ramp", C.c_float)]
+
+
+TANK_KEYS = {"axis", "pivot", "roll_amplitude", "roll_omega", "roll_phase", "spin", "accel", "harmonics", "ramp"}
+
+
+def tank_motion(spec: dict) -> TankMotion:
+    """sphk_tank_motion from dict(axis=(0, 0, 1), pivot=(0, 0, 0), roll_amplitude=0, roll_omega=0, roll_phase=0, spin=0,
+    accel=(0, 0, 0), harmonics=[dict(amplitude=(ax, ay, az), omega=, phase=0), ...], ramp=0) (DESIGN.md section 2.15).  Unknown keys
+    and more than TANK_HARMONICS harmonics raise ValueError; the ranges are checked by the library.  Unused entries are zero."""
+    extra = set(spec) - TANK_KEYS
+    if extra:
+        raise ValueError(f"unknown tank keys {sorted(extra)}")
+    harm = list(spec.get("harmonics", ()))
+    if len(harm) > TANK_HARMONICS:
+        raise ValueError(f"at most {TANK_HARMONICS} harmonics")
+    m = TankMotion()
+    m.axis[:] = [float(x) for x in spec.get("axis", (0.0, 0.0, 1.0))]
+    m.pivot[:] = [float(x) for x in spec.get("pivot", (0.0, 0.0, 0.0))]
+    m.roll_amplitude, m.roll_omega = float(spec.get("roll_amplitude", 0.0)), float(spec.get("roll_omega", 0.0))
+    m.roll_phase, m.spin = float(spec.get("roll_phase", 0.0)), float(spec.get("spin", 0.0))
+    m.accel[:] = [float(x) for x in spec.get("accel", (0.0, 0.0, 0.0))]
+    m.n_harmonics = len(harm)
+    for k, h in enumerate(harm):
+        if set(h) - {"amplitude", "omega", "phase"}:
+            raise ValueError(f"unknown harmonic keys {sorted(set(h) - {'amplitude', 'omega', 'phase'})}")
+        m.harmonic_amplitude[k][:] = [float(x) for x in h.get("amplitude", (0.0, 0.0, 0.0))]
+        m.harmonic_omega[k], m.harmonic_phase[k] = float(h.get("omega", 0.0)), float(h.get("phase", 0.0))
+    m.ramp = float(spec.get("ramp", 0.0))
+    return m
 
 
 def adhesion(spec: dict) -> Adhesion:
@@ -600,6 +642,21 @@ class SphApp:
         if self.L.sph_app_adhesion_stats(self.h, C.byref(w), C.byref(am)):
             raise RuntimeError("sph_app_adhesion_stats failed (reference engine)")
         return {"wetted": w.value, "max_accel": am.value}
+
+    def set_tank_motion(self, spec):
+        """Tank motion from the next step on (spec: a dict for capi.tank_motion; None: off).  Not on the reference engine."""
+        rc = self.L.sph_app_set_tank_motion(self.h, None if spec is None else C.byref(tank_motion(spec)))
+        if rc:
+            raise RuntimeError("sph_app_set_tank_motion failed (reference engine or a refused setting)")
+
+    def tank_state(self) -> dict:
+        """the motion at the simulated time: {"t", "theta", "theta_dot", "theta_ddot", "accel" (a_w, world), "gravity" (R (G - a_w),
+        tank axes)}"""
+        t, v = C.c_double(0.0), (C.c_float * 9)()
+        if self.L.sph_app_tank_state(self.h, C.byref(t), v):
+            raise RuntimeError("sph_app_tank_state failed (reference engine)")
+        return {"t": t.value, "theta": v[0], "theta_dot": v[1], "theta_ddot": v[2], "accel": np.array(v[3:6], np.float32),
+                "gravity": np.array(v[6:9], np.float32)}
 
     def set_probes(self, points=(), gauges=(), threshold: float = 0.5, capacity: int = 1024):
         """Probes and water-level gauges recorded every following step (SPHSystem::setProbes; DESIGN.md section 2.13).  points: (P, 3);

@@ -74,6 +74,32 @@ struct BodyState {
     float* dyn = nullptr;            // device [SPHK_DYN * nBodies]: M, I.xyz, box lo.xyz, box hi.xyz, clamp box hi.xyz
     double* acc = nullptr;           // device [6 * (n - nStatic)]: {J, H} of every body particle, summed over the step's reactions
     float* impulse = nullptr;        // device [6 * nBodies]: {J, H} of the last integrated step
+    bool anyDynamic = false;         // host: some body was declared with M > 0
+};
+
+// Tank motion (sphk_tank_*, sphk_sweeps.cu; DESIGN.md section 2.15): the schedule in double, as sphk_tank_set normalised it
+struct TankParams {
+    double n[3], p[3];               // unit axis, pivot (tank coordinates)
+    double theta, omega, phi, spin;  // roll Theta sin(omega t + phi), spin Omega0
+    double ac[3];                    // constant world acceleration
+    double A[SPHK_TANK_HARMONICS][3], w[SPHK_TANK_HARMONICS], ph[SPHK_TANK_HARMONICS];
+    double ramp;                     // T_r (0: none)
+    double G[3];                     // gravity in the world
+    int nh;                          // harmonics in use
+};
+// the per-step state sphk_tank_force writes on the device (k_tank_begin) and its particle kernel reads
+struct TankStep {
+    double t;                        // frame time of the next step
+    double rot[9];                   // Rot(n, -2 thd dt), row-major: the Coriolis term of the step
+    float dv[3];                     // dt R (G - a_w)
+    float thdd_dt, w2_dt;            // thdd dt, thd^2 dt
+    float state[SPHK_TANK_STATE];    // sphk_tank_eval's outputs at the step's t_n
+};
+struct TankState {
+    bool on = false;                 // a motion is set
+    bool rotates = false;            // Theta != 0 or Omega0 != 0
+    TankParams P{};
+    TankStep* dev = nullptr;         // device [1], allocated at the first sphk_tank_set
 };
 #define SPHK_DYN 16                  // floats per body in BodyState::dyn
 __device__ __forceinline__ float body_group(float4 local) { return local.w; }
@@ -172,6 +198,8 @@ struct sphk_ctx {
     cudaEvent_t speedEvent = nullptr;     // recorded after that copy
     // checkpoints (sphk_state.cu; allocated at the first save or load)
     struct StateStage* state = nullptr;
+    // tank motion (sphk_tank_set; allocated at the first setting)
+    TankState* tank = nullptr;
 };
 
 struct DevScene {

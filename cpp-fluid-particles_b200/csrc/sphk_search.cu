@@ -255,6 +255,7 @@ extern "C" void sphk_destroy(sphk_ctx* c) {
     cudaFree(c->snapA); cudaFree(c->snapB); cudaFree(c->rec.a); cudaFree(c->rec.b); cudaFree(c->massRange); cudaFree(c->dispMax); cudaFree(c->cellFlag);
     cudaFree(c->tmpF); cudaFree(c->partial); cudaFree(c->loops); cudaFree(c->viscStats); cudaFree(c->rheoStats); cudaFree(c->heatGroups); cudaFree(c->heatStats); cudaFree(c->heatRed); cudaFree(c->adhGroups); cudaFree(c->adhStats); cudaFree(c->cnt); cudaFree(c->nbr); cudaFree(c->cubTemp); cudaFree(c->tileWin); cudaFree(c->chunkAct); cudaFree(c->chunkStamp); cudaFree(c->chunkMark);
     if (c->pinned) cudaFreeHost(c->pinned);
+    if (c->tank) { cudaFree(c->tank->dev); delete c->tank; }
     cudaFree(c->openDev);
     if (c->openPinned) cudaFreeHost(c->openPinned);
     if (c->sinkEvent) cudaEventDestroy(c->sinkEvent);
@@ -787,7 +788,8 @@ k_bodies_gather(const int* __restrict__ idxSorted, const float4* __restrict__ sn
 #define SPHK_INTEGRATE_THREADS 256
 __global__ void __launch_bounds__(SPHK_INTEGRATE_THREADS)
 k_bodies_integrate(const int* __restrict__ begin, int nStatic, double* __restrict__ acc, const float* __restrict__ pose,
-                   float* __restrict__ motion, const float* __restrict__ dyn, float* __restrict__ impulse, float dt, float3 G) {
+                   float* __restrict__ motion, const float* __restrict__ dyn, float* __restrict__ impulse, float dt, float3 G,
+                   const float* __restrict__ tankG) {
     __shared__ double red[6][SPHK_INTEGRATE_THREADS];
     const int b = blockIdx.x, t = threadIdx.x;
     const int k0 = begin[b] - nStatic, k1 = begin[b + 1] - nStatic;
@@ -808,7 +810,7 @@ k_bodies_integrate(const int* __restrict__ begin, int nStatic, double* __restric
     const double M = D[0];
     if (!(M > 0.0)) return;                                  // held: kinematic, the reaction is only reported
     float* Mo = motion + 6 * b;
-    const double g[3] = {G.x, G.y, G.z};
+    const double g[3] = {tankG ? tankG[0] : G.x, tankG ? tankG[1] : G.y, tankG ? tankG[2] : G.z};   // tank motion: R (G - a_w)
     for (int a = 0; a < 3; ++a) Mo[a] = static_cast<float>(Mo[a] + J[a] / M + static_cast<double>(dt) * g[a]);
     double R[9];
     quat_matrix(pose + 7 * b + 3, R);
@@ -966,6 +968,9 @@ extern "C" int sphk_bodies_set_dynamics(sphk_ctx* c, const float* mass_inertia, 
         if (m[0] > 0.f && !(m[1] > 0.f && m[2] > 0.f && m[3] > 0.f)) return SPHK_ERR_INVALID;
     }
     if (B->dyn || B->stepped) return SPHK_ERR_STATE;        // once, before the first sphk_bodies_step
+    bool anyDynamic = false;
+    for (int b = 0; b < B->nBodies; ++b) anyDynamic = anyDynamic || mass_inertia[4 * b] > 0.f;
+    if (anyDynamic && c->tank && c->tank->on && c->tank->rotates) return SPHK_ERR_STATE;   // no rigid dynamics in a rotating frame
     std::vector<float> dyn(static_cast<size_t>(SPHK_DYN) * B->nBodies, 0.f);
     for (int b = 0; b < B->nBodies; ++b) {
         float* D = dyn.data() + SPHK_DYN * b;
@@ -984,6 +989,7 @@ extern "C" int sphk_bodies_set_dynamics(sphk_ctx* c, const float* mass_inertia, 
         cudaGetLastError();
         return e == cudaErrorMemoryAllocation ? SPHK_ERR_ALLOC : static_cast<int>(e);
     }
+    B->anyDynamic = anyDynamic;
     return SPHK_OK;
 }
 
@@ -993,7 +999,8 @@ extern "C" int sphk_bodies_integrate(sphk_ctx* c, float dt, const float G[3]) {
     if (!c->bodies || !c->bodies->dyn) return SPHK_ERR_STATE;
     const BodyState* B = c->bodies;
     k_bodies_integrate<<<B->nBodies, SPHK_INTEGRATE_THREADS, 0, c->stream>>>(B->begin, B->nStatic, B->acc, B->pose, B->motion,
-                                                                             B->dyn, B->impulse, dt, make_float3(G[0], G[1], G[2]));
+                                                                             B->dyn, B->impulse, dt, make_float3(G[0], G[1], G[2]),
+                                                                             c->tank && c->tank->on ? c->tank->dev->state + 3 : nullptr);
     c->launches++;
     SPHK_CUDA_TRY(cudaGetLastError());
     return SPHK_OK;

@@ -2987,3 +2987,192 @@ extern "C" int sphk_list_stats(sphk_ctx* c, const sphk_scene* s, long long out_h
     for (int k = 0; k < 3; ++k) out_host[k] = static_cast<long long>(h[k]);
     return SPHK_OK;
 }
+
+// ---- tank motion (DESIGN.md section 2.15) ---------------------------------------------------------------------------------------
+// The schedule of sphk.h in double, host and device alike (k_tank_begin evaluates it at the device-resident frame time).
+struct TankEval {
+    double th, thd, thdd, g[3], aw[3];
+};
+__host__ __device__ static void tank_schedule(const TankParams& P, double t, TankEval& E) {
+    const bool ramping = P.ramp > 0.0 && t < P.ramp;
+    const double e = ramping ? t / P.ramp : 1.0, ed = ramping ? 1.0 / P.ramp : 0.0;
+    const double s = sin(P.omega * t + P.phi), c = cos(P.omega * t + P.phi);
+    const double ths = ramping ? P.spin * t * t / (2.0 * P.ramp) : P.spin * (t - 0.5 * P.ramp);
+    E.th = e * P.theta * s + ths;
+    E.thd = ed * P.theta * s + e * P.theta * P.omega * c + e * P.spin;
+    E.thdd = 2.0 * ed * P.theta * P.omega * c - e * P.theta * P.omega * P.omega * s + ed * P.spin;
+    double d[3];
+    for (int a = 0; a < 3; ++a) {
+        double acc = P.ac[a];
+        for (int k = 0; k < P.nh; ++k) acc += P.A[k][a] * sin(P.w[k] * t + P.ph[k]);
+        E.aw[a] = e * acc;
+        d[a] = P.G[a] - E.aw[a];
+    }
+    // R = Rot(n, -theta): R d = cos(theta) d - sin(theta) n x d + (1 - cos(theta)) n (n . d)
+    const double ct = cos(E.th), st = sin(E.th), nd = P.n[0] * d[0] + P.n[1] * d[1] + P.n[2] * d[2];
+    const double nxd[3] = {P.n[1] * d[2] - P.n[2] * d[1], P.n[2] * d[0] - P.n[0] * d[2], P.n[0] * d[1] - P.n[1] * d[0]};
+    for (int a = 0; a < 3; ++a) E.g[a] = ct * d[a] - st * nxd[a] + (1.0 - ct) * P.n[a] * nd;
+}
+__host__ __device__ static void tank_state_out(const TankEval& E, float* out) {
+    out[0] = static_cast<float>(E.th); out[1] = static_cast<float>(E.thd); out[2] = static_cast<float>(E.thdd);
+    for (int a = 0; a < 3; ++a) { out[3 + a] = static_cast<float>(E.g[a]); out[6 + a] = static_cast<float>(E.aw[a]); }
+}
+
+static bool tank_params(const sphk_tank_motion* m, const float G[3], TankParams& P) {
+    if (!m || !G) return false;
+    const float* f3s[] = {m->axis, m->pivot, m->accel, G};
+    for (const float* v : f3s)
+        for (int a = 0; a < 3; ++a) if (!finite_f(v[a])) return false;
+    const float sc[] = {m->roll_amplitude, m->roll_omega, m->roll_phase, m->spin, m->ramp};
+    for (float v : sc) if (!finite_f(v)) return false;
+    if (m->roll_omega < 0.f || m->ramp < 0.f || m->n_harmonics < 0 || m->n_harmonics > SPHK_TANK_HARMONICS) return false;
+    for (int k = 0; k < m->n_harmonics; ++k) {
+        if (!finite_nonneg(m->harmonic_omega[k]) || !finite_f(m->harmonic_phase[k])) return false;
+        for (int a = 0; a < 3; ++a) if (!finite_f(m->harmonic_amplitude[k][a])) return false;
+    }
+    const double n2 = double(m->axis[0]) * m->axis[0] + double(m->axis[1]) * m->axis[1] + double(m->axis[2]) * m->axis[2];
+    if (!(n2 > 0.0)) return false;
+    P = TankParams{};
+    const double nl = std::sqrt(n2);
+    for (int a = 0; a < 3; ++a) {
+        P.n[a] = m->axis[a] / nl; P.p[a] = m->pivot[a]; P.ac[a] = m->accel[a]; P.G[a] = G[a];
+    }
+    P.theta = m->roll_amplitude; P.omega = m->roll_omega; P.phi = m->roll_phase; P.spin = m->spin; P.ramp = m->ramp;
+    P.nh = m->n_harmonics;
+    for (int k = 0; k < P.nh; ++k) {
+        P.w[k] = m->harmonic_omega[k]; P.ph[k] = m->harmonic_phase[k];
+        for (int a = 0; a < 3; ++a) P.A[k][a] = m->harmonic_amplitude[k][a];
+    }
+    return true;
+}
+
+extern "C" int sphk_tank_eval(const sphk_tank_motion* m, const float G[3], double t, float out[SPHK_TANK_STATE]) {
+    TankParams P;
+    if (!out || !tank_params(m, G, P) || !(t >= 0.0) || !(t - t == 0.0)) return SPHK_ERR_INVALID;
+    TankEval E;
+    tank_schedule(P, t, E);
+    tank_state_out(E, out);
+    return SPHK_OK;
+}
+
+extern "C" int sphk_tank_accel_bound(const sphk_tank_motion* m, const float G[3], const float space[3], double* bound_out) {
+    TankParams P;
+    if (!bound_out || !space || !tank_params(m, G, P)) return SPHK_ERR_INVALID;
+    for (int a = 0; a < 3; ++a) if (!finite_f(space[a]) || !(space[a] > 0.f)) return SPHK_ERR_INVALID;
+    double r2 = 0.0;
+    for (int a = 0; a < 3; ++a) {
+        const double hi = 0.99 * space[a], far = std::fmax(std::fabs(P.p[a]), std::fabs(hi - P.p[a]));
+        r2 += far * far;
+    }
+    const double Th = std::fabs(P.theta), W = P.omega, S = std::fabs(P.spin), rinv = P.ramp > 0.0 ? 1.0 / P.ramp : 0.0;
+    double lin = std::sqrt(P.G[0] * P.G[0] + P.G[1] * P.G[1] + P.G[2] * P.G[2]);
+    lin += std::sqrt(P.ac[0] * P.ac[0] + P.ac[1] * P.ac[1] + P.ac[2] * P.ac[2]);
+    for (int k = 0; k < P.nh; ++k) lin += std::sqrt(P.A[k][0] * P.A[k][0] + P.A[k][1] * P.A[k][1] + P.A[k][2] * P.A[k][2]);
+    const double thd = Th * W + Th * rinv + S;
+    *bound_out = lin + std::sqrt(r2) * (Th * W * W + (2.0 * Th * W + S) * rinv + thd * thd);
+    return SPHK_OK;
+}
+
+extern "C" int sphk_tank_set(sphk_ctx* c, const sphk_tank_motion* m, const float G[3]) {
+    if (!c) return SPHK_ERR_INVALID;
+    TankParams P{};
+    if (m && !tank_params(m, G, P)) return SPHK_ERR_INVALID;
+    if (c->actCount >= 0 || c->rangeDev) return SPHK_ERR_STATE;       // slab ranks: not supported
+    const bool rotates = m && (m->roll_amplitude != 0.f || m->spin != 0.f);
+    if (rotates && c->bodies && c->bodies->anyDynamic) return SPHK_ERR_STATE;
+    if (!m) { if (c->tank) c->tank->on = false; return SPHK_OK; }
+    if (!c->tank) {
+        TankState* T = new TankState();
+        cudaError_t e = cudaMalloc(reinterpret_cast<void**>(&T->dev), sizeof(TankStep));
+        if (e == cudaSuccess) e = cudaMemsetAsync(T->dev, 0, sizeof(TankStep), c->stream);
+        if (e != cudaSuccess) { cudaFree(T->dev); delete T; cudaGetLastError(); return e == cudaErrorMemoryAllocation ? SPHK_ERR_ALLOC : static_cast<int>(e); }
+        c->tank = T;
+    }
+    c->tank->P = P;
+    c->tank->on = true;
+    c->tank->rotates = rotates;
+    return SPHK_OK;
+}
+
+// the step's state at the frame time, then the frame time advanced by (double) dt
+__global__ void k_tank_begin(TankParams P, float dt, TankStep* __restrict__ st) {
+    const double t = st->t;
+    TankEval E;
+    tank_schedule(P, t, E);
+    const double a = -2.0 * E.thd * static_cast<double>(dt), ca = cos(a), sa = sin(a);
+    const double* n = P.n;
+    // Rot(n, a) = cos(a) I + sin(a) [n]x + (1 - cos(a)) n n^T
+    const double K[9] = {0.0, -n[2], n[1], n[2], 0.0, -n[0], -n[1], n[0], 0.0};
+    for (int r = 0; r < 3; ++r)
+        for (int q = 0; q < 3; ++q) st->rot[3 * r + q] = (r == q ? ca : 0.0) + sa * K[3 * r + q] + (1.0 - ca) * n[r] * n[q];
+    float s[SPHK_TANK_STATE];
+    tank_state_out(E, s);
+    for (int k = 0; k < SPHK_TANK_STATE; ++k) st->state[k] = s[k];
+    for (int k = 0; k < 3; ++k) st->dv[k] = dt * s[3 + k];          // as sphk_gravity forms dt G
+    st->thdd_dt = static_cast<float>(E.thdd * dt);
+    st->w2_dt = static_cast<float>(E.thd * E.thd * dt);
+    st->t = t + static_cast<double>(dt);
+}
+// v <- Rot(n, -2 thd dt) v + dt (R (G - a_w) - thdd n x r - thd^2 n x (n x r)); k_gravity's arithmetic when thd = thdd = 0
+__global__ void __launch_bounds__(SPHK_BLOCK)
+k_tank_force(Rec rec, float* __restrict__ vel, int n, const TankStep* __restrict__ st, float3 ax, float3 pivot) {
+    const int i = blockIdx.x * SPHK_BLOCK + threadIdx.x;
+    if (i >= n) return;
+    const float4 hi = rec_hi(rec + i);
+    const float3 dv = f3(st->dv[0], st->dv[1], st->dv[2]);
+    const float s0 = st->state[1], s1 = st->state[2];
+    float3 v;
+    if (s0 == 0.0f && s1 == 0.0f) {
+        v = f3(hi.x + dv.x, hi.y + dv.y, hi.z + dv.z);
+    } else {
+        const float3 r = xyz(rec_lo(rec + i)) - pivot;
+        const float3 nr = f3(ax.y * r.z - ax.z * r.y, ax.z * r.x - ax.x * r.z, ax.x * r.y - ax.y * r.x);
+        const float3 nnr = f3(ax.y * nr.z - ax.z * nr.y, ax.z * nr.x - ax.x * nr.z, ax.x * nr.y - ax.y * nr.x);
+        const double* M = st->rot;
+        const double vx = hi.x, vy = hi.y, vz = hi.z;
+        const float3 vr = f3(static_cast<float>(M[0] * vx + M[1] * vy + M[2] * vz), static_cast<float>(M[3] * vx + M[4] * vy + M[5] * vz),
+                             static_cast<float>(M[6] * vx + M[7] * vy + M[8] * vz));
+        const float a = st->thdd_dt, b = st->w2_dt;
+        v = vr + (dv - a * nr - b * nnr);
+    }
+    rec_set_vel(rec + i, v); store3(vel, i, v);
+}
+
+extern "C" int sphk_tank_force(sphk_ctx* c, const sphk_scene* s, float dt) {
+    SPHK_CHECK_SCENE(c, s);
+    if (!finite_nonneg(dt)) return SPHK_ERR_INVALID;
+    if (!c->tank || !c->tank->on) return SPHK_ERR_STATE;
+    const TankState* T = c->tank;
+    k_tank_begin<<<1, 1, 0, c->stream>>>(T->P, dt, T->dev);
+    c->launches++;
+    if (c->nF > 0) {
+        const float3 ax = make_float3(static_cast<float>(T->P.n[0]), static_cast<float>(T->P.n[1]), static_cast<float>(T->P.n[2]));
+        const float3 pv = make_float3(static_cast<float>(T->P.p[0]), static_cast<float>(T->P.p[1]), static_cast<float>(T->P.p[2]));
+        k_tank_force<<<sphk_blocks(c->nF), SPHK_BLOCK, 0, c->stream>>>(c->rec, s->fluid.vel, c->nF, T->dev, ax, pv);
+        c->launches++;
+    }
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+__global__ void k_tank_set_time(TankStep* st, double t) { st->t = t; }
+
+extern "C" int sphk_tank_set_time(sphk_ctx* c, double t) {
+    if (!c || !(t >= 0.0) || !(t - t == 0.0)) return SPHK_ERR_INVALID;
+    if (!c->tank) return SPHK_ERR_STATE;
+    k_tank_set_time<<<1, 1, 0, c->stream>>>(c->tank->dev, t);
+    c->launches++;
+    SPHK_CUDA_TRY(cudaGetLastError());
+    return SPHK_OK;
+}
+
+extern "C" int sphk_tank_time(sphk_ctx* c, double* t, float* state_or_null) {
+    if (!c || !t) return SPHK_ERR_INVALID;
+    if (!c->tank) return SPHK_ERR_STATE;
+    TankStep h;
+    SPHK_CUDA_TRY(cudaMemcpyAsync(&h, c->tank->dev, sizeof(h), cudaMemcpyDeviceToHost, c->stream));
+    SPHK_CUDA_TRY(cudaStreamSynchronize(c->stream));
+    *t = h.t;
+    if (state_or_null) memcpy(state_or_null, h.state, sizeof(h.state));
+    return SPHK_OK;
+}

@@ -90,6 +90,7 @@ class SphkOps:
     _thermal_viscosity = None
     _rheology = None
     _adhesion = None
+    _tank = None                     # tank motion (SPHSystem::setTankMotion): a capi.tank_motion dict; None: off
     heat_substeps = 0                # conduction substeps of the last step
     implicit_nu_boundary = 0.0
     implicit_tol = 1e-4
@@ -296,6 +297,59 @@ class SphkOps:
     def gravity(self):
         check(self.L.sphk_gravity(self.ctx, self._s(), C.c_float(self.dt), self._G), "sphk_gravity")
 
+    def force(self):
+        """BasicSPHSolver::force: the tank frame's body force while a motion is set, else gravity"""
+        if self._tank is not None:
+            self.tank_force()
+        else:
+            self.gravity()
+
+    # ---- tank motion (no reference counterpart; DESIGN.md section 2.15) ------------------------------------------------------
+    @property
+    def tank(self):
+        """the tank motion (a dict for capi.tank_motion) or None; setting it is SPHSystem::setTankMotion (the frame time starts at the
+        simulated time), None is clearTankMotion.  ValueError for a setting the class layer refuses (the setting is kept)."""
+        return self._tank
+
+    @tank.setter
+    def tank(self, spec):
+        if spec is None:
+            if self._tank is not None:
+                check(self.L.sphk_tank_set(self.ctx, None, None), "sphk_tank_set")
+            self._tank = None
+        else:
+            m = capi.tank_motion(spec)
+            if self.L.sphk_tank_eval(C.byref(m), self._G, C.c_double(0.0), (C.c_float * capi.TANK_STATE)()) != 0:
+                raise ValueError(f"tank motion refused: {spec}")
+            if self._thermal is not None:
+                raise ValueError("tank motion refused: not together with heat transfer")
+            if (m.roll_amplitude != 0.0 or m.spin != 0.0) and getattr(self, "bodies_dynamic", False):
+                raise ValueError("tank motion refused: a rotating tank with dynamic bodies")
+            check(self.L.sphk_tank_set(self.ctx, C.byref(m), self._G), "sphk_tank_set")
+            check(self.L.sphk_tank_set_time(self.ctx, C.c_double(self.simulated_time)), "sphk_tank_set_time")
+            self._tank, self._tank_abi = dict(spec), m
+        if getattr(self, "adaptive", False):
+            self._rule.gravity = self._rule_gravity()
+
+    def _rule_gravity(self) -> float:
+        """the adaptive rule's |G|: |G|, or sphk_tank_accel_bound under a tank motion (as SPHSystem::ruleGravity)"""
+        if self._tank is not None:
+            b = C.c_double(0.0)
+            check(self.L.sphk_tank_accel_bound(C.byref(self._tank_abi), self._G, self._space, C.byref(b)), "sphk_tank_accel_bound")
+            return b.value
+        g = [float(np.float32(x)) for x in self.p.gravity]
+        return float(np.sqrt(g[0] * g[0] + g[1] * g[1] + g[2] * g[2]))
+
+    def tank_force(self, dt=None):
+        """sphk_tank_force with the step's dt (or `dt`)"""
+        check(self.L.sphk_tank_force(self.ctx, self._s(), C.c_float(self.dt if dt is None else dt)), "sphk_tank_force")
+
+    def tank_state(self):
+        """(device frame time, the last sphk_tank_force's state float[9] {theta, thd, thdd, R (G - a_w), a_w}); synchronises"""
+        t, v = C.c_double(0.0), (C.c_float * capi.TANK_STATE)()
+        check(self.L.sphk_tank_time(self.ctx, C.byref(t), v), "sphk_tank_time")
+        return t.value, np.array(v[:], np.float32)
+
     def viscosity(self):
         check(self.L.sphk_viscosity(self.ctx, self._s(), _ptr(self.buffer3), C.c_float(self.p.rho0),
                                     C.c_float(self.p.visc), C.c_float(self.dt)), "sphk_viscosity")
@@ -479,6 +533,8 @@ class SphkOps:
                 raise ValueError(f"{len(spec['bodies'])} body entries, but the system has {self.n_bodies} bodies")
             if self.L.sphk_heat_substeps(C.byref(t), C.c_float(self.p.radius), C.c_float(0.0), C.byref(C.c_int(0))):
                 raise ValueError(f"thermal setting refused: {spec}")
+            if self._tank is not None:
+                raise ValueError("thermal setting refused: not under a tank motion (the buoyancy acts along the constant G)")
             if getattr(self, "temperature", None) is None:
                 n = self.buffer3.shape[0]
                 self.temperature = torch.full((n,), float(np.float32(t.t_ref)), dtype=torch.float32, device=self.device)
@@ -732,7 +788,7 @@ class SphkOps:
     def step_wcsph(self):            # BasicSPHSolver.cu:237-260
         self.set_use_list(self.use_list)
         self._carry_temperature()
-        self.gravity()
+        self.force()
         if self.fused:               # density (+ colour gradient) before the velocity terms: it reads positions and masses only
             if self._surface_enabled():
                 self._run(lambda: self.fused_density_color_grad(False), "array", self.color_grad_buf)
@@ -770,7 +826,7 @@ class SphkOps:
             if self.div_thr >= 0:    # negative threshold: the test cannot depend on the sum (Q11) -> no host sync
                 total = self.reduce_sum(self.reduce_abs_sum(self.owned(self.error)))
         self.it_div = it
-        self.gravity()
+        self.force()
         self._velocity_stage()
         total, it = 3.4e38, 0        # project :160-210
         self.permute(self.warm, 1)
@@ -804,7 +860,7 @@ class SphkOps:
             self.pbd_delta_pos_apply(); self.sync_positions()
         self.pbd_velocity_from_positions()
         self._velocity_stage(xsph=True)
-        self.gravity()
+        self.force()
         self.copy(self.pos_last, self.fluid.pos)
         self.advect()
         self.pbd_last_dt = self.dt
@@ -897,8 +953,7 @@ class SphkOps:
         r.dt_max = f(dt_max) if dt_max > 0 else f(self.p.dt)
         r.dt_min = f(dt_min) if dt_min > 0 else float(np.float32(r.dt_max) / np.float32(64.0))
         r.radius = f(self.p.radius)
-        g = [f(x) for x in self.p.gravity]
-        r.gravity = float(np.sqrt(g[0] * g[0] + g[1] * g[1] + g[2] * g[2]))
+        r.gravity = self._rule_gravity()
         dt, flags = C.c_float(0.0), C.c_int(0)
         if not (dt_min >= 0 and dt_max >= 0) or self.L.sphk_time_step(C.byref(r), C.c_double(0.0), C.c_double(0.0), C.c_double(0.0),
                                                                       C.byref(dt), C.byref(flags)) != 0:
@@ -1074,7 +1129,7 @@ class SphkSystem(SphkOps):
     reference constructor including its implicit first step (Q3)."""
 
     def __init__(self, scene, device="cuda:0", use_list: bool | None = None, list_capacity: int | None = None,
-                 step0: bool = True, bodies=None, max_fluid: int | None = None, emitters=None, sinks=None, adaptive=None):
+                 step0: bool = True, bodies=None, max_fluid: int | None = None, emitters=None, sinks=None, adaptive=None, tank=None):
         """emitters / sinks: open boundaries (DESIGN.md section 2.6), the same C entries in the same order as SPHSystem::step.
         emitters: dicts {"origin", "direction", "speed", "spacing", "width", "height"} (sphk_emitter); sinks: (lo, hi) boxes; max_fluid:
         the capacity of the fluid set (default: the initial count).  fluid_count is the live count.
@@ -1084,7 +1139,8 @@ class SphkSystem(SphkOps):
         when another body is dynamic) and "inertia" (3,) principal
         moments about the centre in the axes of "points".  Masses are in the fluid's units, m0 / spacing^3 per unit volume
         (not rho0).  Their particles follow the static boundary set; every step() moves them before the fluid search.
-        adaptive: dict(C=, dt_min=0, dt_max=0): CFL-adaptive time stepping (set_adaptive) from the step after the constructor's on."""
+        adaptive: dict(C=, dt_min=0, dt_max=0): CFL-adaptive time stepping (set_adaptive) from the step after the constructor's on.
+        tank: a tank motion (the `tank` property; DESIGN.md section 2.15) from the step after the constructor's on."""
         self.L = capi.sphk()
         self.p = scene.params
         self.device = torch.device(device)
@@ -1160,6 +1216,8 @@ class SphkSystem(SphkOps):
             self.step()
         if adaptive is not None:
             self.set_adaptive(adaptive["C"], adaptive.get("dt_min", 0.0), adaptive.get("dt_max", 0.0))
+        if tank is not None:
+            self.tank = tank
 
     # ---- checkpoints (DESIGN.md section 2.14): the class layer's sections, names and config record ---------------------------------
     _STATE_RECORD = struct.Struct("<6qd4f2i")          # SPHSystem::StateRecord
@@ -1212,6 +1270,8 @@ class SphkSystem(SphkOps):
             st += bytes(self._adhesion_abi)
         if getattr(self, "adaptive", False):
             st += bytes(self._rule)
+        if self._tank is not None:
+            st += bytes(self._tank_abi)
         c.settings_hash = (capi.state_hash(st) + len(st)) & M
         return c
 
@@ -1321,6 +1381,8 @@ class SphkSystem(SphkOps):
         check(self.L.sphk_checkpoint_invalidate(self.ctx), "sphk_checkpoint_invalidate")
         if getattr(self, "adaptive", False):
             self.measure_speed()
+        if self._tank is not None:   # the frame time of the saved run
+            check(self.L.sphk_tank_set_time(self.ctx, C.c_double(self.simulated_time)), "sphk_tank_set_time")
         self.synchronize()
         return u.raw[:user_b.value]
 

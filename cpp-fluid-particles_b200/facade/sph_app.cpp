@@ -669,6 +669,46 @@ extern "C" int sph_app_adhesion_stats(sph_app* app, int* wetted, float* max_acce
 #endif
 }
 
+extern "C" int sph_app_set_tank_motion(sph_app* app, const sph_app_tank_motion* m) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)m;
+    return 1;
+#else
+    if (!app) return 1;
+    if (!m) { app->system->clearTankMotion(); return 0; }
+    if (m->n_harmonics < 0 || m->n_harmonics > 4) return 1;
+    sphb200::TankMotion t;
+    t.axis = make_float3(m->axis[0], m->axis[1], m->axis[2]);
+    t.pivot = make_float3(m->pivot[0], m->pivot[1], m->pivot[2]);
+    t.rollAmplitude = m->roll_amplitude; t.rollOmega = m->roll_omega; t.rollPhase = m->roll_phase; t.spin = m->spin;
+    t.accel = make_float3(m->accel[0], m->accel[1], m->accel[2]);
+    for (int k = 0; k < m->n_harmonics; ++k) {
+        sphb200::TankHarmonic h;
+        h.amplitude = make_float3(m->harmonic_amplitude[k][0], m->harmonic_amplitude[k][1], m->harmonic_amplitude[k][2]);
+        h.omega = m->harmonic_omega[k]; h.phase = m->harmonic_phase[k];
+        t.harmonics.push_back(h);
+    }
+    t.ramp = m->ramp;
+    return app->system->setTankMotion(t) ? 0 : 1;        // (refused: the setting is kept)
+#endif
+}
+
+extern "C" int sph_app_tank_state(sph_app* app, double* t, float* state9) {
+#ifdef SPH_APP_REFERENCE_ENGINE
+    (void)app; (void)t; (void)state9;
+    return 1;
+#else
+    if (!app) return 1;
+    const sphb200::TankState s = app->system->tankState();
+    if (t) *t = s.t;
+    if (state9) {
+        const float v[9] = {s.theta, s.thetaDot, s.thetaDDot, s.accel.x, s.accel.y, s.accel.z, s.gravity.x, s.gravity.y, s.gravity.z};
+        std::copy(v, v + 9, state9);
+    }
+    return 0;
+#endif
+}
+
 extern "C" int sph_app_set_probes(sph_app* app, int n_points, const float* points_xyz, int n_gauges, const float* gauge_ab,
                                   const int* gauge_samples, float threshold, int capacity) {
 #ifdef SPH_APP_REFERENCE_ENGINE

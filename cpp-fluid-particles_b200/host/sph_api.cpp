@@ -314,6 +314,10 @@ bool BasicSPHSolver::setThermal(const sphb200::Thermal& t) {
                "the setting is kept\n", SPHK_BODY_LIMIT);
         return false;
     }
+    if (tankOn_) {
+        printf("setThermal: not under a tank motion (the Boussinesq buoyancy acts along the constant G); the setting is kept\n");
+        return false;
+    }
     if (bodies_ >= 0 && static_cast<int>(t.bodies.size()) > bodies_) {
         printf("setThermal: %d body entries, but the system has %d bodies; the setting is kept\n", static_cast<int>(t.bodies.size()),
                bodies_);
@@ -442,6 +446,10 @@ sphb200::AdhesionStats BasicSPHSolver::lastAdhesionStats() const {
 // :227-235
 void BasicSPHSolver::force(std::shared_ptr<SPHParticles>&, float dt, float3 G) {
     if (!current_.ctx) return;
+    if (tankOn_) {                  // addition: the tank frame's body force instead of gravity (DESIGN.md section 2.15)
+        check(sphk_tank_force(current_.ctx, &current_.abi, dt), "sphk_tank_force");
+        return;
+    }
     const float g[3] = {G.x, G.y, G.z};
     check(sphk_gravity(current_.ctx, &current_.abi, dt, g), "sphk_gravity");
 }
@@ -928,6 +936,90 @@ int SPHSystem::openBoundaryCheck() const {
     return bits;
 }
 
+// ---- tank motion (DESIGN.md section 2.15) ----
+static bool tankMotionAbi(const sphb200::TankMotion& m, sphk_tank_motion& a) {
+    std::memset(&a, 0, sizeof(a));
+    if (m.harmonics.size() > SPHK_TANK_HARMONICS) return false;
+    a.axis[0] = m.axis.x; a.axis[1] = m.axis.y; a.axis[2] = m.axis.z;
+    a.pivot[0] = m.pivot.x; a.pivot[1] = m.pivot.y; a.pivot[2] = m.pivot.z;
+    a.roll_amplitude = m.rollAmplitude; a.roll_omega = m.rollOmega; a.roll_phase = m.rollPhase; a.spin = m.spin;
+    a.accel[0] = m.accel.x; a.accel[1] = m.accel.y; a.accel[2] = m.accel.z;
+    a.n_harmonics = static_cast<int>(m.harmonics.size());
+    for (size_t k = 0; k < m.harmonics.size(); ++k) {
+        const auto& h = m.harmonics[k];
+        a.harmonic_amplitude[k][0] = h.amplitude.x; a.harmonic_amplitude[k][1] = h.amplitude.y; a.harmonic_amplitude[k][2] = h.amplitude.z;
+        a.harmonic_omega[k] = h.omega; a.harmonic_phase[k] = h.phase;
+    }
+    a.ramp = m.ramp;
+    return true;
+}
+
+double SPHSystem::ruleGravity() const {
+    const float g[3] = {_sphG.x, _sphG.y, _sphG.z};
+    if (_tankOn) {
+        const float sp[3] = {_spaceSize.x, _spaceSize.y, _spaceSize.z};
+        double b = 0.0;
+        check(sphk_tank_accel_bound(&_tankAbi, g, sp, &b), "sphk_tank_accel_bound");
+        return b;
+    }
+    return std::sqrt(double(g[0]) * g[0] + double(g[1]) * g[1] + double(g[2]) * g[2]);
+}
+
+bool SPHSystem::setTankMotion(const sphb200::TankMotion& m) {
+    auto* solver = dynamic_cast<BasicSPHSolver*>(_solver.get());
+    if (!_engine->ok() || !solver) {
+        printf("setTankMotion: needs a working engine and one of the shipped solvers; the setting is kept\n");
+        return false;
+    }
+    sphk_tank_motion a;
+    const float g[3] = {_sphG.x, _sphG.y, _sphG.z};
+    float probe[SPHK_TANK_STATE];
+    if (!tankMotionAbi(m, a) || sphk_tank_eval(&a, g, 0.0, probe) != 0) {
+        printf("setTankMotion: need finite values, a non-zero axis, rollOmega, harmonic omegas and ramp >= 0 and at most %d harmonics; "
+               "the setting is kept\n", SPHK_TANK_HARMONICS);
+        return false;
+    }
+    if (solver->thermalOn()) {
+        printf("setTankMotion: not together with heat transfer (the Boussinesq buoyancy acts along the constant G); the setting is "
+               "kept\n");
+        return false;
+    }
+    const bool rotates = a.roll_amplitude != 0.0f || a.spin != 0.0f;
+    if (rotates && _bodiesDynamic) {
+        printf("setTankMotion: a rotating tank is not supported with dynamic bodies; the setting is kept\n");
+        return false;
+    }
+    check(sphk_tank_set(_engine->ctx(), &a, g), "sphk_tank_set");
+    // the motion is a function of the simulated time: the frame time starts where the system is
+    check(sphk_tank_set_time(_engine->ctx(), _simTime), "sphk_tank_set_time");
+    dropStepGraph();                        // the graph holds the motion of its capture
+    _tankOn = true; _tankAbi = a;
+    solver->setTankForce(true);
+    if (_adaptive) _rule.gravity = ruleGravity();
+    return true;
+}
+
+void SPHSystem::clearTankMotion() {
+    if (!_tankOn) return;
+    check(sphk_tank_set(_engine->ctx(), nullptr, nullptr), "sphk_tank_set");
+    dropStepGraph();
+    _tankOn = false;
+    if (auto* solver = dynamic_cast<BasicSPHSolver*>(_solver.get())) solver->setTankForce(false);
+    if (_adaptive) _rule.gravity = ruleGravity();
+}
+
+sphb200::TankState SPHSystem::tankState() const {
+    sphb200::TankState s;
+    s.t = _simTime;
+    const float g[3] = {_sphG.x, _sphG.y, _sphG.z};
+    float e[SPHK_TANK_STATE] = {0, 0, 0, g[0], g[1], g[2], 0, 0, 0};
+    if (_tankOn) check(sphk_tank_eval(&_tankAbi, g, _simTime, e), "sphk_tank_eval");
+    s.theta = e[0]; s.thetaDot = e[1]; s.thetaDDot = e[2];
+    s.gravity = make_float3(e[3], e[4], e[5]);
+    s.accel = make_float3(e[6], e[7], e[8]);
+    return s;
+}
+
 // the end of a step with dynamic bodies (after the solver's last reaction, inside a captured step graph)
 void SPHSystem::integrateBodies() {
     if (!_bodiesDynamic) return;
@@ -1016,7 +1108,7 @@ bool SPHSystem::setAdaptiveTimeStep(float C, float dtMin, float dtMax) {
     r.dt_max = dtMax > 0.0f ? dtMax : _dt;
     r.dt_min = dtMin > 0.0f ? dtMin : static_cast<float>(r.dt_max) / 64.0f;
     r.radius = _sphSmoothingRadius;
-    r.gravity = std::sqrt(double(_sphG.x) * _sphG.x + double(_sphG.y) * _sphG.y + double(_sphG.z) * _sphG.z);
+    r.gravity = ruleGravity();
     float dt = 0.0f;
     int flags = 0;
     // the library's rule validates its own parameters
@@ -1423,6 +1515,7 @@ sphk_state_config SPHSystem::stateConfig() const {
     std::vector<unsigned char> settings;
     if (const auto* solver = dynamic_cast<const BasicSPHSolver*>(_solver.get())) solver->stateConfig(c, settings);
     if (_adaptive) putBytes(settings, _rule);
+    if (_tankOn) putBytes(settings, _tankAbi);
     c.settings_hash = stateHash(settings.data(), settings.size()) + settings.size();
     return c;
 }
@@ -1542,6 +1635,7 @@ bool SPHSystem::restore(const std::string& path, std::vector<unsigned char>* use
     dynamic_cast<BasicSPHSolver*>(_solver.get())->stateRestored();
     // the next adaptive dt: the speed bound of the restored state, measured again (a max over the same bits as the saved run's)
     if (_adaptive) measureSpeed();
+    if (_tankOn) check(sphk_tank_set_time(ctx, _simTime), "sphk_tank_set_time");     // the frame time of the saved run
     check(sphk_synchronize(ctx), "sphk_synchronize");
     _restored = true;
     return true;

@@ -194,6 +194,31 @@ struct ProbeSeries {
     long long overwritten = 0;       // rows recorded but no longer in the ring
 };
 
+// addition: tank motion (DESIGN.md section 2.15; sphk_tank_* in sphk.h).  The simulation runs in the tank's frame; the motion is a
+// function of simulatedTime().  Rotation theta(t) = e (rollAmplitude sin(rollOmega t + rollPhase)) + theta_s about `axis` (fixed in
+// the tank) through `pivot` (tank coordinates), d theta_s / dt = e spin; the pivot's world acceleration a_w = e (accel + sum_k
+// amplitude_k sin(omega_k t + phase_k)); e = min(1, t / ramp) (1 when ramp = 0).
+struct TankHarmonic {
+    float3 amplitude{0.0f, 0.0f, 0.0f};  // world
+    float omega = 0.0f, phase = 0.0f;    // omega >= 0
+};
+struct TankMotion {
+    float3 axis{0.0f, 0.0f, 1.0f};       // any length > 0
+    float3 pivot{0.0f, 0.0f, 0.0f};
+    float rollAmplitude = 0.0f, rollOmega = 0.0f, rollPhase = 0.0f;   // rad, rad/s (>= 0), rad
+    float spin = 0.0f;                   // Omega0, rad/s
+    float3 accel{0.0f, 0.0f, 0.0f};      // a_c, world
+    std::vector<TankHarmonic> harmonics; // at most SPHK_TANK_HARMONICS
+    float ramp = 0.0f;                   // seconds >= 0
+};
+// the motion at t = simulatedTime(): a tank-frame vector u is R^T u in the world, R = Rot(axis, -theta)
+struct TankState {
+    double t = 0.0;
+    float theta = 0.0f, thetaDot = 0.0f, thetaDDot = 0.0f;
+    float3 accel{0.0f, 0.0f, 0.0f};      // a_w, world
+    float3 gravity{0.0f, 0.0f, 0.0f};    // R (G - a_w): the body force of the frame without the rotation terms, tank axes
+};
+
 // addition: scenes from triangle meshes (DESIGN.md section 2.12; sphk_mesh_* in sphk.h).  The functions below run on the legacy
 // default stream, need no SPHSystem, and throw std::runtime_error when the library refuses a mesh or a call fails.
 struct TriangleMesh {
@@ -393,6 +418,10 @@ public:
     bool setAdhesion(const sphb200::Adhesion& a);
     void clearAdhesion();
     bool adhesionOn() const { return adhesionOn_; }
+    // addition: tank motion (DESIGN.md section 2.15): force() applies the tank frame's body force (sphk_tank_force) instead of
+    // gravity.  Set by SPHSystem::setTankMotion, which owns the motion.
+    void setTankForce(bool on) { if (on != tankOn_) ++configEpoch_; tankOn_ = on; }
+    bool tankForceOn() const { return tankOn_; }
     // statistics of the last step's adhesion sweep (zeros before the first); synchronises
     sphb200::AdhesionStats lastAdhesionStats() const;
     // addition: true when step() enqueues the same kernel sequence every call and never synchronises the host.
@@ -512,6 +541,7 @@ private:
     void thermalViscosity(const std::shared_ptr<SPHParticles>& fluids, float rho0, float rhoB, float dt);
     bool adhesionOn_ = false;
     sphk_adhesion_setting adhesionAbi_{};    // the setting as the C-ABI takes it
+    bool tankOn_ = false;
 };
 
 // ---- DFSPHSolver.h:20-64 ----------------------------------------------------------------------
@@ -723,6 +753,14 @@ public:
     // restore are not in the file (drain them before checkpointing); rows recorded after it carry the saved run's step indices and
     // times.  A user-derived solver is refused.
     bool checkpoint(const std::string& path, const std::vector<unsigned char>& user = {});
+    // tank motion (DESIGN.md section 2.15): from the next step on, the fluid (and dynamic bodies) feel the tank frame's body force
+    // instead of G; the motion is part of the checkpoint configuration.  Refused (printed, setting kept, false): out-of-range
+    // values, heat transfer, a rotation with dynamic bodies.  Setting or clearing drops the step graph (it is captured again with
+    // the motion inside it).  While a motion is set, the adaptive rule's |G| is sphk_tank_accel_bound.
+    bool setTankMotion(const sphb200::TankMotion& m);
+    void clearTankMotion();
+    bool tankMotionOn() const { return _tankOn; }
+    sphb200::TankState tankState() const;
     bool waitCheckpoint();
     bool restore(const std::string& path, std::vector<unsigned char>* user = nullptr);
 
@@ -802,6 +840,10 @@ private:
     sphk_state_config stateConfig() const;
     bool stateSections(std::vector<sphk_state_section>& out, int n, StateRecord& rec, std::vector<double>& carry,
                        std::vector<float>& motion, const std::vector<unsigned char>& user);
+    // tank motion
+    bool _tankOn = false;
+    sphk_tank_motion _tankAbi{};          // as the C-ABI takes it (zero-filled: its bytes are hashed into the config record)
+    double ruleGravity() const;           // the adaptive rule's |G|: |G|, or sphk_tank_accel_bound under a motion
 };
 
 // ---- vbo.cu:46-51 --------------------------------------------------------------------------------

@@ -401,6 +401,8 @@ float SlabSPHSystem::step() {
         throw std::runtime_error("SlabSPHSystem: heat transfer is not supported on slab ranks (single-GPU SPHSystem only)");
     if (known && known->adhesionOn())       // the boundary walk and the body reaction are single-context only
         throw std::runtime_error("SlabSPHSystem: adhesion is not supported on slab ranks (single-GPU SPHSystem only)");
+    if (known && known->tankForceOn())      // the frame time and the per-step state live in one context
+        throw std::runtime_error("SlabSPHSystem: tank motion is not supported on slab ranks (single-GPU SPHSystem only)");
     if (adaptive_)
         throw std::runtime_error("SlabSPHSystem: adaptive time stepping is not supported on slab ranks (single-GPU SPHSystem only)");
     cudaStream_t st = engine_->stream();

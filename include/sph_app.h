@@ -146,6 +146,28 @@ int   sph_app_sample_lattice(sph_app* app, const float* origin, float spacing, c
 int   sph_app_checkpoint(sph_app* app, const char* path, const void* user, int user_bytes);
 int   sph_app_checkpoint_wait(sph_app* app);
 int   sph_app_restore(sph_app* app, const char* path, void* user_out, int user_cap, int* user_bytes);
+/* Tank motion (SPHSystem::setTankMotion; DESIGN.md section 2.15): the system runs in the frame of a tank rolled about `axis` through
+ * `pivot` (theta = e roll_amplitude sin(roll_omega t + roll_phase) + spin integrated), shaken (pivot acceleration e (accel + sum_k
+ * harmonic_amplitude[k] sin(harmonic_omega[k] t + harmonic_phase[k])), k < n_harmonics <= 4, in the world) and ramped in over
+ * `ramp` seconds (e = min(1, t / ramp)), t the simulated time.  The layout is sphk_tank_motion's.  NULL: off.  Returns 1 on the
+ * reference build and for a setting the class layer refuses (out-of-range values, heat transfer, a rotation with dynamic bodies;
+ * the setting is then kept). */
+typedef struct sph_app_tank_motion {
+    float axis[3];
+    float pivot[3];
+    float roll_amplitude, roll_omega, roll_phase;
+    float spin;
+    float accel[3];
+    int   n_harmonics;
+    float harmonic_amplitude[4][3];
+    float harmonic_omega[4];
+    float harmonic_phase[4];
+    float ramp;
+} sph_app_tank_motion;
+int   sph_app_set_tank_motion(sph_app* app, const sph_app_tank_motion* motion);
+/* The motion at the simulated time *t (SPHSystem::tankState): state9 = {theta, theta', theta'', a_w.xyz (world), R (G - a_w).xyz
+ * (tank axes)}; G and zeros without a motion.  Either pointer may be NULL; 1 on the reference build. */
+int   sph_app_tank_state(sph_app* app, double* t, float* state9);
 /* Kinematic rigid bodies (SPHSystem's constructor with a vector of sphb200::KinematicBody; DESIGN.md section 2.3).  No
  * reference counterpart: NULL / 1 on the reference build.  Body b is the points body_xyz[body_begin[b] .. body_begin[b+1])
  * (body coordinates; body_begin[0] = 0), pose[7 b ..] = {cx, cy, cz, qx, qy, qz, qw} (quaternion scalar part last),

@@ -476,7 +476,8 @@ int sphk_bodies_set_dynamics(sphk_ctx* ctx, const float* mass_inertia, const flo
 int sphk_bodies_react(sphk_ctx* ctx, const sphk_scene* scene, float c);
 /* End of step: the gathered {J, H} of every body become the reported impulse (sphk_bodies_get_impulse) and are cleared; a
  * dynamic body's motion becomes V += J / M + dt G, Omega = (R diag(I) R^T)^-1 (R diag(I) R^T Omega + H), R from the current
- * pose.  The next sphk_bodies_step moves it.  dt > 0, G finite. */
+ * pose.  The next sphk_bodies_step moves it.  dt > 0, G finite.  While a tank motion is set (sphk_tank_set) G is replaced by the
+ * R (G - a_w) of the last sphk_tank_force. */
 int sphk_bodies_integrate(sphk_ctx* ctx, float dt, const float G[3]);
 /* New motion {V, Omega} of one body (host float[6]), enqueued like sphk_bodies_set_motion; the other bodies keep their
  * device-side motion (the integrated one, for dynamic bodies). */
@@ -751,6 +752,67 @@ int  sphk_state_section_bytes(const sphk_state_file* file, const char* name, uns
 int  sphk_checkpoint_load(sphk_ctx* ctx, const sphk_state_file* file, const sphk_state_config* expect,
                           const sphk_state_section* sections, int n_sections, char* msg, int msg_len);
 int  sphk_checkpoint_invalidate(sphk_ctx* ctx);
+
+/* ---- tank motion (no reference counterpart; DESIGN.md section 2.15) ------------------------------------------------------------
+ * The simulation frame is the tank's own frame: walls, grid, clamp box and every sweep stay where they are, and the tank's motion
+ * enters as a body force.  At t = 0 the tank frame coincides with the world whenever theta(0) = 0.  G is gravity in the world.
+ *   rotation about the unit axis n (fixed in the tank) through the pivot p (tank coordinates):
+ *     theta(t) = e(t) Theta sin(w t + phi) + theta_s(t),   d theta_s / dt = e(t) Omega0,  theta_s(0) = 0
+ *   translation, as the world acceleration of the pivot:
+ *     a_w(t) = e(t) (a_c + sum_k A_k sin(w_k t + phi_k)),   k < n_harmonics <= SPHK_TANK_HARMONICS
+ *   ramp: e(t) = min(1, t / T_r) (e = 1 when T_r = 0).  With s = sin(w t + phi), c = cos(w t + phi) and, before the ramp's end
+ *   (t < T_r), e = t / T_r and e' = 1 / T_r, after it e = 1 and e' = 0:
+ *     theta_s = Omega0 t^2 / (2 T_r)                       (t < T_r)
+ *             = Omega0 (t - T_r / 2)                       (t >= T_r; Omega0 t when T_r = 0)
+ *     thd  = e' Theta s + e Theta w c + e Omega0
+ *     thdd = 2 e' Theta w c - e Theta w^2 s + e' Omega0
+ * With Omega = thd n, R = Rot(n, -theta) (world vectors in tank axes) and r = x - p, one step of a fluid particle, every quantity
+ * at t_n (the start of the step):
+ *     v <- Rot(n, -2 thd dt) v + dt (R (G - a_w) - thdd n x r - thd^2 n x (n x r))
+ * (Coriolis as an exact rotation of v: it never changes |v|; Euler; centrifugal).  It replaces the gravity kick sphk_gravity.
+ * Refused by sphk_tank_set and sphk_tank_eval with SPHK_ERR_INVALID: a NULL pointer (motion NULL is a clear for sphk_tank_set), a
+ * non-finite value in the fields in use, |n| = 0, w, w_k or T_r < 0, n_harmonics outside [0, SPHK_TANK_HARMONICS]. */
+#define SPHK_TANK_HARMONICS 4
+#define SPHK_TANK_STATE 9                   /* theta, thd, thdd, R (G - a_w) (3), a_w (3) */
+typedef struct sphk_tank_motion {
+    float axis[3];                          /* n, any length > 0 (normalised in double) */
+    float pivot[3];                         /* p, tank coordinates */
+    float roll_amplitude;                   /* Theta (rad) */
+    float roll_omega;                       /* w >= 0 (rad/s) */
+    float roll_phase;                       /* phi (rad) */
+    float spin;                             /* Omega0 (rad/s) */
+    float accel[3];                         /* a_c, world */
+    int   n_harmonics;                      /* entries of the three arrays below in use; the rest are ignored */
+    float harmonic_amplitude[SPHK_TANK_HARMONICS][3];   /* A_k, world */
+    float harmonic_omega[SPHK_TANK_HARMONICS];          /* w_k >= 0 */
+    float harmonic_phase[SPHK_TANK_HARMONICS];          /* phi_k */
+    float ramp;                             /* T_r >= 0 */
+} sphk_tank_motion;
+/* Host only, no context: {theta, thd, thdd, R (G - a_w), a_w} at t >= 0, computed in double and rounded to float once -- the one
+ * place the schedule is written down.  SPHK_ERR_INVALID also for t < 0 or not finite. */
+int sphk_tank_eval(const sphk_tank_motion* motion, const float G[3], double t, float out[SPHK_TANK_STATE]);
+/* Host only: a bound on the body force per unit mass over all t,
+ *   |G| + |a_c| + sum_k |A_k| + r_max (|Theta| w^2 + (2 |Theta| w + |Omega0|) / T_r + (|Theta| w + |Theta| / T_r + |Omega0|)^2)
+ * (the 1 / T_r terms 0 when T_r = 0), r_max = the distance from p to the farthest corner of the clamp box [0, 0.99 space].  It
+ * bounds |G - a_w| + |r|_max (|thdd| + thd^2); Coriolis adds no speed.  The |G| of the adaptive step rule while a motion is set. */
+int sphk_tank_accel_bound(const sphk_tank_motion* motion, const float G[3], const float space[3], double* bound_out);
+/* Sets (NULL: clears) the context's motion; the frame time is kept (0 at the first setting).  Refusals change nothing:
+ * SPHK_ERR_INVALID as above; SPHK_ERR_STATE under an active range (slab ranks) and for a rotation (Theta != 0 or Omega0 != 0) when
+ * dynamic bodies are declared (a rigid body's angular equation in a rotating frame is not modelled; sphk_bodies_set_dynamics refuses
+ * M > 0 under a rotating motion in turn).  The motion is passed to the kernels by value: a captured step graph must be captured again. */
+int sphk_tank_set(sphk_ctx* ctx, const sphk_tank_motion* motion, const float G[3]);
+/* The step's body force on the live fluid: one single-thread kernel evaluates the schedule in double at the device-resident frame
+ * time t_n into the per-step state {Rot(n, -2 thd dt), dt R (G - a_w), thdd dt, thd^2 dt} and advances the frame time by (double)
+ * dt (in the stream: a replayed step graph advances it too); one kernel per fluid particle applies the update above to the API
+ * velocities and the records.  When the step's thd and thdd are both 0 the particle kernel does exactly sphk_gravity's arithmetic
+ * with dt R (G - a_w) as its dt G (zero amplitudes give sphk_gravity's bits).  While a motion is set, sphk_bodies_integrate uses
+ * R (G - a_w) of the last sphk_tank_force instead of its G.  SPHK_ERR_STATE without a motion; dt >= 0 and finite. */
+int sphk_tank_force(sphk_ctx* ctx, const sphk_scene* scene, float dt);
+/* The frame time (synchronises) and, when state_or_null is given, the state of the last sphk_tank_force as sphk_tank_eval gives it
+ * (float[SPHK_TANK_STATE], zeros before the first); sphk_tank_set_time enqueues a new frame time (t >= 0, finite: a restore).
+ * SPHK_ERR_STATE before the first sphk_tank_set. */
+int sphk_tank_time(sphk_ctx* ctx, double* t, float* state_or_null);
+int sphk_tank_set_time(sphk_ctx* ctx, double t);
 
 /* ---- render export: generate_dots_CUDA, vbo.cu:26-44 (SURVEY 8f-2) -----------------------------------------------
  * dot[i] = pos[i]; colour[i] from density[i] (blue below 0.75, blend to white at 1.0, blend to pink above).  Plain
